@@ -1,12 +1,16 @@
 #!/usr/bin/env python
 """Benchmark of the embed+detect hot path (BASELINE.json metric: embed+detect frames/s).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--card C] [--batch B] [--size S]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--card C] [--batch B] [--size S] [--dump-outputs DIR]
 
 One "step" = model.embed(batch, msgs, is_video=False) followed by model.detect(imgs_w, is_video=False) on one batch of
 synthetic frames (configs[1] of BASELINE.json by default: videoseal_1.0, 256-bit, 64 x 3x256x256 per GPU).  Under torchrun
 every rank processes its own batch (frames are independent units: weak scaling, no data-path collective except the
 all-gather of the [B, 1+K] logits that reassembles the detection output).  Prints ONE JSON line on rank 0.
+
+--dump-outputs DIR writes what rank 0's last timed step returned on rank 0 (its own frames, not the all-gathered logits), as float32 .npy files: imgs_w.npy (the watermarked frames;
+a fixed, seeded sample of frames when they exceed 48 MB, their indices in imgs_w_frames.npy) and preds.npy ([B, 1+K] logits).
+The inputs depend only on the arguments, so two builds can be compared output for output.
 
 --impl reference times the CPU restatement of the reference path (oracle/restate.py, pinned bit-exact to the reference
 modules) on the host cores; the unmodified reference itself needs packages that are not installed here (DESIGN.md).
@@ -14,7 +18,6 @@ modules) on the host cores; the unmodified reference itself needs packages that 
 import argparse
 import json
 import os
-import re
 import subprocess
 import sys
 import threading
@@ -44,11 +47,16 @@ def parse_args():
     ap.add_argument("--clip-frames", type=int, default=512)
     ap.add_argument("--no-hbm-leg", action="store_true", help="skip the 768x768 leg that measures the HBM-bound kernels")
     ap.add_argument("--profile-out", default="", help="write the per-kernel table (JSON) here")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the outputs of rank 0's last timed step here (.npy): its own imgs_w and preds, not the all-gathered logits")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    return args
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -141,21 +149,14 @@ def pointwise_bytes(name: str, S: int = 256) -> float:
     return 0.0
 
 
-def ncu_traffic(tag: str):
-    """per-launch dram__bytes_read+write of a kernel from the committed ncu summaries (profiles/ncu_traffic.json), or None"""
-    p = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(p):
-        return json.load(open(p)).get(tag)
-    return None
-
-
 def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "tf_burst": d["bf16_tflops"], "tf_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "src": "measured"}
-    return {"hbm_gbs": 6650.0, "tf_burst": 1590.0, "tf_sustained": 1400.0, "src": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W): HBM3 bandwidth and dense FP16 tensor rate; denominators only, never reached figures
+    return {"hbm_gbs": 3350.0, "tf_burst": 989.0, "tf_sustained": 989.0, "src": "H100 SXM data sheet"}
 
 
 def build_card_on_disk(card_name: str, seed: int = 0):
@@ -342,6 +343,22 @@ def clip_leg(model, dev, world: int, rank: int, frames: int, size: int, steps: i
     return res
 
 
+def dump_outputs(d: str, imgs_w, preds, limit: int = 48 << 20, seed: int = 0):
+    """imgs_w [B,3,H,W] and preds [B,1+K] -> DIR/*.npy in float32; frames beyond `limit` bytes are replaced by a seeded sample"""
+    import numpy as np
+    import torch
+    os.makedirs(d, exist_ok=True)
+    x = imgs_w.detach().float().cpu()
+    per = x[0].numel() * 4
+    if x.shape[0] * per > limit:
+        n = max(1, limit // per)
+        idx = torch.randperm(x.shape[0], generator=torch.Generator().manual_seed(seed))[:n].sort().values
+        x = x[idx]
+        np.save(os.path.join(d, "imgs_w_frames.npy"), idx.numpy().astype(np.float32))
+    np.save(os.path.join(d, "imgs_w.npy"), x.numpy().astype(np.float32))
+    np.save(os.path.join(d, "preds.npy"), preds.detach().float().cpu().numpy().astype(np.float32))
+
+
 def run_reference(args):
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
@@ -372,7 +389,7 @@ def run_ours(args):
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py (impl=ours) needs a B200; there is no CPU fallback")
+        raise SystemExit("bench.py (impl=ours) needs an H100; there is no CPU fallback")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     # stdout must carry exactly ONE JSON line: libraries (e.g. the NCCL version banner) write to fd 1 directly, so
@@ -392,7 +409,7 @@ def run_ours(args):
     with contextlib.redirect_stdout(io.StringIO()):
         model = videoseal_b200.load(Path(cpath)).eval().to(dev)
     B, S, K = args.batch, args.size, model.spec["nbits"]
-    NB = 4  # rotating input batches: NB * B*3*S*S*4 bytes (201 MB at the default shape) > 126 MB L2
+    NB = 4  # rotating input batches: NB * B*3*S*S*4 bytes (201 MB at the default shape) > 50 MB L2
     g = torch.Generator().manual_seed(1000 + rank)
     imgs = [torch.rand(B, 3, S, S, generator=g).to(dev) for _ in range(NB)]
     msgs = torch.randint(0, 2, (B, K), generator=g).to(dev)
@@ -402,9 +419,13 @@ def run_ours(args):
     msgs_v = msgs[:1]
     n_keys = (B + model.step_size - 1) // model.step_size if vid else B   # frames that go through the U-Net per step
 
+    last = {}
+
     def step_local(i):
         out = model.embed(imgs[i % NB], msgs_v if vid else msgs, is_video=vid)
-        return model.detect(out["imgs_w"], is_video=vid)["preds"]
+        preds = model.detect(out["imgs_w"], is_video=vid)["preds"]
+        last["imgs_w"], last["preds"] = out["imgs_w"], preds
+        return preds
 
     def step(i):
         preds = step_local(i)
@@ -441,6 +462,8 @@ def run_ours(args):
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         ms = t.item()
     fps = world * B * args.steps / (ms / 1000.0)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["imgs_w"], last["preds"])
 
     # ---- end-to-end through the C ABI with HOST buffers (pinned): H2D + embed + D2H, H2D + detect + D2H, every step
     e2e = None
@@ -528,19 +551,13 @@ def run_ours(args):
         peaks = load_peaks()
         dom = next((r for r in table if r["tflops"]), None)
         if dom:
-            # the kernel is event-timed launch by launch at full clock (clocks line: 1965 MHz, no power cap inside these 3 steps),
-            # so the denominator is the BURST cuBLAS figure; the sustained one is reported next to it
-            # finalize_op (conv_gemm_host.cuh) sends 3x3 TMA convs with >= 24 K blocks (C_in >= 192) on whole-row tiles to the CTA-pair kernel
-            mm = re.match(r"unet\.conv3x3\.(\d+)-", dom["name"])
-            pair = bool(mm) and int(mm.group(1)) >= 192 and not os.environ.get("VSB_NO_PAIR")
-            roofline = {"bound": "tensor", "kernel": ("conv_pair_kernel (tcgen05 cta_group::2) " if pair else "conv_gemm_kernel<LD_TMA> ") + dom["name"],
+            # the kernel is event-timed launch by launch, so the denominator is the burst figure; the sustained one is reported next to it
+            roofline = {"bound": "tensor", "kernel": "conv_gemm_kernel " + dom["name"],
                         "achieved": dom["tflops"],
                         "peak": peaks["tf_burst"], "unit": "TFLOP/s", "frac": dom["tflops"] / peaks["tf_burst"],
-                        "peak_source": peaks["src"] + " bf16 cuBLAS, burst (kernel event-timed per launch at full clock)",
+                        "peak_source": peaks["src"] + ", burst (kernel event-timed per launch)",
                         "frac_of_sustained_peak": dom["tflops"] / peaks["tf_sustained"],
                         "share_of_step": dom["share"], "avg_launch_us": dom["avg_us"],
-                        "traffic": ncu_traffic(f"{args.card}:{dom['name']}@b{B}"),
-                        "traffic_source": "dram__bytes_read+write per launch from the committed ncu --set full capture (profiles/ncu_traffic.json)",
                         "step_ms_under_events": tot}
         if args.profile_out:
             json.dump({"batch": B, "card": args.card, "table": table}, open(args.profile_out, "w"), indent=1)
@@ -551,7 +568,7 @@ def run_ours(args):
     roofline_hbm = None
     if rank == 0 and not args.no_hbm_leg:
         HS, HB = (768, 32) if S != 768 else (S, B)
-        gi = [torch.rand(HB, 3, HS, HS, generator=g).to(dev) for _ in range(2)]     # 2 x 226 MB > 126 MB L2
+        gi = [torch.rand(HB, 3, HS, HS, generator=g).to(dev) for _ in range(2)]     # 2 x 226 MB > 50 MB L2
         hm = msgs[:HB] if not vid else msgs_v
 
         def hbm_step(i):
@@ -580,16 +597,14 @@ def run_ours(args):
             by = pointwise_bytes(name, model.spec["img_size"])
             gbs = by / (tms / cnt * 1e-3) / 1e9 if by else None
             rows.append({"name": name, "avg_us": 1000 * tms / cnt, "launches_per_step": cnt // 3, "algorithmic_bytes": by,
-                         "gbs": gbs, "frac": gbs / peaks["hbm_gbs"] if gbs else None,
-                         "traffic": ncu_traffic(f"{args.card}:{name}")})
+                         "gbs": gbs, "frac": gbs / peaks["hbm_gbs"] if gbs else None})
             tot_b += by * cnt / 3
             tot_ms += tms / 3
         rows.sort(key=lambda r: -r["avg_us"] * r["launches_per_step"])
         if rows:
             top = rows[0]
             roofline_hbm = {"bound": "hbm", "kernel": top["name"], "achieved": top["gbs"], "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                            "frac": top["frac"], "peak_source": peaks["src"] + " copy bandwidth",
-                            "traffic": ncu_traffic(f"{args.card}:{top['name']}"),
+                            "frac": top["frac"], "peak_source": peaks["src"] + " HBM bandwidth",
                             "workload": f"{args.card} embed+detect, {'video' if vid else 'image'} mode, {HB} x 3x{HS}x{HS}",
                             "stage_gbs": tot_b / (tot_ms * 1e-3) / 1e9 if tot_ms else None,
                             "stage_frac": (tot_b / (tot_ms * 1e-3) / 1e9 / peaks["hbm_gbs"]) if tot_ms else None,
@@ -616,7 +631,7 @@ def run_ours(args):
             "config": {"workload": f"{args.card} {K}-bit embed+detect, {'video (step ' + str(model.step_size) + ')' if vid else 'image'} mode, "
                                    f"batch {B} x 3x{S}x{S} per GPU" + (" (BASELINE configs[1])" if (B, S, vid, args.card) == (64, 256, False, "videoseal_1.0") else ""),
                        "card": args.card, "batch_per_gpu": B, "size": S, "parallelism": f"dp{world} (frames sharded, weak scaling)",
-                       "l2": f"{NB} rotating input batches ({NB * B * 3 * S * S * 4 / 1e6:.0f} MB > 126 MB L2); activations per step >> L2"},
+                       "l2": f"{NB} rotating input batches ({NB * B * 3 * S * S * 4 / 1e6:.0f} MB > 50 MB L2); activations per step >> L2"},
             "step_tflops": (fe * n_keys + fd * B) * world * args.steps / (ms / 1000.0) / 1e12,
             "clocks": clocks, "e2e": e2e, "gpu_launches": launches, "roofline": roofline, "roofline_hbm": roofline_hbm, "clip": clip, "cpu_baseline": cpu,
             "top_kernels": [{k: (round(v, 4) if isinstance(v, float) else v) for k, v in r.items()} for r in table[:8]],

@@ -1,9 +1,9 @@
-/* libvsb200.so — C ABI of the B200-native VideoSeal embed/detect hot path.
+/* libvsb200.so — C ABI of the H100-native (sm_90a) VideoSeal embed/detect hot path.
  *
  * Plain pointers and sizes only (no torch types).  All `*_dev` pointers are CUDA device pointers on the
  * device the model was finalised on; `stream` is a cudaStream_t passed as void*.  Every entry point returns
  * 0 on success or a negative vsb_status; vsb_last_error() gives the message.  There is NO CPU fallback:
- * without an sm_100 GPU vsb_model_finalize() fails.
+ * on any device other than compute capability 9.0 (H100) vsb_model_finalize() fails.
  *
  * Each entry point names the reference interface it replaces (paths relative to facebookresearch/videoseal):
  *   vsb_model_create / set_tensor / finalize  <-  videoseal/utils/cfg.py:88-149 setup_model (build_embedder
@@ -133,7 +133,7 @@ int64_t vsb_profile_read(char* buf, int64_t capacity);
 /* copy a named intermediate activation of the most recent embed/detect sub-batch to the host as fp32.
  * shape4 receives [B, H, W, C] (NHWC) or [M, C, 1, 1]-style dims; returns the element count or <0. */
 int64_t vsb_debug_get_tensor(vsb_model* m, const char* name, float* host_out, int64_t capacity, int64_t* shape4);
-/* standalone conv/GEMM on the tcgen05 kernel for unit tests: see tests/test_conv_gemm_gpu.py */
+/* standalone conv/GEMM on the wgmma kernels for unit tests: see tests/test_conv_gemm_gpu.py */
 typedef struct vsb_conv_test {
   int32_t loader;            /* 0 TMA per tap, 1 gather conv, 2 halo bilinear-x2+reflect (UBlock), 3 gather GRN-scale, 4 halo conv3x3 */
   int32_t B, IH, IW, C0, C1; /* input NHWC fp16 [B,IH,IW,C0] (+ optional second source [.., C1]) */

@@ -1,4 +1,4 @@
-"""Unit cases for the tcgen05 conv/GEMM kernel (vsb_debug_conv) against a plain PyTorch fp32 reference of the same op
+"""Unit cases for the wgmma conv/GEMM kernels (vsb_debug_conv) against a plain PyTorch fp32 reference of the same op
 computed from the same fp16-rounded operands.  Used by tests/test_conv_gemm_gpu.py and tests/gpu_diag.py."""
 import ctypes as C
 import math

@@ -57,7 +57,7 @@ def test_unknown_preset_is_rejected_at_load_time():
 
 
 def test_videoseal_0_0_card_is_rejected_by_the_product_loader():
-    """configs[0] runs on the reference's CPU path only (oracle); the B200 package has no ViT extractor and no CPU fallback"""
+    """configs[0] runs on the reference's CPU path only (oracle); the CUDA package has no ViT extractor and no CPU fallback"""
     with pytest.raises(NotImplementedError):
         vcfg.spec_from_card(load_card("videoseal_0.0"))
 

@@ -82,6 +82,7 @@ def test_oracle_video_modes_lowres_and_aggregations_match_reference_golden(card)
     spec = restate.spec_from_card(load_card(card))
     orc = restate.OracleModel(spec, restate.synth_state_dict(spec, seed=gold["seed"]))
     c = gold["cases"]["vid_modes"]
+    st = c["sample_stride"]
     g = torch.Generator().manual_seed(c["gen_seed"])
     vid = torch.rand(c["F"], 3, c["H"], c["W"], generator=g)
     msgs = torch.randint(0, 2, (1, spec["nbits"]), generator=g)
@@ -91,13 +92,13 @@ def test_oracle_video_modes_lowres_and_aggregations_match_reference_golden(card)
             mode, lowres = key.split("/")
             orc.video_mode = mode
             o = orc.embed(vid, msgs, is_video=True, lowres_attenuation=bool(int(lowres)))
-            assert (_sample(o["imgs_w"]) - ref["imgs_w_s"]).abs().max() < 1e-5, key
+            assert (_sample(o["imgs_w"], st) - ref["imgs_w_s"]).abs().max() < 1e-5, key
             assert abs(o["imgs_w"].double().mean().item() - ref["imgs_w_stats"]["mean"]) < 1e-6, key
         orc.video_mode = "repeat"
         nointerp = {"mode": "bilinear", "align_corners": False, "antialias": False}
         o = orc.embed(vid[:2], msgs.repeat(2, 1), is_video=False, lowres_attenuation=True, interpolation=nointerp)
-        assert (_sample(o["imgs_w"]) - c["img_lowres_noaa"]["imgs_w_s"]).abs().max() < 1e-5
-        assert (_sample(o["preds_w"]) - c["img_lowres_noaa"]["preds_w_s"]).abs().max() < 1e-5
+        assert (_sample(o["imgs_w"], st) - c["img_lowres_noaa"]["imgs_w_s"]).abs().max() < 1e-5
+        assert (_sample(o["preds_w"], st) - c["img_lowres_noaa"]["preds_w_s"]).abs().max() < 1e-5
         o = orc.embed(vid, msgs, is_video=True)
         for agg, ref in c["aggregations"].items():
             assert (orc.extract_message(o["imgs_w"], aggregation=agg) == ref).all(), agg

@@ -1,4 +1,4 @@
-"""videoseal_b200: B200-native (sm_100a) implementation of VideoSeal's embed/detect hot path behind the
+"""videoseal_b200: H100-native (sm_90a) implementation of VideoSeal's embed/detect hot path behind the
 reference's `videoseal.load() / model.embed() / model.detect()` API (videoseal/__init__.py:13-17)."""
 
 __version__ = "0.1"

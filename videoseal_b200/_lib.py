@@ -6,7 +6,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# VSB200_LIB selects another build of the same sources (e.g. the experimental -DVSB_PDL variant, see __graft_entry__.py)
+# VSB200_LIB selects another build of the same sources (e.g. one without -DVSB_PDL, see __graft_entry__.py)
 LIB_PATH = os.environ.get("VSB200_LIB") or os.path.join(_HERE, "libvsb200.so")
 
 EXPORTS = [
@@ -55,7 +55,7 @@ def lib():
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a).  videoseal_b200 has no CPU / PyTorch fallback.")
+            "(nvcc, sm_90a).  videoseal_b200 has no CPU / PyTorch fallback.")
     L = C.CDLL(LIB_PATH)
     L.vsb_last_error.restype = C.c_char_p
     L.vsb_version.restype = C.c_int

@@ -70,9 +70,9 @@ def spec_from_card(card: dict) -> dict:
     emb_name = str(card["embedder"]["model"])
     ext_name = str(card["extractor"]["model"])
     if not emb_name.startswith("unet"):
-        raise NotImplementedError(f"embedder '{emb_name}': only the unet* family is on the B200 hot path")
+        raise NotImplementedError(f"embedder '{emb_name}': only the unet* family is on the CUDA hot path")
     if not ext_name.startswith("convnext"):
-        raise NotImplementedError(f"extractor '{ext_name}': only the convnext* family is on the B200 hot path")
+        raise NotImplementedError(f"extractor '{ext_name}': only the convnext* family is on the CUDA hot path")
     u = card["embedder"]["params"]["unet"]
     mp = card["embedder"]["params"].get("msg_processor", {})
     if mp.get("msg_processor_type", "binary+concat") != "binary+concat":
@@ -161,7 +161,7 @@ def get_config_from_checkpoint(ckpt_path) -> dict:
     ext_model = args.get("extractor_model") or ext_cfg["model"]
     for name, cfg_, kind in ((emb_model, emb_cfg, "embedder"), (ext_model, ext_cfg, "extractor")):
         if name not in cfg_:
-            raise NotImplementedError(f"{kind} preset '{name}' is not on the B200 hot path (known: "
+            raise NotImplementedError(f"{kind} preset '{name}' is not on the CUDA hot path (known: "
                                       f"{', '.join(k for k in cfg_ if k != 'model')})")
     return {"checkpoint_path": str(ckpt_path), "args": args,
             "embedder": {"model": emb_model, "params": emb_cfg[emb_model]},
@@ -172,7 +172,7 @@ def setup_model_from_checkpoint(ckpt_path) -> "Videoseal":
     """utils/cfg.py:156-178 of the reference: a model-card name, or the path of a raw training checkpoint (.pth)."""
     ckpt_path = str(ckpt_path)
     if "baseline" in ckpt_path:
-        raise NotImplementedError("baseline watermarkers (videoseal/models/baselines.py) are outside the B200 hot path")
+        raise NotImplementedError("baseline watermarkers (videoseal/models/baselines.py) are outside the CUDA hot path")
     if not ckpt_path.endswith(".pth") and "/" not in ckpt_path:
         return setup_model_from_model_card(ckpt_path)
     return setup_model(get_config_from_checkpoint(ckpt_path), ckpt_path)

@@ -5,16 +5,16 @@
 // (rw >= W + 2, multiple of 8):   P = (b*(H+2) + yy)*rw + xx,  yy = y+1, xx = x+1.   Number the outputs on the same grid,
 // Q = (b*(H+2) + y)*rw + x.  Then tap (r, s) of output Q reads input P = Q + r*rw + s: a pure shift, the same for every
 // output.  Shared memory holds a ring of padded input rows, split in PLANES of 8 channels (16 bytes per position), which
-// is exactly the UMMA no-swizzle K-major canonical layout: 8 consecutive positions x 16 B form one core matrix,
+// is exactly the wgmma no-swizzle K-major canonical layout: 8 consecutive positions x 16 B form one core matrix,
 // SBO = 128 B to the next 8 positions, LBO = plane stride to the next 8 channels.  A tile of 128 consecutive outputs
-// therefore needs, per tap and 16 input channels, ONE tcgen05.mma whose A descriptor simply points at
-// ring + (Q0 + r*rw + s)*16 B.  The input crosses L2->SM once (16-byte cp.async per position and plane, zero fill = the
+// therefore needs, per tap and 16 input channels, two m64 wgmma whose A descriptors simply point at
+// ring + (Q0 + 64h + r*rw + s)*16 B.  The input crosses L2->SM once (16-byte cp.async per position and plane, zero fill = the
 // conv padding, also between images), nothing is copied inside shared memory, and the 2/(H+2) + (rw-W)/rw junk outputs
 // (pad rows / pad columns) are computed and dropped in the epilogue.
 //
-// Roles: warps 0, 2 = row producers, warps 1, 3 = MMA issuers (alternate tiles), warp 2 also allocates TMEM, warps 4.. = epilogue sets (4 warps per
-// set, one TMEM lane quadrant each; a set owns every kD3EpiSets-th tile).  Weights (<= 72 KB) stay resident in shared
-// memory in the same core-matrix layout.  Epilogue: + folded-BN bias, ReLU, + residual, fp16 NHWC store, optionally the
+// Roles: warps 0, 2 = row producers, warps 4.. = MMA + epilogue sets (one warpgroup each; a set owns every kD3EpiSets-th
+// tile, issues its wgmma and runs its epilogue, so the sets overlap each other's MMAs and epilogues).  Weights (<= 72 KB)
+// stay resident in shared memory in the same core-matrix layout.  Epilogue: + folded-BN bias, ReLU, + residual, fp16 NHWC store, optionally the
 // fused 1x1 `outc` + tanh of the last block (unet.py:191-197).
 #pragma once
 #include <cuda_fp16.h>
@@ -25,21 +25,20 @@ namespace vsb {
 
 constexpr int kD3MaxRing = 32;    // row_full barriers (ring rows)
 constexpr int kD3TileBars = 64;   // tile_done barrier ring
-constexpr int kD3MaxAcc = 8;      // TMEM accumulator stages
 constexpr int kD3EpiSets = 3;
 constexpr int kD3Threads = 128 + kD3EpiSets * 128;
-constexpr int kD3HeaderBytes = 2048;
+constexpr int kD3XposeOff = 2048;     // per epilogue warp: [32 rows][kD3XposePitch] fp32 fragment -> row transpose buffer
+constexpr int kD3XposePitch = 20;     // 16 columns + 4: conflict-free float4 row reads
+constexpr int kD3HeaderBytes = kD3XposeOff + kD3EpiSets * 4 * 32 * kD3XposePitch * 4;
 
 struct Conv3DirectParams {
   int B, H, W, C, N, R;     // R = 3 (3x3, zero pad 1) or 1 (1x1)
   int rw, hp;               // linear row pitch in positions (>= W + R - 1, multiple of 8); H + R - 1
   int n_tiles;              // ceil(B*hp*rw / 128)
   int ring_rows, mirror_rows;
-  int acc_stages, tmem_cols;
   uint32_t plane_stride;    // bytes between 8-channel planes of the ring
   uint32_t w_off, ring_off; // offsets from the 1024-aligned dynamic smem base
   uint32_t w_bytes;
-  uint32_t idesc;
   int swap_lbo_sbo;         // debugging aid (unit test of the descriptor convention)
   FastDiv fd_rw, fd_hp;
   const __half* x;          // input, dense NHWC fp16
@@ -58,19 +57,15 @@ struct Conv3DirectParams {
 struct D3Header {
   uint64_t row_full[kD3MaxRing];
   uint64_t tile_done[kD3TileBars];
-  uint64_t acc_full[kD3MaxAcc];
-  uint64_t acc_empty[kD3MaxAcc];
-  uint32_t tmem_base; uint32_t pad_[3];
   float bias[64];
   float ocw[3][64];
 };
-static_assert(sizeof(D3Header) <= kD3HeaderBytes, "direct conv header");
+static_assert(sizeof(D3Header) <= kD3XposeOff, "direct conv header");
 
 // no-swizzle K-major operand: core matrices of 8 rows x 16 B; LBO = byte distance between the two core matrices along K,
 // SBO = byte distance between consecutive 8-row groups
 __device__ __forceinline__ uint64_t make_smem_desc_ns(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo >> 4) & 0x3FFF) << 32) |
-         (1ull << 46);
+  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo >> 4) & 0x3FFF) << 32);
 }
 
 // [N][T*C] (k = tap*C + c, T = 9 or 1 taps) fp16  ->  [tap][C/16][k-half][N/8][8 rows][8 halves]
@@ -109,11 +104,9 @@ __global__ void __launch_bounds__(kD3Threads, 1) conv3_direct_kernel(const Conv3
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < kD3MaxRing; ++i) mbar_init(&hd->row_full[i], 32);   // 32 cp.async arrivals (one producer warp per row)
-    for (int i = 0; i < kD3TileBars; ++i) mbar_init(&hd->tile_done[i], 1);
-    for (int i = 0; i < kD3MaxAcc; ++i) { mbar_init(&hd->acc_full[i], 1); mbar_init(&hd->acc_empty[i], 4); }
+    for (int i = 0; i < kD3TileBars; ++i) mbar_init(&hd->tile_done[i], 4);   // the 4 warps of the set that computed the tile
     fence_barrier_init();
   }
-  if (warp == 2) { tmem_alloc(&hd->tmem_base, (uint32_t)p.tmem_cols); tmem_relinquish(); }
   {
     const uint4* src = reinterpret_cast<const uint4*>(p.wpk);
     uint4* dst = reinterpret_cast<uint4*>(wsm);
@@ -124,20 +117,17 @@ __global__ void __launch_bounds__(kD3Threads, 1) conv3_direct_kernel(const Conv3
       if (UP && threadIdx.x < 16) { hd->ocw[0][threadIdx.x] = __ldg(p.ln_w + threadIdx.x); hd->ocw[1][threadIdx.x] = __ldg(p.ln_b + threadIdx.x); }
     }
   }
-  fence_proxy_async_smem();   // weights were written through the generic proxy, tcgen05.mma reads them through the async proxy
-  tc_fence_before();
+  fence_proxy_async_smem();   // weights were written through the generic proxy, wgmma reads them through the async proxy
   __syncthreads();
-  tc_fence_after();
   // (PDL builds) so far only weights / bias / LN parameters were read: the resident-weight copy overlaps the predecessor's tail
   pdl_launch_dependents();
   pdl_wait();
-  const uint32_t tmem_base = hd->tmem_base;
 
   if (warp == 0 || warp == 2) {
     // ================================================================= producers (warps 0 and 2): one padded input row per
     // ring slot, 16-byte cp.async per (position, plane) with zero fill for the padding.  (A TMA box with a 16-byte inner
     // extent does the same split, but every 16-byte line is its own request and the TMA unit's request window, not
-    // bandwidth, then bounds the kernel: measured 20 G lines/s chip-wide, profiles/r1_history.md.)
+    // bandwidth, then bounds the kernel.)
     const int pw = warp >> 1;
     const int planes = p.C >> 3, pshift = planes == 2 ? 1 : (planes == 4 ? 2 : 3);
     int tiles_conf = 0;
@@ -203,73 +193,36 @@ __global__ void __launch_bounds__(kD3Threads, 1) conv3_direct_kernel(const Conv3
       }
       cp_async_mbar_arrive_noinc(&hd->row_full[slot]);
     }
-  } else if (warp == 1 || warp == 3) {
-    // ================================================================= MMA issuers (two warps, alternate tiles)
-    // One thread issues everything, so its scalar instruction stream IS the pace of the kernel for these tiny MMAs (first
-    // version: ~3400 cycles per tile in integer divisions and descriptor assembly, 10x the tensor work).  Everything
-    // is therefore strength-reduced: positions advance incrementally, the 64-bit descriptors differ only in the
-    // 14-bit address field (one position = 16 B = one unit of addr>>4), and the 9*KS MMAs are fully unrolled.
-    if (lane == 0) {
-      const uint32_t a_lbo = p.swap_lbo_sbo ? 128u : p.plane_stride, a_sbo = p.swap_lbo_sbo ? p.plane_stride : 128u;
-      const uint32_t b_lbo = p.swap_lbo_sbo ? 128u : (uint32_t)N * 16u, b_sbo = p.swap_lbo_sbo ? (uint32_t)N * 16u : 128u;
-      const uint32_t a_lo = (((a_lbo >> 4) & 0x3FFFu) << 16) + (smem_u32(ring) >> 4);
-      const uint32_t b_lo = (((b_lbo >> 4) & 0x3FFFu) << 16) + (smem_u32(wsm) >> 4);
-      const uint64_t a_hi = (uint64_t)(((a_sbo >> 4) & 0x3FFFu) | (1u << 14)) << 32;
-      const uint64_t b_hi = (uint64_t)(((b_sbo >> 4) & 0x3FFFu) | (1u << 14)) << 32;
-      const uint32_t kk_step = (2u * p.plane_stride) >> 4;
-      const int rows_total = row_hi - row_lo;
-      int x0 = 128 * t0 - row_lo * rw, slot0 = 0;          // first output position of the tile: (ring slot, column)
-      int xn = x0 + 127 + (R - 1), gn = 0;                  // last input position of tap (0, R-1): row (relative), column
-      while (xn >= rw) { xn -= rw; ++gn; }
-      int rows_conf = 0, rslot = 0;
-      uint32_t rpar = 0;
-      const int mw = warp >> 1;   // 0 / 1: this issuer takes tiles mw, mw + 2, ...
-      for (int i = 0; i < nt; ++i) {
-        if ((i & 1) != mw) {
-          x0 += 128;
-          while (x0 >= rw) { x0 -= rw; if (++slot0 == NR) slot0 = 0; }
-          xn += 128;
-          while (xn >= rw) { xn -= rw; ++gn; }
-          continue;
-        }
-        const int need = min(rows_total, gn + (R - 1));
-        while (rows_conf <= need) {
-          mbar_wait(&hd->row_full[rslot], rpar);
-          ++rows_conf;
-          if (++rslot == NR) { rslot = 0; rpar ^= 1u; }
-        }
-        fence_proxy_async_smem();   // rows were written by cp.async (generic proxy); tcgen05.mma reads through the async proxy
-        const int as = i & (kD3MaxAcc - 1);
-        mbar_wait(&hd->acc_empty[as], (((uint32_t)i / kD3MaxAcc) & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t d_addr = tmem_base + (uint32_t)(as * N);
-        int s1 = slot0 + 1; if (s1 >= NR) s1 -= NR;
-        int s2 = s1 + 1; if (s2 >= NR) s2 -= NR;
-        const uint32_t arow[3] = {a_lo + (uint32_t)(slot0 * rw + x0), a_lo + (uint32_t)(s1 * rw + x0), a_lo + (uint32_t)(s2 * rw + x0)};
-#pragma unroll
-        for (int r = 0; r < (S2 ? 2 : R); ++r) {
-#pragma unroll
-          for (int s = 0; s < (S2 ? 2 : R); ++s) {
-#pragma unroll
-            for (int kk = 0; kk < KS; ++kk) {
-              const uint64_t adesc = a_hi | (uint64_t)(arow[r] + (uint32_t)s + (uint32_t)kk * kk_step);
-              const uint64_t bdesc = b_hi | (uint64_t)(b_lo + (uint32_t)(((r * R + s) * KS + kk) * 2 * N));
-              umma_f16_ss(d_addr, adesc, bdesc, p.idesc, (r | s | kk) != 0 ? 1u : 0u);
-            }
-          }
-        }
-        umma_commit(&hd->acc_full[as]);
-        umma_commit(&hd->tile_done[i & (kD3TileBars - 1)]);
+  } else if (warp >= 4) {
+    // ================================================================= MMA + epilogue sets.  Set e takes tiles e, e + kD3EpiSets, ...
+    // Its 128 threads issue the tile's MMAs as two m64 wgmma (rows [64h, 64h + 64)); the thread's scalar work is strength-reduced:
+    // positions advance incrementally and the 64-bit descriptors differ only in the 14-bit address field (one position = 16 B =
+    // one unit of addr>>4).  Warp `quad` then holds tile rows 16*quad + (0..15) and 64 + 16*quad + (0..15) and gives lane l the
+    // row `row` below: one output position per thread.
+    const int e = (warp - 4) >> 2, quad = warp & 3;
+    const int row = 16 * quad + (lane & 15) + 64 * (lane >> 4);
+    float* xp = reinterpret_cast<float*>(smem + kD3XposeOff) + (size_t)(warp - 4) * 32 * kD3XposePitch;
+    const uint32_t a_lbo = p.swap_lbo_sbo ? 128u : p.plane_stride, a_sbo = p.swap_lbo_sbo ? p.plane_stride : 128u;
+    const uint32_t b_lbo = p.swap_lbo_sbo ? 128u : (uint32_t)N * 16u, b_sbo = p.swap_lbo_sbo ? (uint32_t)N * 16u : 128u;
+    const uint32_t a_lo = (((a_lbo >> 4) & 0x3FFFu) << 16) + (smem_u32(ring) >> 4);
+    const uint32_t b_lo = (((b_lbo >> 4) & 0x3FFFu) << 16) + (smem_u32(wsm) >> 4);
+    const uint64_t a_hi = (uint64_t)((a_sbo >> 4) & 0x3FFFu) << 32;
+    const uint64_t b_hi = (uint64_t)((b_sbo >> 4) & 0x3FFFu) << 32;
+    const uint32_t kk_step = (2u * p.plane_stride) >> 4;
+    const int rows_total = row_hi - row_lo;
+    int x0 = 128 * t0 - row_lo * rw, slot0 = 0, g0 = 0;   // first output position of the tile: (ring slot, column), relative row
+    int xn = x0 + 127 + (R - 1), gn = 0;                  // last input position of tap (0, R-1): row (relative), column
+    while (xn >= rw) { xn -= rw; ++gn; }
+    auto advance = [&](int tiles) {
+      for (int k = 0; k < tiles; ++k) {
         x0 += 128;
-        while (x0 >= rw) { x0 -= rw; if (++slot0 == NR) slot0 = 0; }
+        while (x0 >= rw) { x0 -= rw; ++g0; if (++slot0 == NR) slot0 = 0; }
         xn += 128;
         while (xn >= rw) { xn -= rw; ++gn; }
       }
-    }
-  } else if (warp >= 4) {
-    // ================================================================= epilogue: one output position per thread
-    const int e = (warp - 4) >> 2, quad = warp & 3;
-    const int row = quad * 32 + lane;
+    };
+    advance(e);
+    int rows_conf = 0;
     // Coordinates and the residual row of a tile depend on nothing the MMAs produce, so they are fetched early: for
     // N <= 32 one whole tile ahead (the global-load latency hides behind the previous tile's epilogue), for N = 64 (128
     // bytes per thread) just before the wait for the accumulator.
@@ -310,18 +263,66 @@ __global__ void __launch_bounds__(kD3Threads, 1) conv3_direct_kernel(const Conv3
       const bool valid = cur.valid;
       const long pix = cur.pix;
       const int b = cur.b, y = cur.y, x = cur.x;
-      const int as = i & (kD3MaxAcc - 1);
-      mbar_wait(&hd->acc_full[as], ((uint32_t)i / kD3MaxAcc) & 1u);
-      tc_fence_after();
-      uint32_t v[N / 16][16];
-      const uint32_t trow = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(as * N);
+      // rows of the ring this tile reads: [g0, need].  Each is waited for by its own (slot, parity), so a set never waits on
+      // a row that only other sets' tiles read (the producer may already have refilled that slot)
+      {
+        const int need = min(rows_total, gn + (R - 1));
+        for (int k = max(rows_conf, g0); k <= need; ++k) mbar_wait(&hd->row_full[k % NR], (uint32_t)(k / NR) & 1u);
+        rows_conf = max(rows_conf, need + 1);
+      }
+      fence_proxy_async_smem();   // rows were written by cp.async (generic proxy); wgmma reads through the async proxy
+      float acc[2][N / 2];
+      {
+        int s1 = slot0 + 1; if (s1 >= NR) s1 -= NR;
+        int s2 = s1 + 1; if (s2 >= NR) s2 -= NR;
+        const uint32_t arow[3] = {a_lo + (uint32_t)(slot0 * rw + x0), a_lo + (uint32_t)(s1 * rw + x0), a_lo + (uint32_t)(s2 * rw + x0)};
+        wgmma_fence_regs(acc[0]);
+        wgmma_fence_regs(acc[1]);
+        wgmma_fence();
 #pragma unroll
-      for (int c = 0; c < N / 16; ++c) tmem_ld16_issue(trow + c * 16, v[c]);
+        for (int h = 0; h < 2; ++h) {
 #pragma unroll
-      for (int c = 0; c < N / 16; ++c) tmem_ld_wait(v[c]);
-      tc_fence_before();
+          for (int r = 0; r < (S2 ? 2 : R); ++r) {
+#pragma unroll
+            for (int s = 0; s < (S2 ? 2 : R); ++s) {
+#pragma unroll
+              for (int kk = 0; kk < KS; ++kk) {
+                const uint64_t adesc = a_hi | (uint64_t)(arow[r] + (uint32_t)(64 * h + s) + (uint32_t)kk * kk_step);
+                const uint64_t bdesc = b_hi | (uint64_t)(b_lo + (uint32_t)(((r * R + s) * KS + kk) * 2 * N));
+                Wgmma<N>::mma(acc[h], adesc, bdesc, (r | s | kk) != 0 ? 1u : 0u);
+              }
+            }
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc[0]);
+        wgmma_fence_regs(acc[1]);
+      }
       __syncwarp();
-      if (lane == 0) mbar_arrive(&hd->acc_empty[as]);
+      if (lane == 0) mbar_arrive(&hd->tile_done[i & (kD3TileBars - 1)]);   // this warp's reads of the ring are complete
+      advance(kD3EpiSets);
+      // fragments -> one row per lane, 16 columns at a time
+      uint32_t v[N / 16][16];
+#pragma unroll
+      for (int c = 0; c < N / 16; ++c) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int j = 8 * c; j < 8 * c + 8; j += 2) {
+            const int lr = (lane >> 2) + 8 * ((j >> 1) & 1) + 16 * h, lc = 8 * ((j >> 2) - 2 * c) + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(xp + lr * kD3XposePitch + lc) = make_float2(acc[h][j], acc[h][j + 1]);
+          }
+        }
+        __syncwarp();
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const float4 t = *reinterpret_cast<const float4*>(xp + lane * kD3XposePitch + 4 * u);
+          v[c][4 * u] = __float_as_uint(t.x); v[c][4 * u + 1] = __float_as_uint(t.y);
+          v[c][4 * u + 2] = __float_as_uint(t.z); v[c][4 * u + 3] = __float_as_uint(t.w);
+        }
+        __syncwarp();
+      }
       if (UP) {
         // accumulator columns = (phase py*2+px, co): per phase a LayerNorm over the 16 channels (biased variance,
         // modules/common.py:150-155), ReLU, and the pixel shuffle to (2y+py, 2x+px)
@@ -410,16 +411,10 @@ __global__ void __launch_bounds__(kD3Threads, 1) conv3_direct_kernel(const Conv3
 #pragma unroll
         for (int j = 0; j < N / 8; ++j) rr[j] = rn[j];
       }
-      __syncwarp();   // tcgen05.ld of the next tile is warp-collective
     }
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
-  }
 }
 
 }  // namespace vsb

@@ -23,11 +23,13 @@ inline int conv3_direct_ring_rows(int C, int N, int W, int R = 3) {
   rows = std::min(rows, (kD3TileBars - 16) * 128 / rw);   // tiles in flight must stay below the tile_done barrier ring
   return rows;
 }
-// Fewest ring rows that cannot deadlock: a tile touches ceil(129/rw) + R rows at once, the producer refills a slot only after
-// the tiles that read its previous row are done, and the issuers run in order; two more rows keep loads ahead of the MMAs.
+// Fewest ring rows that are safe.  The kD3EpiSets sets work on consecutive tiles at the same time, and a set waits for ring row k
+// on (slot k % NR, parity of k / NR), which is only sound once row k - NR has landed; the producer refills a slot only after the
+// tiles that read its previous row are done.  So the ring must hold every row that kD3EpiSets consecutive tiles read
+// (ceil((kD3EpiSets*128 + R - 1) / rw) + R - 1) plus one; two more rows keep loads ahead of the MMAs.
 inline int conv3_direct_min_rows(int W, int R = 3) {
   const int rw = (W + R - 1 + 7) / 8 * 8;
-  return (129 + rw - 1) / rw + R + 2;
+  return (kD3EpiSets * 128 + R - 1 + rw - 1) / rw + R + 2;
 }
 // W = 0: channel-count check only (weight packing time)
 inline bool conv3_direct_ok(int C, int N, int ld_in, int W = 0, int R = 3) {
@@ -61,9 +63,6 @@ inline void setup_conv3_direct(Conv3DirectOp& op, const __half* x, int B, int H,
   p.w_off = kD3HeaderBytes;
   p.ring_off = kD3HeaderBytes + w_pad;
   op.smem = 1024 + (size_t)p.ring_off + (size_t)(C / 8) * p.plane_stride;
-  p.acc_stages = kD3MaxAcc;      // 8 stages x N <= 64 columns
-  p.tmem_cols = kD3MaxAcc * N;   // 128 / 256 / 512: powers of two
-  p.idesc = (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
   p.fd_rw = make_fastdiv(p.rw);
   p.fd_hp = make_fastdiv(p.hp);
   p.wpk = wpk;

@@ -1,12 +1,10 @@
-// K1/K2: implicit-GEMM convolution / linear layer on the 5th-gen tensor cores (tcgen05.mma,
-// accumulators in TMEM), persistent and warp-specialised:
+// K1/K2: implicit-GEMM convolution / linear layer on the Hopper tensor cores (wgmma, fp32 accumulators in registers),
+// persistent and warp-specialised:
 //
-//   warp 0        : TMA producer (weights unless resident; activations for LD_TMA; input halo tiles for LD_HALO_*)
-//   warp 1        : single-thread tcgen05.mma issuer
-//   warp 2        : TMEM allocator
-//   warps 4..11   : epilogue (TMEM -> registers -> fused bias/BN-fold/act/residual/LN/tanh/GRN-stats -> HBM);
-//                   warp w owns TMEM lane quadrant w%4 and every second 16-column chunk ((w-4)/4)
-//   warps 12..15  : A-tile builders (all loaders except LD_TMA):
+//   warps 0..E-1  : epilogue, E = 8 (LD_TMA) or 4 (accumulator tile in shared memory -> registers -> fused bias/BN-fold/act/
+//                   residual/LN/tanh/GRN-stats -> HBM); warp w owns rows 32*(w%4) .. +31 (one row per lane) and the 16-column
+//                   chunks c with c % (E/4) == w/4
+//   warps E..E+3  : A-tile builders (all loaders except LD_TMA):
 //       LD_HALO_CONV3 : on-chip im2col - the (8+2)x(16+2) input halo of an 8x16 output tile is TMA-loaded ONCE per channel
 //                       chunk (zero fill = conv padding) and the tap tiles are copied smem->smem into the swizzled
 //                       UMMA layout (input pixels cross L2->SM once instead of nine times)
@@ -17,9 +15,14 @@
 //                       reflect-padded head conv)
 //       LD_GATHER_SCALE: A[m,k] = G[m,k] * scale[sample(m), k]  (ConvNeXt pwconv2 with the GRN factor folded in)
 //
+//   next 8 warps  : two MMA warpgroups; warpgroup h issues the wgmma of rows [64h, 64h + 64) of the tile
+//   last warp     : TMA producer (weights unless resident; activations for LD_TMA; input halo tiles for LD_HALO_*)
+//
 // GEMM view: D[M = output pixels, N = C_out] = A[M, K = taps*C_in] * W[N, K]^T, fp16 operands, fp32 accumulation.
-// BLOCK_M = 128 (one UMMA M=128 atom, cta_group::1), BLOCK_N <= 256, two TMEM accumulator stages so the epilogue of
-// tile i overlaps the main loop of tile i+1.  Small weight matrices stay resident in shared memory.
+// BLOCK_M = 128, BLOCK_N <= 128.  The MMA warpgroups hand each finished accumulator round to the epilogue through one
+// [128 x 128] fp32 tile in shared memory (the epilogue reads one row per thread) and meanwhile run the main loop of the
+// next round in registers, so the epilogue of tile i overlaps the main loop of tile i+1.  Small weight matrices stay
+// resident in shared memory.
 //
 // Replaces: nn.Conv2d / nn.Linear + BatchNorm2d(eval) + ReLU / LayerNorm / GELU / GRN / tanh call sites of
 // videoseal/modules/unet.py:17-197, modules/common.py:45-52,150-169, modules/convnext.py:41-57,
@@ -36,8 +39,12 @@ enum : int { ACT_NONE = 0, ACT_RELU = 1, ACT_GELU = 2 };
 constexpr int kBlockM = 128;
 constexpr int kMaxStages = 24;
 constexpr int kMaxHalo = 8;
-constexpr int kTmemCols = 512;
-constexpr int kAccStride = 256;     // TMEM columns between the two accumulator stages
+constexpr int kMaxBlockN = 128;
+constexpr int kAccCols = 128;       // columns of one accumulator round (group * block_n)
+constexpr int kAccPitch = kAccCols + 4;   // floats per row of the shared accumulator tile: row-per-thread float4 reads are conflict-free
+constexpr uint32_t kAccBytes = (uint32_t)kBlockM * kAccPitch * 4;
+constexpr int kEpiWarps = 8;       // LD_TMA; the loaders with 4 builder warps have 4 epilogue warps (17 warps either way: 96 registers)
+constexpr int kMmaThreads = 256;    // two MMA warpgroups
 constexpr int kHeaderBytes = 11264;  // barriers | bias x2 | LN w,b / outc rows | outc partials (3 x [128][3])
 constexpr int kHaloTW = 16, kHaloTH = 8;
 constexpr int kHaloW = kHaloTW + 2, kHaloH = kHaloTH + 2;   // 18 x 10 input (or upsampled) halo of an 8x16 output tile
@@ -53,7 +60,7 @@ struct ConvGemmParams {
   FastDiv fd_ntiles, fd_tpi, fd_tx, fd_tw, fd_group, fd_rps, fd_hw, fd_cc, fd_ow, fd_oh, fd_ct, fd_s;
   // ---- GEMM view
   int M, N, num_kb, kblk, block_n, n_tiles, m_tiles, num_tiles, stages;
-  uint32_t a_stage_bytes, b_stage_bytes, stage_bytes, idesc;
+  uint32_t a_stage_bytes, b_stage_bytes, stage_bytes;
   int group;                      // consecutive M tiles that share one accumulator round (amortises per-tile handshakes for small N)
   int b_resident;                 // whole [block_n x K] weight slab lives in shared memory for the kernel's lifetime
   int b_fixed_ntile;              // b_resident with several N tiles: this CTA only ever sees N tile blockIdx.x % n_tiles
@@ -66,7 +73,7 @@ struct ConvGemmParams {
   int ost_swz;                    //   0 linear, 1 / 2 / 3: 32 / 64 / 128-byte TMA swizzle of the box rows
   int bias_global;                // epilogue reads the bias straight from global memory (warp-uniform 16-byte loads, L1 hits) instead
                                   // of a shared copy: no per-tile barrier between the epilogue warps (whole tiles only)
-  uint32_t bres_off;
+  uint32_t bres_off, acc_off;
   // ---- output-tile geometry: tile_mode 0: rows are consecutive GEMM rows; 1: tile_h x tile_w pixel patch of an H x W map
   int tile_mode, H, W, tile_w, tile_h, tiles_x, tiles_per_img;
   // ---- A via TMA (LD_TMA): a_is_conv 0: 2D map (K, M); 1: 4D map (C, W, H, B) with zero-fill halo, one load per tap
@@ -108,8 +115,7 @@ struct ConvGemmParams {
 //   gelu(x) = 0.5 x (1 + erf(x / sqrt2)) = max(x, 0) - 0.5 |x| erfc(|x| / sqrt2),   erfc(|x| / sqrt2) = 2^Q(|x|)
 // Q = degree-5 polynomial without constant term (erfc(0) = 1), weighted minimax fit of log2 erfc on [0, 3.3 sqrt2] (oracle-side
 // check in tests/test_cpu_library.py): |gelu - exact| <= 1.0e-6 for every fp32 x in [-30, 30] (the tail runs to 2^-88 -> 0 on its
-// own).  The version this replaces (Abramowitz-Stegun 7.1.25) needed rcp AND ex2 per element and was MUFU-bound in the pwconv1
-// epilogue (profiles/r1_cnx_kernels_ncu.md: MIO stalls 19 %); its error was 2.5e-5.
+// own).  Abramowitz-Stegun 7.1.25 would need rcp AND ex2 per element, and its error is 2.5e-5.
 constexpr float kGeluQ0 = -1.1510894298553467f, kGeluQ1 = -0.4592657685279846f, kGeluQ2 = -0.05254320427775383f,
                 kGeluQ3 = 0.007386638317257166f, kGeluQ4 = -0.0005183160537853837f;
 __device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
@@ -124,9 +130,10 @@ __device__ __forceinline__ float gelu_erf(float x) {
   return fmaf(-0.5f * ax, e, fmaxf(x, 0.f));
 }
 
-// two GELUs at once with Blackwell's packed fp32 arithmetic (fma/mul .f32x2): the polynomial costs half the issue slots
-__device__ __forceinline__ float2 f2fma(float2 a, float2 b, float2 c) { return __ffma2_rn(a, b, c); }
-__device__ __forceinline__ float2 f2mul(float2 a, float2 b) { return __fmul2_rn(a, b); }
+// two GELUs at once, written on float2 pairs (each component rounds exactly like the scalar fma / mul / add)
+__device__ __forceinline__ float2 f2fma(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 f2mul(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 f2add(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 // packed in, packed out; max(x, 0) as 0.5 (x + |x|) so that the tail is two packed FMAs: gelu = 0.5 x + 0.5 |x| (1 - e)
 __device__ __forceinline__ float2 gelu_erf_p(float2 x) {
   const float2 ax = make_float2(fabsf(x.x), fabsf(x.y));
@@ -199,27 +206,99 @@ __device__ __forceinline__ void cp_async_wait_pending(int n) {   // wait until a
 template <int NT> __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory"); }
 __device__ __forceinline__ void bld_bar_sync() { asm volatile("bar.sync 2, 128;" ::: "memory"); }
 
-// epilogue warps: 16 for the pure-TMA kernels (GELU / GRN statistics are issue-bound; the small-K affine epilogues are bound by
-// the TMEM-load -> math -> store chain of each warp, profiles/r2g_gemm_ncu.md: twice the warps hide twice the latency), 8 when 4
-// builder warps also need registers
-template <int LOADER, int ACT> struct EpiCfg { static constexpr int kWarps = (LOADER == LD_TMA) ? 16 : 8; };
+// one row of the shared accumulator tile -> 16 registers
+__device__ __forceinline__ void acc_ld16(const float* src, uint32_t (&r)[16]) {
+#pragma unroll
+  for (int u = 0; u < 4; ++u) {
+    const float4 t = reinterpret_cast<const float4*>(src)[u];
+    r[4 * u] = __float_as_uint(t.x); r[4 * u + 1] = __float_as_uint(t.y); r[4 * u + 2] = __float_as_uint(t.z); r[4 * u + 3] = __float_as_uint(t.w);
+  }
+}
+__device__ __forceinline__ void acc_ld16(const float* src, float (&v)[16]) {
+#pragma unroll
+  for (int u = 0; u < 4; ++u) {
+    const float4 t = reinterpret_cast<const float4*>(src)[u];
+    v[4 * u] = t.x; v[4 * u + 1] = t.y; v[4 * u + 2] = t.z; v[4 * u + 3] = t.w;
+  }
+}
+
+// The MMA warpgroups: warpgroup wg computes rows [64 wg, 64 wg + 64) of every sub-tile in registers (BN = block_n columns),
+// keeping one wgmma group in flight, then writes them into the shared accumulator tile once the epilogue has drained it.
+template <int BN, int LOADER>
+__device__ __forceinline__ void mma_warpgroup(const ConvGemmParams& p, uint8_t* tiles, uint8_t* bres, uint64_t* full_bar,
+                                              uint64_t* empty_bar, uint64_t* tfull_bar, uint64_t* tempty_bar, uint64_t* bres_bar,
+                                              float* acc_s, int wg) {
+  const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
+  float d[BN / 2];
+  int stage = 0;
+  uint32_t phase = 0, aphase = 0;
+  const uint32_t row_bytes = (uint32_t)p.kblk * 2u;
+  const uint32_t a_off = (uint32_t)wg * 64u * row_bytes;   // 8-row swizzle atoms: a multiple of 1024 bytes
+  const int nmma = p.kblk >> 4;
+  if (p.b_resident) mbar_wait(bres_bar, 0u);
+  const uint32_t bres_addr = smem_u32(bres);
+  const int r0 = wg * 64 + wq * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+  auto release = [&](int s) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[s]);
+  };
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    const int st = p.fd_ntiles.div(tile);
+    for (int g = 0; g < p.group; ++g) {
+      if (st * p.group + g >= p.m_tiles) break;
+      int prev = -1;
+      for (int kb = 0; kb < p.num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        if (LOADER == LD_GATHER_CONV) fence_proxy_async_smem();   // cp.async-written A tile -> async proxy
+        const uint32_t sa = smem_u32(tiles + (size_t)stage * p.stage_bytes);
+        const uint64_t adesc = make_smem_desc(sa + a_off, row_bytes);
+        const uint64_t bdesc = make_smem_desc(p.b_resident ? bres_addr + (uint32_t)kb * p.b_stage_bytes : sa + p.a_stage_bytes, row_bytes);
+        wgmma_fence_regs(d);
+        wgmma_fence();
+        for (int j = 0; j < nmma; ++j) {
+          // advance 16 K-elements = 32 bytes inside the swizzled row: +2 in the (addr >> 4) field
+          Wgmma<BN>::mma(d, adesc + (uint64_t)(2 * j), bdesc + (uint64_t)(2 * j), (uint32_t)((kb | j) != 0));
+        }
+        wgmma_commit();
+        wgmma_fence_regs(d);
+        if (prev >= 0) {
+          wgmma_wait<1>();   // the previous K-block's wgmma have read their slot
+          release(prev);
+        }
+        prev = stage;
+        if (++stage == p.stages) { stage = 0; phase ^= 1u; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(d);
+      release(prev);
+      if (g == 0) mbar_wait(tempty_bar, aphase ^ 1u);   // the epilogue has read the previous round
+      float* dst = acc_s + g * BN;
+#pragma unroll
+      for (int i = 0; i < BN / 2; i += 2) {
+        const int r = r0 + 8 * ((i >> 1) & 1), c = 8 * (i >> 2) + c0;
+        *reinterpret_cast<float2*>(dst + r * kAccPitch + c) = make_float2(d[i], d[i + 1]);
+      }
+    }
+    mbar_arrive(tfull_bar);
+    aphase ^= 1u;
+  }
+}
 
 template <int LOADER, int ACT>
-__global__ void __launch_bounds__(LOADER == LD_TMA ? 640 : 512, 1)
+__global__ void __launch_bounds__(544, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
                  const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
                  const __grid_constant__ ConvGemmParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  // header (kHeaderBytes): barriers | tmem ptr | s_bias[2][256] | s_lnw[256] s_lnb[256] s_oc2[256] | s_dot[128][3]
+  // header (kHeaderBytes): barriers | s_bias[2][256] | s_lnw[256] s_lnb[256] s_oc2[256] | s_dot[128][3]
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem);
   uint64_t* empty_bar = full_bar + kMaxStages;
-  uint64_t* tfull_bar = empty_bar + kMaxStages;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint64_t* hfull_bar = tempty_bar + 2;
+  uint64_t* tfull_bar = empty_bar + kMaxStages;    // accumulator tile written by the MMA warpgroups
+  uint64_t* tempty_bar = tfull_bar + 1;            // accumulator tile read by the epilogue
+  uint64_t* hfull_bar = tempty_bar + 1;
   uint64_t* hempty_bar = hfull_bar + kMaxHalo;
   uint64_t* bres_bar = hempty_bar + kMaxHalo;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bres_bar + 1);
   float* s_bias = reinterpret_cast<float*>(smem + 1024);        // [2][256]
   float* s_lnw = reinterpret_cast<float*>(smem + 3072);         // [256]  (LN weight | outc row 0)
   float* s_lnb = reinterpret_cast<float*>(smem + 4096);         // [256]  (LN bias   | outc row 1)
@@ -230,26 +309,27 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint8_t* ubuf = smem + p.u_off;
   uint8_t* bres = smem + p.bres_off;
   uint8_t* rbuf = smem + p.resid_off;
+  float* acc_s = reinterpret_cast<float*>(smem + p.acc_off);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   constexpr uint32_t kNumBuilders = 128;
   constexpr bool kHalo = (LOADER == LD_HALO_CONV3 || LOADER == LD_HALO_UPS);
-  constexpr int kEpiWarps = EpiCfg<LOADER, ACT>::kWarps;
-  constexpr int kEpiThreads = kEpiWarps * 32;
-  constexpr int kEpiSplit = kEpiWarps / 4;          // warps sharing one TMEM lane quadrant (interleaved 16-column chunks)
-  constexpr int kBuilderWarp0 = 4 + kEpiWarps;
+  constexpr int kEpiW = LOADER == LD_TMA ? kEpiWarps : 4;
+  constexpr int kEpiThreads = kEpiW * 32;
+  constexpr int kEpiSplit = kEpiW / 4;              // warps sharing one 32-row quadrant (interleaved 16-column chunks)
+  constexpr int kBuilderWarp0 = kEpiW;
+  constexpr int kMmaWarp0 = kBuilderWarp0 + (LOADER == LD_TMA ? 0 : 4);   // warpgroup-aligned
+  constexpr int kProducerWarp = kMmaWarp0 + kMmaThreads / 32;
 
   if (threadIdx.x == 0) {
     const uint32_t full_count = LOADER == LD_TMA ? 1u : kNumBuilders + (p.b_resident ? 0u : 1u);
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], full_count);
-      mbar_init(&empty_bar[s], 1u);
+      mbar_init(&empty_bar[s], (uint32_t)(kMmaThreads / 32));
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1u);
-      mbar_init(&tempty_bar[s], (uint32_t)kEpiThreads);
-    }
+    mbar_init(tfull_bar, (uint32_t)kMmaThreads);
+    mbar_init(tempty_bar, (uint32_t)kEpiThreads);
     for (int s = 0; s < kMaxHalo; ++s) {
       mbar_init(&hfull_bar[s], 1u);
       mbar_init(&hempty_bar[s], kNumBuilders);
@@ -261,10 +341,6 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     tma_prefetch_desc(&tmB);
     if (p.tma_store) tma_prefetch_desc(&tmO);
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_ptr_smem, kTmemCols);
-    tmem_relinquish();
-  }
   if (p.epi == EPI_LN) {
     for (int i = threadIdx.x; i < p.N; i += blockDim.x) { s_lnw[i] = p.ln_w[i]; s_lnb[i] = p.ln_b[i]; }
   } else if (p.outc_w != nullptr) {  // fused 1x1 outc: N <= 256 (n_tiles == 1), up to 3 output channels
@@ -274,16 +350,12 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       s_oc2[i] = p.n_out > 2 ? p.outc_w[2 * p.N + i] : 0.f;
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   // (PDL builds) nothing above reads or writes a tensor produced by an earlier kernel: only parameters and weights
   pdl_launch_dependents();
   pdl_wait();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  const uint32_t row_bytes = (uint32_t)p.kblk * 2u;
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ===================================================================== TMA producer
     if (elect_one()) {
       int stage = 0;
@@ -359,49 +431,25 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
        }
       }
     }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer
-    if (elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      const int nmma = p.kblk >> 4;
-      if (p.b_resident) { mbar_wait(bres_bar, 0u); tc_fence_after(); }
-      const uint32_t bres_addr = smem_u32(bres);
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        mbar_wait(&tempty_bar[as], aphase ^ 1u);
-        tc_fence_after();
-        const int st = p.fd_ntiles.div(tile);
-       for (int g = 0; g < p.group; ++g) {
-        if (st * p.group + g >= p.m_tiles) break;
-        const uint32_t d_tmem = tmem_base + (uint32_t)(as * kAccStride + g * p.block_n);
-        for (int kb = 0; kb < p.num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          if (LOADER == LD_GATHER_CONV) fence_proxy_async_smem();   // cp.async-written A tile -> async proxy
-          tc_fence_after();
-          const uint32_t sa = smem_u32(tiles + (size_t)stage * p.stage_bytes);
-          const uint64_t adesc = make_smem_desc(sa, row_bytes);
-          const uint64_t bdesc = make_smem_desc(p.b_resident ? bres_addr + (uint32_t)kb * p.b_stage_bytes : sa + p.a_stage_bytes, row_bytes);
-          for (int j = 0; j < nmma; ++j) {
-            // advance 16 K-elements = 32 bytes inside the swizzled row: +2 in the (addr >> 4) field
-            umma_f16_ss(d_tmem, adesc + (uint64_t)(2 * j), bdesc + (uint64_t)(2 * j), p.idesc, (uint32_t)((kb | j) != 0));
-          }
-          umma_commit(&empty_bar[stage]);  // frees the smem slot once these MMAs have read it
-          if (++stage == p.stages) { stage = 0; phase ^= 1u; }
-        }
-       }
-        umma_commit(&tfull_bar[as]);  // accumulators of the whole group complete -> epilogue
-        as ^= 1;
-        if (as == 0) aphase ^= 1u;
-      }
+  } else if (warp >= kMmaWarp0) {
+    // ===================================================================== MMA warpgroups
+    const int wg = (warp - kMmaWarp0) >> 2;
+    switch (p.block_n) {
+      case 16: mma_warpgroup<16, LOADER>(p, tiles, bres, full_bar, empty_bar, tfull_bar, tempty_bar, bres_bar, acc_s, wg); break;
+      case 32: mma_warpgroup<32, LOADER>(p, tiles, bres, full_bar, empty_bar, tfull_bar, tempty_bar, bres_bar, acc_s, wg); break;
+      case 48: mma_warpgroup<48, LOADER>(p, tiles, bres, full_bar, empty_bar, tfull_bar, tempty_bar, bres_bar, acc_s, wg); break;
+      case 64: mma_warpgroup<64, LOADER>(p, tiles, bres, full_bar, empty_bar, tfull_bar, tempty_bar, bres_bar, acc_s, wg); break;
+      case 80: mma_warpgroup<80, LOADER>(p, tiles, bres, full_bar, empty_bar, tfull_bar, tempty_bar, bres_bar, acc_s, wg); break;
+      case 96: mma_warpgroup<96, LOADER>(p, tiles, bres, full_bar, empty_bar, tfull_bar, tempty_bar, bres_bar, acc_s, wg); break;
+      case 112: mma_warpgroup<112, LOADER>(p, tiles, bres, full_bar, empty_bar, tfull_bar, tempty_bar, bres_bar, acc_s, wg); break;
+      default: mma_warpgroup<128, LOADER>(p, tiles, bres, full_bar, empty_bar, tfull_bar, tempty_bar, bres_bar, acc_s, wg); break;
     }
-  } else if (warp >= 4 && warp < 4 + kEpiWarps) {
-    // ===================================================================== epilogue (8 or 16 warps)
-    const int q = warp & 3;            // TMEM lane quadrant this warp may access
-    const int half = (warp - 4) >> 2;  // which 16-column chunks: chunk index modulo kEpiSplit
+  } else if (warp < kEpiW) {
+    // ===================================================================== epilogue (4 or 8 warps)
+    const int q = warp & 3;            // 32-row quadrant of the tile this warp owns
+    const int half = warp >> 2;        // which 16-column chunks: chunk index modulo kEpiSplit
     const int row = q * 32 + lane;
-    const int et = threadIdx.x - 128;  // 0..kEpiThreads-1
+    const int et = threadIdx.x;        // 0..kEpiThreads-1
     const int nchunks = p.block_n >> 4;
     // 16-column chunks of this warp: interleaved (half, half + kEpiSplit, ...) or, with TMA stores, cpw consecutive ones
     int c_beg = half, c_end = nchunks, c_step = kEpiSplit;
@@ -411,7 +459,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       c_end = c_beg + base + (half < rem ? 1 : 0);
       c_step = 1;
     }
-    uint8_t* ost = smem + p.ostage_off + (size_t)(warp - 4) * p.ostage_bytes;   // this warp's output staging boxes
+    uint8_t* ost = smem + p.ostage_off + (size_t)warp * p.ostage_bytes;   // this warp's output staging boxes
     const uint32_t ost_box = 32u * p.ost_rowb;
     const uint32_t ost_upc = p.tma_store == 2 ? 4u : 2u;                         // 16-byte units per chunk
     // 16-byte unit u of row r of a swizzled box lives at unit u ^ f(r) (CU_TENSOR_MAP_SWIZZLE_{32,64,128}B)
@@ -471,7 +519,6 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       cp_async_commit();
     };
 
-    int as = 0;
     uint32_t aphase = 0;
     int bsel = 0;
     int slot = 0;
@@ -495,10 +542,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         if (pslot >= D) pslot -= D;
         prefetch_resid(sq + D - 1, pslot);
       }
-      if (g == 0) {
-        mbar_wait(&tfull_bar[as], aphase);
-        tc_fence_after();
-      }
+      if (g == 0) mbar_wait(tfull_bar, aphase);
       cp_async_wait_pending(D - 1);
       const int m_tile = st * G + g;
       const uint8_t* rb_ = rbuf + (size_t)slot * p.resid_stride;
@@ -507,13 +551,12 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       long m; bool mvalid;
       tile_row(m_tile, m, mvalid);
       const bool res_fast = mvalid && (n0 + p.block_n <= p.N);
-      const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * kAccStride + g * p.block_n);
+      const float* trow = acc_s + row * kAccPitch + g * p.block_n;
 
       if (p.epi == EPI_LN) {
         // channels-first LayerNorm over the full C_out row (biased variance), then activation.  The kEpiSplit warps that share a
-        // TMEM lane quadrant split the 16-column chunks: pass 1 = per-warp partial (sum, sum of squares) of its chunks, exchanged
-        // through shared memory and added in a fixed order; pass 2 = normalise + store its chunks.  (The first version let one warp
-        // per quadrant walk the whole row three times: stem GEMM 124 us at 19 TF/s.)
+        // 32-row quadrant split the 16-column chunks: pass 1 = per-warp partial (sum, sum of squares) of its chunks, exchanged
+        // through shared memory and added in a fixed order; pass 2 = normalise + store its chunks.
         {
           const int N = p.N;
           float* s_part = s_dot;                                  // [kEpiSplit][128][2]
@@ -521,7 +564,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           for (int ch = half; ch < nchunks; ch += kEpiSplit) {
             const int c = ch * 16;
             float v[16];
-            tmem_ld16(trow + c, v);
+            acc_ld16(trow + c, v);
 #pragma unroll
             for (int j = 0; j < 16; ++j) {
               const float x = (c + j < N) ? v[j] + sb[c + j] : 0.f;
@@ -540,7 +583,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           for (int ch = half; ch < nchunks; ch += kEpiSplit) {
             const int c = ch * 16;
             float v[16];
-            tmem_ld16(trow + c, v);
+            acc_ld16(trow + c, v);
             if (c >= N) continue;
 #pragma unroll
             for (int j = 0; j < 16; ++j) {
@@ -598,7 +641,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         const bool lean = ACT == ACT_GELU ? (whole && !has_res && (p.grn_stats == nullptr || grn_uniform))
                                           : (whole && p.grn_stats == nullptr && (!has_res || (p.resid16 != nullptr && res_fast)));
         uint32_t vnext[16];
-        if (c_beg < c_end) tmem_ld16_issue(trow + c_beg * 16, vnext);
+        if (c_beg < c_end) acc_ld16(trow + c_beg * 16, vnext);
         const bool use_ts = p.tma_store == 1 && lean;      // this warp's part of the tile leaves through its staging boxes + TMA stores
         const bool use_ts32 = p.tma_store == 2 && lean32 && p.out16 == nullptr;
         if (use_ts || use_ts32) {                          // the previous stores of this warp have finished reading the staging boxes
@@ -607,21 +650,19 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
         if (ACT == ACT_GELU && lean) {
           // pwconv1 on whole tiles (every shipped card): bias + GELU + fp16 store + GRN column statistics and nothing else, in packed
-          // fp32 arithmetic throughout.  The accumulators are consumed straight out of the TMEM load registers by the packed bias add,
-          // so the next chunk's load can be issued without a register copy; one saturating F2FP per output pair.
+          // fp32 arithmetic throughout; one saturating F2FP per output pair.
           const __half* orow = p.out16 + m * p.ld_out16 + n0;
           for (int ch = c_beg; ch < c_end; ch += c_step) {
             const int c = ch * 16;
-            tmem_ld_wait(vnext);
             const float4* sb4 = reinterpret_cast<const float4*>(sb + c);
             float2 w2[8];
 #pragma unroll
             for (int u = 0; u < 4; ++u) {
               const float4 bq = sb4[u];
-              w2[2 * u] = __fadd2_rn(make_float2(__uint_as_float(vnext[4 * u]), __uint_as_float(vnext[4 * u + 1])), make_float2(bq.x, bq.y));
-              w2[2 * u + 1] = __fadd2_rn(make_float2(__uint_as_float(vnext[4 * u + 2]), __uint_as_float(vnext[4 * u + 3])), make_float2(bq.z, bq.w));
+              w2[2 * u] = f2add(make_float2(__uint_as_float(vnext[4 * u]), __uint_as_float(vnext[4 * u + 1])), make_float2(bq.x, bq.y));
+              w2[2 * u + 1] = f2add(make_float2(__uint_as_float(vnext[4 * u + 2]), __uint_as_float(vnext[4 * u + 3])), make_float2(bq.z, bq.w));
             }
-            if (ch + c_step < c_end) tmem_ld16_issue(trow + c + 16 * c_step, vnext);   // overlaps the math below
+            if (ch + c_step < c_end) acc_ld16(trow + c + 16 * c_step, vnext);   // overlaps the math below
 #pragma unroll
             for (int j = 0; j < 8; ++j) w2[j] = gelu_erf_p(w2[j]);
             {
@@ -641,7 +682,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               float sq[16];
 #pragma unroll
               for (int j = 0; j < 8; ++j) {
-                const float2 t2 = __fmul2_rn(w2[j], w2[j]);
+                const float2 t2 = f2mul(w2[j], w2[j]);
                 sq[2 * j] = t2.x; sq[2 * j + 1] = t2.y;
               }
 #pragma unroll
@@ -678,10 +719,9 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int ch = c_beg; ch < c_end; ch += c_step) {
           const int c = ch * 16;
           float v[16];
-          tmem_ld_wait(vnext);
 #pragma unroll
           for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(vnext[j]);
-          if (ch + c_step < c_end) tmem_ld16_issue(trow + c + 16 * c_step, vnext);   // overlaps the math below
+          if (ch + c_step < c_end) acc_ld16(trow + c + 16 * c_step, vnext);   // overlaps the math below
           const int n = n0 + c;
           if (ACT == ACT_NONE && lean32) {
             // pwconv2 on whole tiles: bias + fp32 residual stream from the prefetch ring, updated in place (+ fp16 copy)
@@ -917,10 +957,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
      }  // g
-      tc_fence_before();
-      mbar_arrive(&tempty_bar[as]);
-      as ^= 1;
-      if (as == 0) aphase ^= 1u;
+      mbar_arrive(tempty_bar);
+      aphase ^= 1u;
       bsel ^= 1;
     }
     if (p.tma_store && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // all stores of this warp have landed
@@ -1122,12 +1160,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     }
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
 }
 
 }  // namespace vsb

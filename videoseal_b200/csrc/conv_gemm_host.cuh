@@ -6,7 +6,6 @@
 #include <string>
 
 #include "conv_gemm.cuh"
-#include "conv_pair.cuh"
 
 namespace vsb {
 
@@ -86,27 +85,18 @@ struct ConvGemmOp {
   CUtensorMap tmA, tmA2, tmB, tmO;
   int grid = 0, threads = 0;
   int w_samples = 1;   // > 1: weights are [w_samples][N][K], sample = row / rows_per_sample (finalize_op)
-  bool pair = false;   // long-K conv on whole 128-pixel row tiles: CTA-pair kernel (conv_pair.cuh), parameters in pp, weights map in tmB
-  ConvPairParams pp;
-  size_t pair_smem = 0;
-  int pair_grid = 0;
   size_t smem = 0;
   const char* name = "";
-  ConvGemmOp() { memset(&pp, 0, sizeof(pp)); memset(&p, 0, sizeof(p)); memset(&tmA, 0, sizeof(tmA)); memset(&tmA2, 0, sizeof(tmA2)); memset(&tmB, 0, sizeof(tmB)); memset(&tmO, 0, sizeof(tmO)); }
+  ConvGemmOp() { memset(&p, 0, sizeof(p)); memset(&tmA, 0, sizeof(tmA)); memset(&tmA2, 0, sizeof(tmA2)); memset(&tmB, 0, sizeof(tmB)); memset(&tmO, 0, sizeof(tmO)); }
 };
 
-inline int pick_block_n(int N, int max_bn = 256) {
+// the largest tile in {max_bn, ..., 32} (multiples of 16) that divides N rounded up to 16; else max_bn with a ragged last tile
+inline int pick_block_n(int N, int max_bn = kMaxBlockN) {
   const int n16 = (N + 15) / 16 * 16;
   if (n16 <= max_bn) return n16;
-  if (max_bn < 256) {
-    for (int bn = max_bn / 16 * 16; bn >= 64; bn -= 16)
-      if (n16 % bn == 0) return bn;
-    return max_bn / 16 * 16;
-  }
-  // prefer the largest tile in {256,...,128} (multiples of 16) that divides n16; else 256 with a ragged last tile
-  for (int bn = 256; bn >= 128; bn -= 16)
+  for (int bn = max_bn / 16 * 16; bn >= 32; bn -= 16)
     if (n16 % bn == 0) return bn;
-  return 256;
+  return max_bn / 16 * 16;
 }
 
 // Common finalisation: weights map, tiling, stage count, smem, grid.
@@ -114,15 +104,16 @@ inline int pick_block_n(int N, int max_bn = 256) {
 inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw, int num_sms, int block_n_override = 0) {
   ConvGemmParams& p = op.p;
   p.N = N;
-  // an fp32 residual tile is prefetched into shared memory: keep it <= 64 KB
-  p.block_n = block_n_override ? block_n_override : pick_block_n(N, p.resid32 ? 128 : 256);
-  VSB_CHECK(p.block_n % 16 == 0 && p.block_n >= 16 && p.block_n <= 256, "bad block_n");
+  // block_n <= 128: the two MMA warpgroups hold a 128 x block_n fp32 accumulator in registers (block_n / 2 per thread); an fp32
+  // residual tile is prefetched into shared memory beside the accumulator tile: keep it <= 32 KB
+  p.block_n = block_n_override ? block_n_override : pick_block_n(N, p.resid32 ? 64 : kMaxBlockN);
+  VSB_CHECK(p.block_n % 16 == 0 && p.block_n >= 16 && p.block_n <= kMaxBlockN, "bad block_n");
   p.n_tiles = (N + p.block_n - 1) / p.block_n;
-  // small-N layers: several consecutive M tiles share one accumulator round (TMEM columns g*block_n) so that the per-tile
-  // barrier handshakes / index math are amortised
+  // small-N layers: several consecutive M tiles share one accumulator round (columns g*block_n of the accumulator tile) so that
+  // the per-tile barrier handshakes / index math are amortised
   p.group = 1;
   if (!getenv("VSB_NO_GROUP")) {
-    p.group = p.block_n <= 32 ? kAccStride / p.block_n : 1;   // measured: only pays off for N <= 32
+    p.group = p.block_n <= 32 ? kAccCols / p.block_n : 1;
     if (p.group > 4) p.group = 4;
     if (p.group < 1) p.group = 1;
     if (p.m_tiles < 4 * num_sms) p.group = 1;   // keep enough tiles for load balance
@@ -136,7 +127,8 @@ inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw,
   p.b_stage_bytes = (uint32_t)(p.block_n * p.kblk * 2);
   p.stage_bytes = p.a_stage_bytes + ((p.b_stage_bytes + 1023u) & ~1023u);
   VSB_CHECK(p.a_stage_bytes % 1024 == 0, "A stage must be 1024B aligned");
-  // shared memory: [header | stages x (A|B) | 2 halo tiles | upsampled halo | resident weights | residual ring]
+  // shared memory: [header | stages x (A|B) | halo tiles | upsampled halo | resident weights | residual ring | output staging |
+  // accumulator tile]
   size_t resid_one = 0;
   p.resid_direct = 0;
   if (p.resid16 && op.loader == LD_TMA && p.num_kb >= 24 && (p.ld_res16 % 8) == 0 && N % p.block_n == 0 && (long)p.m_tiles * kBlockM == (long)p.M &&
@@ -150,9 +142,9 @@ inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw,
   p.resid_stride = (uint32_t)resid_one;
   const size_t resid_bytes = resid_one * depth;
   p.halo_stride = (uint32_t)(((size_t)p.halo_bytes + 1023) & ~size_t(1023));
-  // halo ring: as deep as ~48 KB allows (2..8): the producer prefetches that many tiles ahead of the builders
+  // halo ring: as deep as ~24 KB allows (2..8): the producer prefetches that many tiles ahead of the builders
   p.halo_bufs = 2;
-  if (p.halo_stride) { p.halo_bufs = (int)(49152 / p.halo_stride); if (p.halo_bufs > kMaxHalo) p.halo_bufs = kMaxHalo; if (p.halo_bufs < 2) p.halo_bufs = 2; }
+  if (p.halo_stride) { p.halo_bufs = (int)(24576 / p.halo_stride); if (p.halo_bufs > kMaxHalo) p.halo_bufs = kMaxHalo; if (p.halo_bufs < 2) p.halo_bufs = 2; }
   const size_t halo_total = (size_t)p.halo_bufs * p.halo_stride;
   const size_t u_bytes = op.loader == LD_HALO_UPS ? (((size_t)kHaloH * kHaloW * p.cc * 2 + 1023) & ~size_t(1023)) : 0;
   // resident weights: one N tile, whole K slab <= 48 KB -> loaded once per CTA instead of once per tile
@@ -160,21 +152,25 @@ inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw,
   p.b_resident = (p.n_tiles == 1 && bslab <= 48 * 1024 && op.w_samples == 1) ? 1 : 0;
   // several N tiles: every CTA keeps ONE N tile for its whole life (grid a multiple of n_tiles, tile = blockIdx.x + k * gridDim.x),
   // so its [block_n x K] weight slab can stay resident too when it fits beside >= 4 A stages.  Without this the slab is re-streamed
-  // from L2 for every M tile (res 1x1 384->384 @32^2: 151 MB of weight traffic per launch against 100 MB of activations: L2-bound).
+  // from L2 for every M tile (res 1x1 384->384: 295 KB of weights per M tile against 98 KB of activations).
   p.b_fixed_ntile = 0;
   if (!p.b_resident && p.n_tiles > 1 && p.n_tiles <= 8 && op.w_samples == 1 && op.loader == LD_TMA && !getenv("VSB_NO_BRES2") &&
-      kHeaderBytes + resid_bytes + bslab + 4 * (size_t)p.a_stage_bytes + 64 * 1024 <= 225 * 1024 && p.num_tiles >= 2 * num_sms) {
+      kHeaderBytes + resid_bytes + bslab + kAccBytes + 4 * (size_t)p.a_stage_bytes + 64 * 1024 <= 225 * 1024 && p.num_tiles >= 2 * num_sms) {
     p.b_resident = 1;
     p.b_fixed_ntile = 1;
   }
   if (getenv("VSB_NO_BRES")) { p.b_resident = 0; p.b_fixed_ntile = 0; }
+  // a resident slab that leaves fewer than 2 pipeline stages beside the rest is streamed instead
+  if (p.b_resident && !p.b_fixed_ntile &&
+      kHeaderBytes + resid_bytes + halo_total + u_bytes + bslab + kAccBytes + 2 * (size_t)p.a_stage_bytes + 1024 > 225 * 1024)
+    p.b_resident = 0;
   const size_t bres_bytes = p.b_resident ? bslab : 0;
   if (p.b_resident) p.stage_bytes = p.a_stage_bytes;
   // TMA-store epilogue (short main loops only: there the epilogue is the critical path; long-K layers keep their shared memory for
   // pipeline stages): whole tiles, fp16 output (affine / GELU epilogues) or the in-place fp32 residual stream of pwconv2
   p.tma_store = 0; p.cpw = 0; p.ostage_bytes = 0;
   {
-    const int nchunks = p.block_n / 16, epw = 4;     // 16 epilogue warps = 4 per TMEM lane quadrant
+    const int nchunks = p.block_n / 16, epw = kEpiWarps / 4;     // epilogue warps per 32-row quadrant
     const bool common = op.loader == LD_TMA && p.outc_w == nullptr && p.epi == EPI_AFFINE && (long)p.m_tiles * kBlockM == (long)p.M &&
                         N % p.block_n == 0 && p.num_kb <= 12 && !getenv("VSB_NO_TMA_STORE");
     if (common && p.out16 != nullptr && p.out32 == nullptr && (p.ld_out16 % 8) == 0 && (reinterpret_cast<uintptr_t>(p.out16) & 15) == 0)
@@ -195,9 +191,15 @@ inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw,
       p.ostage_bytes = (uint32_t)p.cpw * 32u * cb;               // per warp: multiples of 1024 bytes (swizzle atoms stay aligned)
     }
   }
-  const size_t ostage_total = p.tma_store ? (size_t)16 * p.ostage_bytes + 1024 : 0;
-  const size_t fixed = kHeaderBytes + resid_bytes + halo_total + u_bytes + bres_bytes + ostage_total;
-  VSB_CHECK(fixed + 2 * (size_t)p.stage_bytes <= 225 * 1024, "tile does not fit in shared memory");
+  size_t ostage_total = p.tma_store ? (size_t)kEpiWarps * p.ostage_bytes + 1024 : 0;
+  size_t fixed = kHeaderBytes + resid_bytes + halo_total + u_bytes + bres_bytes + ostage_total + kAccBytes;
+  if (p.tma_store && fixed + 2 * (size_t)p.stage_bytes > 225 * 1024) {   // no room for the staging boxes: plain stores
+    fixed -= ostage_total;
+    ostage_total = 0;
+    p.tma_store = 0; p.cpw = 0; p.ostage_bytes = 0;
+  }
+  VSB_CHECK(fixed + 2 * (size_t)p.stage_bytes <= 225 * 1024, "tile does not fit in shared memory (" + std::to_string(fixed) + " + 2 x " +
+            std::to_string(p.stage_bytes) + " bytes)");
   int stages = (int)((225 * 1024 - fixed) / p.stage_bytes);
   if (stages > kMaxStages) stages = kMaxStages;
   p.stages = stages;
@@ -206,7 +208,8 @@ inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw,
   p.bres_off = (uint32_t)(p.u_off + u_bytes);
   p.resid_off = (uint32_t)(p.bres_off + bres_bytes);
   p.ostage_off = (uint32_t)((p.resid_off + resid_bytes + 1023) & ~size_t(1023));   // swizzle atoms of the staging boxes need 1024-byte alignment
-  op.smem = 1024 /*align slack*/ + p.ostage_off + ostage_total;
+  p.acc_off = (uint32_t)(p.ostage_off + ostage_total);
+  op.smem = 1024 /*align slack*/ + p.acc_off + kAccBytes;
   if (p.tma_store) {   // output map: [M rows][N cols], box = one staging box (32 rows x 16 columns), dense rows
     uint64_t odims[2] = {(uint64_t)N, (uint64_t)p.M};
     uint32_t obox[2] = {(uint32_t)(p.ost_cpb * 16), 32u};
@@ -219,9 +222,7 @@ inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw,
       encode_map(&op.tmO, p.out32, 2, odims, ostrides, obox, 0, /*no_swizzle=*/true, /*f32=*/true, swzb);
     }
   }
-  // instruction descriptor (kind::f16): D=f32 (bit 4), A=B=f16 (0), K-major both, N>>3 at bit 17, M>>4 at bit 24
-  p.idesc = (1u << 4) | ((uint32_t)(p.block_n >> 3) << 17) | ((uint32_t)(kBlockM >> 4) << 24);
-  if (p.epi == EPI_LN || p.outc_w) VSB_CHECK(p.n_tiles == 1 && N <= 256, "LN / fused-outc epilogues need the full row in one tile");
+  if (p.epi == EPI_LN || p.outc_w) VSB_CHECK(p.n_tiles == 1 && N <= kMaxBlockN, "LN / fused-outc epilogues need the full row in one tile");
   // weights: dims (K, N)
   if (op.w_samples > 1) {
     VSB_CHECK(op.loader == LD_TMA && !p.a_is_conv && p.rows_per_sample > 0 && p.rows_per_sample % kBlockM == 0 && N % p.block_n == 0,
@@ -239,35 +240,9 @@ inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw,
                    (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0 && !getenv("VSB_NO_BIAS_GLOBAL")) ? 1 : 0;
   op.grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
   if (p.b_fixed_ntile) op.grid = (num_sms / p.n_tiles) * p.n_tiles;
-  op.threads = op.loader == LD_TMA ? 640 : 512;
+  // 8 epilogue warps (LD_TMA) or 4 epilogue + 4 builder warps, 2 MMA warpgroups, the producer warp
+  op.threads = 544;
   VSB_CHECK((long)p.m_tiles * kBlockM < (1L << 31), "M too large for 32-bit row indices");
-  // CTA-pair kernel for the long-K convs on whole row tiles (the 16 bottleneck convs of the U-Net): plain bias / ReLU / fp16 residual epilogue
-  static const bool no_pair = getenv("VSB_NO_PAIR") != nullptr;
-  if (!no_pair && op.loader == LD_TMA && p.a_is_conv && p.kblk == 64 && p.num_kb >= 24 && p.tile_w == p.W && p.m_tiles % 2 == 0 &&
-      p.epi == EPI_AFFINE && (p.act == ACT_NONE || p.act == ACT_RELU) && p.out16 != nullptr && p.out32 == nullptr && p.resid32 == nullptr &&
-      p.outc_w == nullptr && p.grn_stats == nullptr && op.w_samples == 1 && p.bias != nullptr && (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0 &&
-      (p.ld_out16 % 8) == 0 && (p.resid16 == nullptr || p.ld_res16 % 8 == 0) && num_sms >= 2) {
-    int bn = 0;
-    for (int cand : {256, 192, 128}) if (N % cand == 0) { bn = cand; break; }
-    if (const char* e = getenv("VSB_PAIR_BN")) { const int v = atoi(e); if (v >= 32 && v <= 256 && v % 32 == 0 && N % v == 0) bn = v; }
-    if (bn) {
-      ConvPairParams& q = op.pp;
-      q.M = p.M; q.N = N; q.num_kb = p.num_kb; q.c_blocks = p.c_blocks; q.S = p.S; q.pad = p.pad;
-      q.tile_h = p.tile_h; q.tiles_per_img = p.tiles_per_img;
-      q.m_pairs = p.m_tiles / 2; q.n_tiles = N / bn; q.num_work = q.m_pairs * q.n_tiles;
-      q.block_n = bn; q.a_bytes = 128 * 64 * 2; q.b_bytes = (uint32_t)(bn / 2) * 64 * 2;
-      q.stages = (int)std::min<size_t>(kPairMaxStages, (size_t)(200 * 1024) / (q.a_bytes + q.b_bytes));
-      if (const char* e = getenv("VSB_PAIR_STAGES")) { const int v = atoi(e); if (v >= 2 && v <= q.stages) q.stages = v; }
-      q.idesc = (1u << 4) | ((uint32_t)(bn >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-      q.relu = p.act == ACT_RELU ? 1 : 0;
-      q.bias = p.bias; q.resid = p.resid16; q.ld_res = p.ld_res16; q.out = p.out16; q.ld_out = p.ld_out16;
-      uint32_t pbox[2] = {64u, (uint32_t)(bn / 2)};
-      encode_map(&op.tmB, W, 2, dims, strides, pbox, 64);      // each CTA of the pair stages half of the tile's weight rows
-      op.pair_smem = (size_t)q.stages * (q.a_bytes + q.b_bytes) + (2 * kPairMaxStages + 4) * sizeof(uint64_t) + 16 + 1024;
-      op.pair_grid = 2 * std::min(num_sms / 2, q.num_work);
-      op.pair = true;
-    }
-  }
 }
 
 // A = NHWC fp16 activation [B, H, W, C] (pixel pitch ld elements); conv RxS stride 1, zero padding `pad`
@@ -463,21 +438,7 @@ inline void launch_one(const ConvGemmOp& op, cudaStream_t st) {
 }
 
 // instantiated (loader, activation) pairs: only what the networks need, to bound compile time
-inline void launch_pair(const ConvGemmOp& op, cudaStream_t st) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    VSB_CUDA(cudaFuncSetAttribute(conv_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
-#ifdef VSB_PDL
-  launch_pdl(conv_pair_kernel, dim3(op.pair_grid), dim3(kPairThreads), op.pair_smem, st, op.tmA, op.tmB, op.pp);
-#else
-  conv_pair_kernel<<<op.pair_grid, kPairThreads, op.pair_smem, st>>>(op.tmA, op.tmB, op.pp);
-#endif
-}
-
 inline void launch(const ConvGemmOp& op, cudaStream_t st) {
-  if (op.pair) { launch_pair(op, st); VSB_CUDA(cudaGetLastError()); return; }
   const int a = op.p.act;
   switch (op.loader) {
     case LD_TMA:

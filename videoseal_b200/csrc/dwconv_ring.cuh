@@ -4,12 +4,12 @@
 //   * a block owns a band of NS*SX output columns of one image and walks R output rows; a thread owns one channel pair and a strip
 //     of SX columns.  Its 49 weights (packed fp32 pairs) stay in registers; every input row is read ONCE (SX+6 64-bit shared loads)
 //     and feeds the 7 output rows it overlaps: 7 x SX accumulators in a statically rotated register ring (slot = (row phase + j + 1)
-//     mod 7), 49*SX packed FMAs (FFMA2) per input row against SX+6 loads -- the tap loop is >90 % FMA-pipe instructions.
+//     mod 7), 49*SX FMA pairs per input row against SX+6 loads -- the tap loop is >90 % FMA-pipe instructions.
 //   * one producer warp streams the input rows of the band into a shared-memory ring with cp.async.bulk.tensor (4-D fp32 map of the
 //     NHWC residual stream, box = [channels, NS*SX+6 pixels, 1 row]): out-of-image columns are zero-filled by the TMA unit (the
 //     conv padding costs nothing), rows above / below the image are skipped on both sides, and the copy of row i+k is in flight
-//     while row i is consumed -- the strip kernels this replaces re-loaded a 7 x 14 window per 8 outputs straight from L1/L2 and
-//     stalled on every one of them (profiles/r1_cnx_kernels_ncu.md: long scoreboard 40 %, 93 M instructions for 19 M FFMA2).
+//     while row i is consumed -- the strip kernels re-load a 7 x 14 window per 8 outputs straight from L1/L2 and stall on every
+//     one of them.
 //   * a finished output row is normalised in registers: the per-pixel sums over the channel pairs are reduced with a halving
 //     butterfly over 16-lane segments, combined across the segments through a few floats of shared memory (one named barrier of the
 //     compute warps per row, double-buffered partials), one-pass variance.
@@ -131,12 +131,12 @@ dwconv7_ln_ring_kernel(const __grid_constant__ CUtensorMap tmX, int B, int H, in
       constexpr int SL = (PH + 7) % 7;
       if (rowok && i < R) {
 #pragma unroll
-        for (int p = 0; p < SX; ++p) acc[SL][p] = __ffma2_rn(cur[p], WGT(0), bias);
+        for (int p = 0; p < SX; ++p) acc[SL][p] = f2fma(cur[p], WGT(0), bias);
 #pragma unroll
         for (int k = 1; k < 7; ++k) {
           const float2 wk = WGT(k);
 #pragma unroll
-          for (int p = 0; p < SX; ++p) acc[SL][p] = __ffma2_rn(cur[p + k], wk, acc[SL][p]);
+          for (int p = 0; p < SX; ++p) acc[SL][p] = f2fma(cur[p + k], wk, acc[SL][p]);
         }
       } else {
 #pragma unroll
@@ -154,7 +154,7 @@ dwconv7_ln_ring_kernel(const __grid_constant__ CUtensorMap tmX, int B, int H, in
           for (int j = 0; j < 6; ++j) {
             const float2 wk = WGT((6 - j) * 7 + k);
 #pragma unroll
-            for (int p = 0; p < SX; ++p) acc[(PH + j + 1) % 7][p] = __ffma2_rn(cur[p + k], wk, acc[(PH + j + 1) % 7][p]);
+            for (int p = 0; p < SX; ++p) acc[(PH + j + 1) % 7][p] = f2fma(cur[p + k], wk, acc[(PH + j + 1) % 7][p]);
           }
       } else {
 #pragma unroll
@@ -165,7 +165,7 @@ dwconv7_ln_ring_kernel(const __grid_constant__ CUtensorMap tmX, int B, int H, in
             for (int k = 0; k < 7; ++k) {
               const float2 wk = WGT((6 - j) * 7 + k);
 #pragma unroll
-              for (int p = 0; p < SX; ++p) acc[(PH + j + 1) % 7][p] = __ffma2_rn(cur[p + k], wk, acc[(PH + j + 1) % 7][p]);
+              for (int p = 0; p < SX; ++p) acc[(PH + j + 1) % 7][p] = f2fma(cur[p + k], wk, acc[(PH + j + 1) % 7][p]);
             }
           }
         }

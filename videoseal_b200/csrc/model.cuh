@@ -215,8 +215,8 @@ inline void launch_dw_ring_t(const DwRingOp& op, cudaStream_t st) {
   VSB_CUDA(cudaGetLastError());
 }
 inline bool dw_ring_ok(int C, int H, int ld) {
-  // (the 384-channel instantiation exists and is correct, but at 16 x 16 maps it measured 50 us against 33 us for the whole-row strip
-  //  kernel: one 192-thread block per SM with a 14-step prologue per 8 rows; profiles/r2_history.md)
+  // (the 384-channel instantiation exists and is correct, but at 16 x 16 maps it runs one 192-thread block per SM with a 14-step
+  //  prologue per 8 rows; the whole-row strip kernel handles those maps)
   static const bool all = getenv("VSB_DW_RING_384") != nullptr;
   return ld == C && ((C == 96 && H % 16 == 0) || (C == 192 && H % 16 == 0) || (all && C == 384 && H % 8 == 0));
 }
@@ -471,7 +471,7 @@ class Model {
     VSB_CUDA(cudaSetDevice(dev));
     cudaDeviceProp prop;
     VSB_CUDA(cudaGetDeviceProperties(&prop, dev));
-    if (prop.major != 10) throw Error("libvsb200 is built for sm_100a only (found sm_" + std::to_string(prop.major) + std::to_string(prop.minor) + ")", kErrUnsupported);
+    if (prop.major != 9 || prop.minor != 0) throw Error("libvsb200 is built for sm_90a only (found sm_" + std::to_string(prop.major) + std::to_string(prop.minor) + ")", kErrUnsupported);
     device = dev;
     num_sms = prop.multiProcessorCount;
     if (d.unet_act != 0 || d.unet_norm != 0) throw Error("unsupported card: only BatchNorm+ReLU U-Nets are implemented on the GPU path", kErrUnsupported);
@@ -803,7 +803,7 @@ class Model {
           const long nb = (long)B * (2 * (2 * IH) + 2 * (2 * IH - 2));
           static bool attr = false;
           if (!attr) { VSB_CUDA(cudaFuncSetAttribute(up_border_fix_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kUpFixSmem)); attr = true; }
-          up_border_fix_kernel<<<(unsigned)std::min<long>((nb + kUpFixPPB - 1) / kUpFixPPB, 148L * 3), 256, kUpFixSmem, st>>>(x0, Ci, x1, Ci, B, IH, IH, wk, lw, lb, 1e-6f, u);
+          up_border_fix_kernel<<<(unsigned)std::min<long>((nb + kUpFixPPB - 1) / kUpFixPPB, (long)num_sms * 3), 256, kUpFixSmem, st>>>(x0, Ci, x1, Ci, B, IH, IH, wk, lw, lb, 1e-6f, u);
           VSB_CUDA(cudaGetLastError());
         }, 1, "unet.upborder." + std::to_string(Cout) + "@" + std::to_string(ho)});
       } else {
@@ -841,7 +841,7 @@ class Model {
         pl.steps.push_back(Step{[=](cudaStream_t st) {
           const int ppb = 256 / gthreads;
           const long blocks = (Mo + ppb - 1) / ppb;
-          const unsigned grid = (unsigned)std::min<long>(blocks, 148L * 32);
+          const unsigned grid = (unsigned)std::min<long>(blocks, (long)num_sms * 32);
           if (vpt == 1) ups_gather_ln_kernel<1><<<grid, 256, 0, st>>>(ytap, B, IH, IH, Cc, lw, lb, 1e-6f, u, Cc);
           else ups_gather_ln_kernel<2><<<grid, 256, 0, st>>>(ytap, B, IH, IH, Cc, lw, lb, 1e-6f, u, Cc);
           VSB_CUDA(cudaGetLastError());
@@ -884,7 +884,7 @@ class Model {
       float *wk = stem_wk, *sb = stem_b, *lw = stem_lnw, *lb = stem_lnb;
       pl.steps.push_back(Step{[=](cudaStream_t st) {
         const long npix = (long)B * OH * OH;
-        const int grid = (int)std::min<long>((npix + 7) / 8, 148L * 16);
+        const int grid = (int)std::min<long>((npix + 7) / 8, (long)num_sms * 16);
         stem_ln_kernel<<<grid, 256, (size_t)8 * (48 + Cc) * sizeof(float), st>>>(plp->in_imgs, B, S, S, OH, OH, st_, wk, sb, lw, lb, Cc, x, ldo);
         VSB_CUDA(cudaGetLastError());
       }, 1, "cnx.stem_ln." + std::to_string(C) + "@" + std::to_string(hs)});
@@ -897,7 +897,7 @@ class Model {
       __half* patches = pl.pool.alloc_n<__half>(M * 64);
       pl.steps.push_back(Step{[=](cudaStream_t st) {
         const long total = M * 4;
-        const int grid = (int)std::min<long>((total + 255) / 256, 148L * 32);
+        const int grid = (int)std::min<long>((total + 255) / 256, (long)num_sms * 32);
         stem_im2col_kernel<<<grid, 256, 0, st>>>(plp->in_imgs, B, S, S, OH, OH, st_, patches);
         VSB_CUDA(cudaGetLastError());
       }, 1, "cnx.stem_im2col"});
@@ -953,7 +953,7 @@ class Model {
           float *lw = ds[s - 1].lnw, *lb = ds[s - 1].lnb;
           const float* xin = x;
           pl.steps.push_back(Step{[=](cudaStream_t st) {
-            const int grid = (int)std::min<long>((Mp + 7) / 8, 148L * 16);
+            const int grid = (int)std::min<long>((Mp + 7) / 8, (long)num_sms * 16);
             ln_rows_kernel<<<grid, 256, 0, st>>>(xin, Mp, Cv, Cvp, lw, lb, 1e-6f, xn, Cvp);
             VSB_CUDA(cudaGetLastError());
           }, 1, "cnx.ln_rows"});
@@ -1014,9 +1014,9 @@ class Model {
 #define VSB_DWC(CC, ST, FR, SPB, NGR, RPB) dwconv7_ln_c_kernel<CC, ST, FR><<<(unsigned)(((NGR) + (SPB) - 1) / (SPB)), (SPB) * (CC) / 2, \
     (size_t)(SPB) * (ST) * (CC) * sizeof(float), st>>>(xin, B, H, H, dww, dwb, lw, lb, a, Cc, SPB, (int)(NGR), RPB)
             {
-              // rows per block: 1.  Walking 2-4 consecutive rows per block (L1 reuse of the 7-row input window) was measured
-              // SLOWER (96@64: 148 -> 228 us, 192@32: 58 -> 87 us): the kernel is latency-bound and fewer, longer blocks with
-              // two block barriers per row hide less of it; VSB_DW_RPB re-enables the experiment
+              // rows per block: 1.  Walking 2-4 consecutive rows per block (L1 reuse of the 7-row input window) gives fewer,
+              // longer blocks with two block barriers per row, which hide less of this latency-bound kernel's stalls;
+              // VSB_DW_RPB selects it
               int rpb = 1;
               if (const char* e = getenv("VSB_DW_RPB")) { const int r2 = atoi(e); if (r2 > 0 && H % r2 == 0) rpb = r2; }
               // narrow maps: one strip = the whole row, so no column is ever out of the image
@@ -1062,7 +1062,7 @@ class Model {
             // enough row-slabs per sample to fill the GPU (~8 blocks per SM)
             static bool attr = false;
             if (!attr) { VSB_CUDA(cudaFuncSetAttribute(grn_apply_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr = true; }
-            int slabs = std::max(1, std::min(rows_per_sample, (148 * 8 + B - 1) / B));
+            int slabs = std::max(1, std::min(rows_per_sample, (num_sms * 8 + B - 1) / B));
             grn_apply_kernel<<<B * slabs, 256, 2 * K4 * sizeof(float), st>>>(g, rows_per_sample, K4, K4, stats, stats_next, gamma, slabs, part_rows);
             VSB_CUDA(cudaGetLastError());
           }, 1, "cnx.grn_apply." + std::to_string(C) + "@" + std::to_string(hs)});
@@ -1277,7 +1277,7 @@ class Model {
       VSB_CUDA(cudaEventRecord(ev_in[k], s_in));
       VSB_CUDA(cudaStreamWaitEvent(s_cmp, ev_in[k], 0));
       const long npx = (long)n * plane;
-      const unsigned blocks = (unsigned)std::min<long>((npx + 255) / 256, 148L * 16);
+      const unsigned blocks = (unsigned)std::min<long>((npx + 255) / 256, (long)num_sms * 16);
       u8hwc_to_f32chw_kernel<<<blocks, 256, 0, s_cmp>>>(in8 + (size_t)f0 * fpx, imgs + (size_t)f0 * fpx, npx, plane);
       g_launches += 1;
       const float* det_in = imgs + (size_t)f0 * fpx;

@@ -495,8 +495,8 @@ __global__ void __launch_bounds__(256) up_border_fix_kernel(const __half* __rest
   // the block keeps its weights and walks over groups of PPB border pixels
   for (int q0 = (int)blockIdx.x * PPB; q0 < total; q0 += (int)gridDim.x * PPB) {
   __syncthreads();   // U of the previous group has been consumed (and Ws is complete on the first pass)
-  // (a two-pass variant that issues all 36 loads of a thread first was measured SLOWER, 232 vs 168 us: 178 registers -> one block per SM;
-  //  the kernel is bound by the shared-memory reads of its fp32 MAC loop, not by these loads - profiles/r2_history.md)
+  // (a two-pass variant that issues all 36 loads of a thread first needs 178 registers -> one block per SM; the kernel is bound by the
+  //  shared-memory reads of its fp32 MAC loop, not by these loads)
   for (int it = threadIdx.x; it < PPB * 9 * 16; it += 256) {
     const int g4 = it & 15, tap = (it >> 4) % 9, pp = it / 144;
     const int q = q0 + pp;
@@ -642,7 +642,7 @@ __global__ void __launch_bounds__(256) stem_ln_kernel(const float* __restrict__ 
 // x: NHWC fp32 [B, H, W, C] (pixel pitch ldx).  One block = one strip of kDwStrip output pixels along x; each thread owns
 // a channel pair and slides over the 7 x (strip+6) input window; pre-LN results go to smem, then LN per pixel by warps.
 constexpr int kDwStrip = 8;
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return __ffma2_rn(a, b, c); }   // Blackwell packed fp32 FMA
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return f2fma(a, b, c); }
 // K4 for arbitrary (even) widths, used for the proportional chunkyseal trunk (362 / 724 / 1448 / 2896 channels on 127 / 63 / 31 /
 // 15 pixel maps): one block per strip of kDwStrip output pixels; the threads LOOP over the channel pairs (C/2 may exceed the
 // block size) and the LayerNorm stage re-reads the pre-LN strip from shared memory instead of holding it in registers.
@@ -713,8 +713,8 @@ __global__ void __launch_bounds__(512) dwconv7_ln_wide_kernel(const float* __res
 }
 
 // K4, fixed-width variant used for the ConvNeXt trunk widths (96/192/384/768).  Same mapping as above, but written around
-// the instruction count: the generic kernel spent 91 % of its 4300 instructions per thread on 64-bit address arithmetic,
-// bounds tests and the divergence bookkeeping of branchy conditional loads (profiles/r1_history.md).  Here C is a template
+// the instruction count: the generic kernel spends most of its instructions on 64-bit address arithmetic, bounds tests and
+// the divergence bookkeeping of branchy conditional loads.  Here C is a template
 // constant, so every input and weight load is `base + immediate`; rows advance by one pointer add; interior strips take a
 // path with no predicates at all and edge strips use a single predicated load per tap column (inline PTX, no branches).
 template <int OFF>
@@ -898,8 +898,9 @@ __global__ void __launch_bounds__(256) grn_scale_kernel(float* __restrict__ stat
 // K2d: GRN (common.py:166-169) applied in place on the fp16 pwconv1 output, fused with the statistics -> multiplier step:
 //   Gx = sqrt(stats[b,k]);  Nx = Gx / (mean_k Gx + 1e-6);  g[m,k] *= gamma[k] * Nx + 1     (beta is folded into pwconv2's bias)
 // One block per (sample, row-slab); the per-sample mean is recomputed by every block (K <= 3072 values).  `stats_next` (the
-// ping-pong buffer the NEXT block's pwconv1 accumulates into) is cleared here.  For all but the first stage g fits in the
-// 126 MB L2, so this pass mostly runs out of L2; pwconv2 is then a plain TMA-fed GEMM.
+// ping-pong buffer the NEXT block's pwconv1 accumulates into) is cleared here.  At batch 64 x 256^2 g is 201 / 100 / 50 / 25 MB in
+// the four stages, so on the H100's 50 MB L2 only the last stage's pass runs out of L2 and the others stream g from HBM (one
+// read + one write of g, against the pwconv2 GEMM that reads it again); pwconv2 is then a plain TMA-fed GEMM.
 // part_rows > 0: `stats` holds part_rows partial rows per sample ([B * part_rows][K], written by the pwconv1 epilogue warps without
 // atomics).  They are added here in a FIXED order (so the result does not depend on the order in which the tiles finished): 128-bit
 // loads, 8 rows in flight per thread, and two row groups per column when the block has the threads for it (combined lower rows first).

@@ -11,8 +11,6 @@
 //                            over 4 tiles per block; separable 5x5 / Sobel sums and jnd_value in packed fp32, SFU transcendentals.
 //       jnd_blend2_kernel    the same arithmetic with per-thread loads: widths that are not multiples of 4, unaligned tensors,
 //                            anti-aliased delta down-scale, frames smaller than a TMA box.
-// Measured (B200, 32 x 3x768x768, profiles/r2_pointwise_ncu.md): resize 63 us = 0.61, blend + preds_w 119 us = 0.69 of the measured
-// HBM copy bandwidth; DRAM traffic = algorithmic bytes.
 #pragma once
 #include "conv_gemm.cuh"
 #include "pointwise.cuh"
@@ -54,8 +52,8 @@ __global__ void __launch_bounds__(256) resize_sep_kernel(const float* __restrict
     fence_barrier_init();
   }
   __syncthreads();
-  // vec (IW % 4 == 0, 16-byte aligned planes): a round is ONE bulk copy issued by thread 0 (the first version's cp.async loop cost
-  // ~70 instructions per thread and round for three 16-byte requests: profiles/r2_final pointwise capture), kRsStages - 1 rounds in flight.
+  // vec (IW % 4 == 0, 16-byte aligned planes): a round is ONE bulk copy issued by thread 0 instead of a cp.async loop in every thread,
+  // kRsStages - 1 rounds in flight.
   // otherwise: 4-byte cp.async by every thread, one round in flight.
   const int depth = vec ? kRsStages - 1 : 1;
   auto issue = [&](int rd) {
@@ -79,8 +77,7 @@ __global__ void __launch_bounds__(256) resize_sep_kernel(const float* __restrict
     }
   };
   // OW <= 256 (every card: processing size 256): a thread owns ONE output column for the whole block, so its taps are loaded once
-  // (ncu of the per-round version, profiles/r2t: 2116 warp instructions per warp of which 534 were LDS + FFMA; 81 LDG of the same
-  // weights every round, 214 ISETP + 117 BRA of row / column predicates, 310 IMAD of addresses)
+  // instead of every round, and the row / column predicates and addresses are computed once
   const bool single = MAXT > 0 && OW <= 256;
   const bool act = (int)threadIdx.x < OW;
   int xs1 = 0;
@@ -229,11 +226,9 @@ __device__ __forceinline__ float jnd_value(float la_sum, float gx, float gy) {
 //     VD_j = row j+1 - row j+3;
 //   then per pixel  la = sum_5 V5 + sum_3 V3 - 2 centre,  gx = VS[x+1] - VS[x-1],  gy = VD[x-1] + 2 VD[x] + VD[x+1]
 //   (the 5x5 kernel of modules/jnd.py:37-43 is ones(5,5) + ones(3,3) - 2 delta; Sobel pair jnd.py:44-53).
-__device__ __forceinline__ float2 f2add(float2 a, float2 b) { return __fadd2_rn(a, b); }
-__device__ __forceinline__ float2 f2sub(float2 a, float2 b) { return __ffma2_rn(b, make_float2(-1.f, -1.f), a); }
+__device__ __forceinline__ float2 f2sub(float2 a, float2 b) { return f2fma(b, make_float2(-1.f, -1.f), a); }
 __device__ __forceinline__ float2 f2s(float v) { return make_float2(v, v); }
-// jnd_value of two pixels with Blackwell's packed fp32 arithmetic (add / mul / fma .f32x2): 12 packed + 8 SFU + 8 scalar
-// instructions per pair instead of 2 x 26.  Same operations in the same order as jnd_value, except that hi's (la0 - 127) * 3/128 + 3
+// jnd_value of two pixels on float2 pairs (add / mul / fma per component).  Same operations in the same order as jnd_value, except that hi's (la0 - 127) * 3/128 + 3
 // is one FMA with the constant folded (1 rounding less).
 __device__ __forceinline__ float2 jnd_value2(float2 la_sum, float2 gx, float2 gy) {
   const float2 la0 = f2mul(la_sum, f2s(1.f / 32.f));
@@ -637,9 +632,8 @@ __global__ void __launch_bounds__(256, 3) jnd_blend2_kernel(const BlendParams p)
 // axis): a block walks kB3NT vertically adjacent 128 x 16 tiles.  ONE TMA box per tile brings the raw RGB tile with its 2-pixel
 // halo ([3][20][136] floats at (x0 - 4, y0 - 2); the engine zero-fills what lies outside the image, which is exactly the zero padding of
 // the reference's conv2d), a second one the delta tile at processing resolution; both land in the other half of a double buffer while
-// the current tile is computed.  ncu of the load-then-compute kernel above (profiles/r2q): 1316 warp instructions per warp, of which
-// 291 were the predicated halo / image loads and 142 per-block set-up, 53 % issue utilisation with 22 % of the samples at the barrier
-// behind the loads; here the loads cost one instruction per tile and the set-up is amortised over kB3NT tiles.
+// the current tile is computed.  Unlike the load-then-compute kernel above, the loads cost one instruction per tile and the per-block
+// set-up is amortised over kB3NT tiles.
 constexpr int kB3NT = 4;
 constexpr int kB3RAW = 3 * (kB2TH + 4) * kB2LP;             // floats of one raw tile (32 640 B, a multiple of 128)
 constexpr int kB3DW = kB2DW + 4;                            // delta tile pitch: the box starts at a 16-byte aligned source column (TMA faults otherwise)

@@ -1,5 +1,5 @@
 // libvsb200.so: the single translation unit behind include/vsb200.h.
-//   nvcc -std=c++17 -O3 -lineinfo -gencode arch=compute_100a,code=sm_100a -shared -Xcompiler -fPIC vsb200.cu -o libvsb200.so
+//   nvcc -std=c++17 -O3 -lineinfo -gencode arch=compute_90a,code=sm_90a -shared -Xcompiler -fPIC vsb200.cu -o libvsb200.so
 #include "model.cuh"
 
 using namespace vsb;

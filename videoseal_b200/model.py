@@ -186,7 +186,7 @@ class Videoseal(nn.Module):
     def _handle(self):
         dev = self.device
         if dev.type != "cuda":
-            raise RuntimeError("videoseal_b200 runs on an NVIDIA B200 (sm_100a) only: call model.to('cuda') first; "
+            raise RuntimeError("videoseal_b200 runs on an NVIDIA H100 (sm_90a) only: call model.to('cuda') first; "
                                "there is no CPU fallback")
         idx = dev.index if dev.index is not None else torch.cuda.current_device()
         if self._native is not None and self._native[0] == idx:

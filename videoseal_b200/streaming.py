@@ -236,7 +236,7 @@ def main(argv=None):
     """python -m videoseal_b200.streaming --input in.mp4 --output_dir outputs  (inference_streaming.py:167-200)"""
     import argparse
     import os
-    ap = argparse.ArgumentParser(description="streaming video watermarking on the B200 backend")
+    ap = argparse.ArgumentParser(description="streaming video watermarking on the H100 (CUDA) backend")
     ap.add_argument("--input", required=True)
     ap.add_argument("--output_dir", default="outputs")
     ap.add_argument("--model", default="videoseal")
