@@ -135,15 +135,15 @@ int64_t vsb_profile_read(char* buf, int64_t capacity);
 int64_t vsb_debug_get_tensor(vsb_model* m, const char* name, float* host_out, int64_t capacity, int64_t* shape4);
 /* standalone conv/GEMM on the wgmma kernels for unit tests: see tests/test_conv_gemm_gpu.py */
 typedef struct vsb_conv_test {
-  int32_t loader;            /* 0 TMA per tap, 1 gather conv, 2 halo bilinear-x2+reflect (UBlock), 3 gather GRN-scale, 4 halo conv3x3 */
+  int32_t loader;            /* 0 TMA per tap, 1 gather conv, 4 halo conv3x3, 5 direct 3x3 ring conv */
   int32_t B, IH, IW, C0, C1; /* input NHWC fp16 [B,IH,IW,C0] (+ optional second source [.., C1]) */
   int32_t R, S, stride, pad, pad_mode;
   int32_t N;                 /* C_out; weights fp16 [N][R*S*(C0+C1)] */
   int32_t epi, act;          /* 0 affine / 1 LN;  0 none 1 relu 2 gelu */
-  int32_t rows_per_sample;   /* GRN / scale */
+  int32_t rows_per_sample;   /* GRN */
   int32_t block_n;           /* 0 = auto */
   const void* src0; const void* src1; const void* weights;
-  const float* bias; const void* resid16; const float* resid32; const float* a_scale;
+  const float* bias; const void* resid16; const float* resid32;
   const float* ln_w; const float* ln_b;
   const float* outc_w; const float* outc_b; int32_t n_out;
   void* out16; float* out32; float* delta; float* grn_stats;

@@ -8,7 +8,7 @@ import torch.nn.functional as F
 
 from videoseal_b200 import _lib
 
-LD_TMA, LD_GCONV, LD_GUPS, LD_GSCALE, LD_HALO, LD_DIRECT = 0, 1, 2, 3, 4, 5
+LD_TMA, LD_GCONV, LD_HALO, LD_DIRECT = 0, 1, 4, 5
 
 CASES = {
     # name: dict(loader, B, IH, IW, C0, C1, R, S, stride, pad, pad_mode, N, extras...)
@@ -43,14 +43,10 @@ CASES = {
     "direct1_wrap":    dict(loader=LD_DIRECT, B=96, IH=128, IW=128, C0=16, N=16, R=1, S=1, bias=True, act=1, out="f16"),
     "direct_ringwrap": dict(loader=LD_DIRECT, B=96, IH=128, IW=128, C0=16, N=16, R=3, S=3, pad=1, bias=True, act=1, resid16=True, out="f16"),
     "direct_wrap_c64": dict(loader=LD_DIRECT, B=80, IH=64, IW=64, C0=64, N=64, R=3, S=3, pad=1, bias=True, act=1, out="f16"),
-    "gups_c16":        dict(loader=LD_GUPS, B=1, IH=64, IW=64, C0=16, C1=16, N=16, R=3, S=3, epi=1, act=1, out="f16"),
     "gconv_s2":        dict(loader=LD_GCONV, B=2, IH=64, IW=64, C0=16, N=32, R=3, S=3, stride=2, pad=1, bias=True, out="f16"),
     "gconv_patch":     dict(loader=LD_GCONV, B=2, IH=16, IW=16, C0=96, N=192, R=2, S=2, stride=2, pad=0, bias=True, out="f32"),
     "gconv_reflect":   dict(loader=LD_GCONV, B=3, IH=8, IW=8, C0=64, N=64, R=3, S=3, stride=1, pad=1, pad_mode=1, out="f32"),
     "gconv_odd":       dict(loader=LD_GCONV, B=1, IH=15, IW=15, C0=72, N=40, R=3, S=3, stride=1, pad=1, pad_mode=1, out="f32"),
-    "gups_ln":         dict(loader=LD_GUPS, B=2, IH=16, IW=16, C0=32, C1=32, N=32, R=3, S=3, epi=1, act=1, out="f16"),
-    "gups_big":        dict(loader=LD_GUPS, B=1, IH=32, IW=32, C0=384, C1=384, N=64, R=3, S=3, epi=1, act=1, out="f16"),
-    "gscale":          dict(loader=LD_GSCALE, B=2, IH=8, IW=8, C0=384, N=96, R=1, S=1, bias=True, resid32=True, scale=True, rps=64, out="f32"),
     "gelu_grn":        dict(loader=LD_TMA, B=1, IH=1, IW=512, C0=96, N=384, R=1, S=1, bias=True, act=2, grn=True, rps=256, out="f16"),
     "gelu_grn_rag":    dict(loader=LD_TMA, B=1, IH=1, IW=450, C0=96, N=384, R=1, S=1, bias=True, act=2, grn=True, rps=225, out="f16"),
     # chunkyseal's proportional trunk: widths 362 / 724 / 1448 (not multiples of 8 / 16) in rows padded to 8 elements, odd maps
@@ -76,32 +72,17 @@ def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else None
 
 
-def reference(cfg, x0, x1, w, bias, resid, scale, lnw, lnb):
+def reference(cfg, x0, x1, w, bias, resid, lnw, lnb):
     """fp32 torch reference on the GPU. x0/x1 NHWC fp16; w [N, R, S, Ct] fp16."""
-    ld = cfg["loader"]
-    R, S = cfg["R"], cfg["S"]
     xin = x0.float().permute(0, 3, 1, 2)
     if x1 is not None:
         xin = torch.cat([xin, x1.float().permute(0, 3, 1, 2)], dim=1)
     wt = w.float().permute(0, 3, 1, 2).contiguous()          # [N, Ct, R, S]
-    if ld == LD_GSCALE:
-        B, H, W_, K = x0.shape
-        a = x0.float().reshape(B, H * W_, K) * scale[:, None, :]
-        # the kernel rounds the scaled operand back to fp16 before the MMA
-        a = a.half().float()
-        y = a.reshape(-1, K) @ w.float().reshape(cfg["N"], K).t()
-        y = y.reshape(B, H, W_, cfg["N"]).permute(0, 3, 1, 2)
-    elif ld == LD_GUPS:
-        up = F.interpolate(xin, scale_factor=2, mode="bilinear", align_corners=False)
-        up = up.half().float()                                 # kernel rounds the interpolated operand to fp16
-        up = F.pad(up, (1, 1, 1, 1), mode="reflect")
-        y = F.conv2d(up, wt)
-    else:
-        pad = cfg.get("pad", 0)
-        if cfg.get("pad_mode", 0) == 1 and pad:
-            xin = F.pad(xin, (pad,) * 4, mode="reflect")
-            pad = 0
-        y = F.conv2d(xin, wt, stride=cfg.get("stride", 1), padding=pad)
+    pad = cfg.get("pad", 0)
+    if cfg.get("pad_mode", 0) == 1 and pad:
+        xin = F.pad(xin, (pad,) * 4, mode="reflect")
+        pad = 0
+    y = F.conv2d(xin, wt, stride=cfg.get("stride", 1), padding=pad)
     if cfg.get("epi", 0) == 1:
         u = y.mean(1, keepdim=True)
         s = (y - u).pow(2).mean(1, keepdim=True)
@@ -134,11 +115,8 @@ def run_case(name, seed=0, verbose=False, time_iters=0):
     bias = torch.randn(N, generator=g).to(dev) if cfg.get("bias") else None
     lnw = (1 + 0.1 * torch.randn(N, generator=g)).to(dev) if cfg.get("epi", 0) == 1 else None
     lnb = (0.1 * torch.randn(N, generator=g)).to(dev) if cfg.get("epi", 0) == 1 else None
-    scale = (1 + 0.3 * torch.randn(B, C0, generator=g)).to(dev) if cfg.get("scale") else None
     ld = cfg["loader"]
-    if ld == LD_GUPS:
-        OH, OW = 2 * IH, 2 * IW
-    elif ld == LD_GCONV:
+    if ld == LD_GCONV:
         st, pad = cfg.get("stride", 1), cfg.get("pad", 0)
         OH, OW = (IH + 2 * pad - R) // st + 1, (IW + 2 * pad - S) // st + 1
     else:
@@ -171,7 +149,7 @@ def run_case(name, seed=0, verbose=False, time_iters=0):
     t.loader, t.B, t.IH, t.IW, t.C0, t.C1 = ld, B, IH, IW, C0, C1
     t.R, t.S, t.stride, t.pad, t.pad_mode = R, S, cfg.get("stride", 1), cfg.get("pad", 0), cfg.get("pad_mode", 0)
     t.N, t.epi, t.act, t.rows_per_sample, t.block_n = N, cfg.get("epi", 0), cfg.get("act", 0), cfg.get("rps", 0), cfg.get("block_n", 0)
-    w_dev = halo_layout(w, C0, C1) if ld in (LD_GUPS, LD_HALO) else w
+    w_dev = halo_layout(w, C0, C1) if ld == LD_HALO else w
     if ldw:
         w_p = torch.full((N, ldw), SENT, dtype=torch.float16, device=dev)
         w_p[:, :K] = w.reshape(N, K)
@@ -182,7 +160,7 @@ def run_case(name, seed=0, verbose=False, time_iters=0):
     if ld_out:
         out32_true, out32 = out32, out32_p
     t.resid32 = _ptr(out32) if resid32 is not None else None     # in place, like the ConvNeXt residual stream
-    t.a_scale, t.ln_w, t.ln_b = _ptr(scale), _ptr(lnw), _ptr(lnb)
+    t.ln_w, t.ln_b = _ptr(lnw), _ptr(lnb)
     t.outc_w, t.outc_b, t.n_out = _ptr(outc_w), _ptr(outc_b), n_out
     t.out16, t.out32, t.delta, t.grn_stats = _ptr(out16), _ptr(out32), _ptr(delta), _ptr(stats)
     _lib.check(_lib.lib().vsb_debug_conv(C.byref(t), None))
@@ -206,7 +184,7 @@ def run_case(name, seed=0, verbose=False, time_iters=0):
             torch.cuda.synchronize()
 
     resid = resid16 if resid16 is not None else resid32
-    ref, pre = reference(cfg, x0, x1, w, bias, resid, scale, lnw, lnb)
+    ref, pre = reference(cfg, x0, x1, w, bias, resid, lnw, lnb)
     res = {}
     if ld_out:
         res["pad_untouched"] = bool((out32[..., N:] == SENT).all())

@@ -19,12 +19,8 @@ BIG = {
     "p_halo3_c64":  dict(loader=cc.LD_HALO, B=64, IH=64, IW=64, C0=64, N=64, R=3, S=3, pad=1, bias=True, act=1, resid16=True, out="f16"),
     "p_conv3_c64":  dict(loader=cc.LD_TMA, B=64, IH=64, IW=64, C0=64, N=64, R=3, S=3, pad=1, bias=True, act=1, resid16=True, out="f16"),
     "p_halo3_bott": dict(loader=cc.LD_HALO, B=64, IH=32, IW=32, C0=384, N=384, R=3, S=3, pad=1, bias=True, act=1, resid16=True, out="f16"),
-    "p_up_128_32":  dict(loader=cc.LD_GUPS, B=64, IH=64, IW=64, C0=64, C1=64, N=32, R=3, S=3, epi=1, act=1, out="f16"),
     "p_conv1_bott": dict(loader=cc.LD_TMA, B=64, IH=32, IW=32, C0=384, N=384, R=1, S=1, bias=True, out="f16"),
     "p_pw1_96":     dict(loader=cc.LD_TMA, B=1, IH=1, IW=64 * 4096, C0=96, N=384, R=1, S=1, bias=True, act=2, grn=True, rps=4096, out="f16"),
-    "p_pw2_96":     dict(loader=cc.LD_GSCALE, B=64, IH=64, IW=64, C0=384, N=96, R=1, S=1, bias=True, resid32=True, scale=True, rps=4096, out="f32"),
-    "p_up_64_16":   dict(loader=cc.LD_GUPS, B=64, IH=128, IW=128, C0=32, C1=32, N=16, R=3, S=3, epi=1, act=1, out="f16"),
-    "p_up_768_64":  dict(loader=cc.LD_GUPS, B=64, IH=32, IW=32, C0=384, C1=384, N=64, R=3, S=3, epi=1, act=1, out="f16"),
     "p_pw1_384":    dict(loader=cc.LD_TMA, B=1, IH=1, IW=64 * 256, C0=384, N=1536, R=1, S=1, bias=True, act=2, grn=True, rps=256, out="f16"),
     "p_pw2_384":    dict(loader=cc.LD_TMA, B=1, IH=1, IW=64 * 256, C0=1536, N=384, R=1, S=1, bias=True, resid32=True, out="f32"),
     "p_pw2_96t":    dict(loader=cc.LD_TMA, B=1, IH=1, IW=64 * 4096, C0=384, N=96, R=1, S=1, bias=True, resid32=True, out="f32"),

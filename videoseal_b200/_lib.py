@@ -6,7 +6,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# VSB200_LIB selects another build of the same sources (e.g. one without -DVSB_PDL, see __graft_entry__.py)
+# VSB200_LIB selects another build of the library (e.g. one compiled from an earlier revision, to compare outputs)
 LIB_PATH = os.environ.get("VSB200_LIB") or os.path.join(_HERE, "libvsb200.so")
 
 EXPORTS = [
@@ -36,7 +36,7 @@ class ConvTest(C.Structure):
         ("R", C.c_int32), ("S", C.c_int32), ("stride", C.c_int32), ("pad", C.c_int32), ("pad_mode", C.c_int32),
         ("N", C.c_int32), ("epi", C.c_int32), ("act", C.c_int32), ("rows_per_sample", C.c_int32), ("block_n", C.c_int32),
         ("src0", C.c_void_p), ("src1", C.c_void_p), ("weights", C.c_void_p),
-        ("bias", C.c_void_p), ("resid16", C.c_void_p), ("resid32", C.c_void_p), ("a_scale", C.c_void_p),
+        ("bias", C.c_void_p), ("resid16", C.c_void_p), ("resid32", C.c_void_p),
         ("ln_w", C.c_void_p), ("ln_b", C.c_void_p),
         ("outc_w", C.c_void_p), ("outc_b", C.c_void_p), ("n_out", C.c_int32),
         ("out16", C.c_void_p), ("out32", C.c_void_p), ("delta", C.c_void_p), ("grn_stats", C.c_void_p),

@@ -39,7 +39,6 @@ struct Conv3DirectParams {
   uint32_t plane_stride;    // bytes between 8-channel planes of the ring
   uint32_t w_off, ring_off; // offsets from the 1024-aligned dynamic smem base
   uint32_t w_bytes;
-  int swap_lbo_sbo;         // debugging aid (unit test of the descriptor convention)
   FastDiv fd_rw, fd_hp;
   const __half* x;          // input, dense NHWC fp16
   const __half* wpk;        // weights in core-matrix layout (pack_direct_weights_kernel)
@@ -61,12 +60,6 @@ struct D3Header {
   float ocw[3][64];
 };
 static_assert(sizeof(D3Header) <= kD3XposeOff, "direct conv header");
-
-// no-swizzle K-major operand: core matrices of 8 rows x 16 B; LBO = byte distance between the two core matrices along K,
-// SBO = byte distance between consecutive 8-row groups
-__device__ __forceinline__ uint64_t make_smem_desc_ns(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo >> 4) & 0x3FFF) << 32);
-}
 
 // [N][T*C] (k = tap*C + c, T = 9 or 1 taps) fp16  ->  [tap][C/16][k-half][N/8][8 rows][8 halves]
 __global__ void pack_direct_weights_kernel(const __half* __restrict__ w, int N, int C, int T, __half* __restrict__ out) {
@@ -119,7 +112,7 @@ __global__ void __launch_bounds__(kD3Threads, 1) conv3_direct_kernel(const Conv3
   }
   fence_proxy_async_smem();   // weights were written through the generic proxy, wgmma reads them through the async proxy
   __syncthreads();
-  // (PDL builds) so far only weights / bias / LN parameters were read: the resident-weight copy overlaps the predecessor's tail
+  // so far only weights / bias / LN parameters were read: the resident-weight copy overlaps the predecessor's tail
   pdl_launch_dependents();
   pdl_wait();
 
@@ -202,8 +195,10 @@ __global__ void __launch_bounds__(kD3Threads, 1) conv3_direct_kernel(const Conv3
     const int e = (warp - 4) >> 2, quad = warp & 3;
     const int row = 16 * quad + (lane & 15) + 64 * (lane >> 4);
     float* xp = reinterpret_cast<float*>(smem + kD3XposeOff) + (size_t)(warp - 4) * 32 * kD3XposePitch;
-    const uint32_t a_lbo = p.swap_lbo_sbo ? 128u : p.plane_stride, a_sbo = p.swap_lbo_sbo ? p.plane_stride : 128u;
-    const uint32_t b_lbo = p.swap_lbo_sbo ? 128u : (uint32_t)N * 16u, b_sbo = p.swap_lbo_sbo ? (uint32_t)N * 16u : 128u;
+    // no-swizzle K-major descriptors: LBO = byte distance between the two core matrices along K (next 8 channels), SBO = byte
+    // distance between consecutive 8-row groups (next 8 positions / output channels)
+    const uint32_t a_lbo = p.plane_stride, a_sbo = 128u;
+    const uint32_t b_lbo = (uint32_t)N * 16u, b_sbo = 128u;
     const uint32_t a_lo = (((a_lbo >> 4) & 0x3FFFu) << 16) + (smem_u32(ring) >> 4);
     const uint32_t b_lo = (((b_lbo >> 4) & 0x3FFFu) << 16) + (smem_u32(wsm) >> 4);
     const uint64_t a_hi = (uint64_t)((a_sbo >> 4) & 0x3FFFu) << 32;

@@ -33,9 +33,7 @@ inline int conv3_direct_min_rows(int W, int R = 3) {
 }
 // W = 0: channel-count check only (weight packing time)
 inline bool conv3_direct_ok(int C, int N, int ld_in, int W = 0, int R = 3) {
-  static const bool off = getenv("VSB_NO_DIRECT") != nullptr;
-  static const bool off1 = getenv("VSB_NO_DIRECT1") != nullptr;
-  if (off || (R == 1 && off1) || ld_in != C) return false;
+  if (ld_in != C) return false;
   if (W == 0) return conv3_direct_ring_rows(C, N, 64, R) > 0;
   return W % 8 == 0 && conv3_direct_ring_rows(C, N, W, R) >= conv3_direct_min_rows(W, R);
 }
@@ -66,8 +64,6 @@ inline void setup_conv3_direct(Conv3DirectOp& op, const __half* x, int B, int H,
   p.fd_rw = make_fastdiv(p.rw);
   p.fd_hp = make_fastdiv(p.hp);
   p.wpk = wpk;
-  static const bool swap = getenv("VSB_DIRECT_SWAP") != nullptr;
-  p.swap_lbo_sbo = swap ? 1 : 0;
   p.x = x;
   VSB_CHECK((reinterpret_cast<uintptr_t>(x) & 15) == 0, "direct conv3: input must be 16-byte aligned");
   op.grid = std::min(num_sms, p.n_tiles);
@@ -80,11 +76,7 @@ inline void launch_direct_nkr(const Conv3DirectOp& op, cudaStream_t st) {
     VSB_CUDA(cudaFuncSetAttribute(conv3_direct_kernel<N, KS, R, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr = true;
   }
-#ifdef VSB_PDL
   launch_pdl(conv3_direct_kernel<N, KS, R, MODE>, dim3(op.grid), dim3(kD3Threads), op.smem, st, op.p);
-#else
-  conv3_direct_kernel<N, KS, R, MODE><<<op.grid, kD3Threads, op.smem, st>>>(op.p);
-#endif
   VSB_CUDA(cudaGetLastError());
 }
 template <int N, int KS>

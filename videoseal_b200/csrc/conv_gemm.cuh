@@ -6,17 +6,13 @@
 //                   chunks c with c % (E/4) == w/4
 //   warps E..E+3  : A-tile builders (all loaders except LD_TMA):
 //       LD_HALO_CONV3 : on-chip im2col - the (8+2)x(16+2) input halo of an 8x16 output tile is TMA-loaded ONCE per channel
-//                       chunk (zero fill = conv padding) and the tap tiles are copied smem->smem into the swizzled
-//                       UMMA layout (input pixels cross L2->SM once instead of nine times)
-//       LD_HALO_UPS   : the UBlock's bilinear x2 (align_corners=False) + ReflectionPad2d(1) + virtual skip-concat: a 6x10
-//                       low-resolution halo is TMA-loaded, the 10x18 upsampled+padded halo is built from it in shared
-//                       memory once, then tap tiles are copied as in LD_HALO_CONV3
+//                       chunk (zero fill = conv padding) and the tap tiles are copied smem->smem into the 128-byte-swizzled
+//                       wgmma operand layout (input pixels cross L2->SM once instead of nine times)
 //       LD_GATHER_CONV: generic strided / reflect-padded conv gathered from global memory (stride-2 3x3, k2s2 patchify,
 //                       reflect-padded head conv)
-//       LD_GATHER_SCALE: A[m,k] = G[m,k] * scale[sample(m), k]  (ConvNeXt pwconv2 with the GRN factor folded in)
 //
 //   next 8 warps  : two MMA warpgroups; warpgroup h issues the wgmma of rows [64h, 64h + 64) of the tile
-//   last warp     : TMA producer (weights unless resident; activations for LD_TMA; input halo tiles for LD_HALO_*)
+//   last warp     : TMA producer (weights unless resident; activations for LD_TMA; input halo tiles for LD_HALO_CONV3)
 //
 // GEMM view: D[M = output pixels, N = C_out] = A[M, K = taps*C_in] * W[N, K]^T, fp16 operands, fp32 accumulation.
 // BLOCK_M = 128, BLOCK_N <= 128.  The MMA warpgroups hand each finished accumulator round to the epilogue through one
@@ -32,7 +28,7 @@
 
 namespace vsb {
 
-enum : int { LD_TMA = 0, LD_GATHER_CONV = 1, LD_HALO_UPS = 2, LD_GATHER_SCALE = 3, LD_HALO_CONV3 = 4 };
+enum : int { LD_TMA = 0, LD_GATHER_CONV = 1, LD_HALO_CONV3 = 4 };
 enum : int { EPI_AFFINE = 0, EPI_LN = 1 };
 enum : int { ACT_NONE = 0, ACT_RELU = 1, ACT_GELU = 2 };
 
@@ -47,7 +43,7 @@ constexpr int kEpiWarps = 8;       // LD_TMA; the loaders with 4 builder warps h
 constexpr int kMmaThreads = 256;    // two MMA warpgroups
 constexpr int kHeaderBytes = 11264;  // barriers | bias x2 | LN w,b / outc rows | outc partials (3 x [128][3])
 constexpr int kHaloTW = 16, kHaloTH = 8;
-constexpr int kHaloW = kHaloTW + 2, kHaloH = kHaloTH + 2;   // 18 x 10 input (or upsampled) halo of an 8x16 output tile
+constexpr int kHaloW = kHaloTW + 2, kHaloH = kHaloTH + 2;   // 18 x 10 input halo of an 8x16 output tile
 
 // division by a runtime constant as multiply-high + shift (valid for 0 <= n < 2^31); the host precomputes (mul, shr)
 struct FastDiv {
@@ -81,19 +77,20 @@ struct ConvGemmParams {
   // ---- halo loaders: the input is cut into `c_blocks` channel chunks of `cc` (= min(C, 64)) channels, the first c0_blocks
   //      from source 0; each chunk contributes kb_per_c K-blocks of 64 (K order inside a chunk: (tap, channel), zero padded)
   int c0_blocks, cc, kb_per_c;
-  uint32_t halo_bytes /*TMA box bytes*/, halo_stride /*buffer pitch*/, halo_off, u_off;
-  int halo_bufs;                  // ring depth of the halo tiles (prefetch distance of the producer)
+  uint32_t halo_bytes /*TMA box bytes*/, halo_stride /*buffer pitch*/, halo_off;
   // ---- residual prefetch ring (thread-private slots)
   uint32_t resid_off, resid_stride;
   int resid_depth;
   int resid_direct;               // 1: no shared-memory ring, the epilogue reads the fp16 residual straight from global memory (long-K layers:
                                   //    their epilogue is hidden behind the main loop, the 48 KB buy one more TMA pipeline stage)
+  // (declared here, not with the halo fields: this keeps the 8-byte pairing of the int fields above, without which ptxas gives
+  //  the gather and halo kernels more stack)
+  int halo_bufs;                  // ring depth of the halo tiles (prefetch distance of the producer)
   // ---- gather loaders (NHWC fp16 sources; K order = (r, s, c) with c over the virtual concat [src0 | src1])
   const __half* src0;
   const __half* src1;
   int C0, C1, ld0, ld1, IH, IW, OH, OW, stride, pad_mode /*0 zero, 1 reflect*/, Ktot;
-  const float* a_scale;  // LD_GATHER_SCALE: [num_samples, ld_scale] fp32
-  int rows_per_sample, ld_scale;
+  int rows_per_sample;            // GEMM rows per sample (GRN statistics, per-sample weights)
   int b_sample_rows;              // > 0: per-sample weights [samples][N][K] (GRN folded into pwconv2); = N
   FastDiv fd_tps;                 // M tiles per sample
   // ---- epilogue
@@ -118,7 +115,6 @@ struct ConvGemmParams {
 // own).  Abramowitz-Stegun 7.1.25 would need rcp AND ex2 per element, and its error is 2.5e-5.
 constexpr float kGeluQ0 = -1.1510894298553467f, kGeluQ1 = -0.4592657685279846f, kGeluQ2 = -0.05254320427775383f,
                 kGeluQ3 = 0.007386638317257166f, kGeluQ4 = -0.0005183160537853837f;
-__device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float ex2_approx(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float gelu_erf(float x) {
   const float ax = fabsf(x);
@@ -165,25 +161,6 @@ __device__ __forceinline__ int reflect_idx(int i, int n) {
   return i;
 }
 
-// separable bilinear tap: (wy*(wx*a + (1-wx)*b) + (1-wy)*(wx*c + (1-wx)*d)) on 8 packed halves
-__device__ __forceinline__ uint4 lerp2x2_h8(uint4 a, uint4 b, uint4 c, uint4 d, float wx, float wy) {
-  const __half2 hx = __float2half2_rn(wx), hx1 = __float2half2_rn(1.f - wx);
-  const __half2 hy = __float2half2_rn(wy), hy1 = __float2half2_rn(1.f - wy);
-  const __half2* pa = reinterpret_cast<const __half2*>(&a);
-  const __half2* pb = reinterpret_cast<const __half2*>(&b);
-  const __half2* pc = reinterpret_cast<const __half2*>(&c);
-  const __half2* pd = reinterpret_cast<const __half2*>(&d);
-  uint4 o;
-  __half2* po = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const __half2 t0 = __hfma2(hx, pa[i], __hmul2(hx1, pb[i]));
-    const __half2 t1 = __hfma2(hx, pc[i], __hmul2(hx1, pd[i]));
-    po[i] = __hfma2(hy, t0, __hmul2(hy1, t1));
-  }
-  return o;
-}
-
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
 }
@@ -204,7 +181,6 @@ __device__ __forceinline__ void cp_async_wait_pending(int n) {   // wait until a
   }
 }
 template <int NT> __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory"); }
-__device__ __forceinline__ void bld_bar_sync() { asm volatile("bar.sync 2, 128;" ::: "memory"); }
 
 // one row of the shared accumulator tile -> 16 registers
 __device__ __forceinline__ void acc_ld16(const float* src, uint32_t (&r)[16]) {
@@ -306,7 +282,6 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   float* s_dot = reinterpret_cast<float*>(smem + 6144);         // [128][3]
   uint8_t* tiles = smem + kHeaderBytes;
   uint8_t* halo = smem + p.halo_off;
-  uint8_t* ubuf = smem + p.u_off;
   uint8_t* bres = smem + p.bres_off;
   uint8_t* rbuf = smem + p.resid_off;
   float* acc_s = reinterpret_cast<float*>(smem + p.acc_off);
@@ -314,7 +289,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   constexpr uint32_t kNumBuilders = 128;
-  constexpr bool kHalo = (LOADER == LD_HALO_CONV3 || LOADER == LD_HALO_UPS);
+  constexpr bool kHalo = LOADER == LD_HALO_CONV3;
   constexpr int kEpiW = LOADER == LD_TMA ? kEpiWarps : 4;
   constexpr int kEpiThreads = kEpiW * 32;
   constexpr int kEpiSplit = kEpiW / 4;              // warps sharing one 32-row quadrant (interleaved 16-column chunks)
@@ -337,7 +312,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     mbar_init(bres_bar, 1u);
     fence_barrier_init();
     if (LOADER == LD_TMA || kHalo) tma_prefetch_desc(&tmA);
-    if (LOADER == LD_HALO_UPS || (LOADER == LD_TMA && p.c0_blocks != 0)) tma_prefetch_desc(&tmA2);
+    if (LOADER == LD_TMA && p.c0_blocks != 0) tma_prefetch_desc(&tmA2);
     tma_prefetch_desc(&tmB);
     if (p.tma_store) tma_prefetch_desc(&tmO);
   }
@@ -351,7 +326,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     }
   }
   __syncthreads();
-  // (PDL builds) nothing above reads or writes a tensor produced by an earlier kernel: only parameters and weights
+  // nothing above reads or writes a tensor produced by an earlier kernel: only parameters and weights
   pdl_launch_dependents();
   pdl_wait();
 
@@ -384,13 +359,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           for (int c = 0; c < p.c_blocks; ++c) {
             mbar_wait(&hempty_bar[hb], hphase ^ 1u);
             mbar_arrive_expect_tx(&hfull_bar[hb], p.halo_bytes);
-            if (LOADER == LD_HALO_CONV3) {
-              tma_load_4d(&tmA, &hfull_bar[hb], halo + (size_t)hb * p.halo_stride, c * p.cc, cx - 1, cy - 1, cb);
-            } else {
-              const bool s0 = c < p.c0_blocks;
-              tma_load_4d(s0 ? &tmA : &tmA2, &hfull_bar[hb], halo + (size_t)hb * p.halo_stride,
-                          (s0 ? c : c - p.c0_blocks) * p.cc, (cx >> 1) - 1, (cy >> 1) - 1, cb);
-            }
+            tma_load_4d(&tmA, &hfull_bar[hb], halo + (size_t)hb * p.halo_stride, c * p.cc, cx - 1, cy - 1, cb);
             if (++hb == p.halo_bufs) { hb = 0; hphase ^= 1u; }
             if (!p.b_resident) {
               int kcoord = c * p.kb_per_c * 64;
@@ -971,7 +940,6 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     uint32_t phase = 0;
     if (kHalo) {
       const uint32_t pb = (uint32_t)p.cc * 2u;   // bytes per halo pixel
-      const int cpp = p.cc >> 3;                 // 16-byte chunks per halo pixel
       int hb = 0;
       uint32_t hphase = 0;
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
@@ -989,36 +957,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int c = 0; c < p.c_blocks; ++c) {
           mbar_wait(&hfull_bar[hb], hphase);
           const uint8_t* hsrc = halo + (size_t)hb * p.halo_stride;
-          if (LOADER == LD_HALO_UPS) {
-            // phase 1: build the 10 x 18 upsampled + reflect-padded halo (once per channel chunk) from the 6 x 10
-            // low-resolution tile that starts at source pixel (cy/2 - 1, cx/2 - 1)
-            bld_bar_sync();  // everyone is done reading the previous U
-            const int sy0 = (cy >> 1) - 1, sx0 = (cx >> 1) - 1;
-            for (int e = gt; e < kHaloH * kHaloW * cpp; e += 128) {
-              const int ch = e % cpp;
-              const int px = e / cpp;
-              const int hy = px / kHaloW, hx = px - hy * kHaloW;
-              const int uy = reflect_idx(cy + hy - 1, 2 * p.IH);
-              const int ux = reflect_idx(cx + hx - 1, 2 * p.IW);
-              const int iy = uy >> 1, ix = ux >> 1;
-              int ya, yb, xa, xb;
-              float wya, wxa;
-              if (uy & 1) { ya = iy; yb = min(iy + 1, p.IH - 1); wya = 0.75f; }
-              else        { ya = max(iy - 1, 0); yb = iy; wya = 0.25f; }
-              if (ux & 1) { xa = ix; xb = min(ix + 1, p.IW - 1); wxa = 0.75f; }
-              else        { xa = max(ix - 1, 0); xb = ix; wxa = 0.25f; }
-              const uint8_t* base = hsrc + ch * 16;
-              const uint4 v00 = *reinterpret_cast<const uint4*>(base + (size_t)((ya - sy0) * 10 + (xa - sx0)) * pb);
-              const uint4 v01 = *reinterpret_cast<const uint4*>(base + (size_t)((ya - sy0) * 10 + (xb - sx0)) * pb);
-              const uint4 v10 = *reinterpret_cast<const uint4*>(base + (size_t)((yb - sy0) * 10 + (xa - sx0)) * pb);
-              const uint4 v11 = *reinterpret_cast<const uint4*>(base + (size_t)((yb - sy0) * 10 + (xb - sx0)) * pb);
-              *reinterpret_cast<uint4*>(ubuf + (size_t)px * pb + ch * 16) = lerp2x2_h8(v00, v01, v10, v11, wxa, wya);
-            }
-            mbar_arrive(&hempty_bar[hb]);  // low-res tile consumed
-            bld_bar_sync();                // U complete
-            hsrc = ubuf;
-          }
-          // phase 2: tap tiles.  K-block kbi of this chunk holds K indices [64*kbi, 64*kbi+64) of the (tap, channel)
+          // tap tiles.  K-block kbi of this chunk holds K indices [64*kbi, 64*kbi+64) of the (tap, channel)
           // order; 16-byte chunk j covers k = 64*kbi + 8*j -> tap = k / cc, channel offset = k % cc
           const int stage0 = stage;
           const uint32_t phase0 = phase;
@@ -1060,7 +999,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             }
           }
           (void)phase0;
-          if (LOADER == LD_HALO_CONV3) mbar_arrive(&hempty_bar[hb]);
+          mbar_arrive(&hempty_bar[hb]);
           if (++hb == p.halo_bufs) { hb = 0; hphase ^= 1u; }
         }
        }
@@ -1076,16 +1015,10 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int i = 0; i < 8; ++i) {
           const int m = m_tile * kBlockM + rg + 16 * i;      // M < 2^31 (host-checked)
           if (m < p.M) {
-            if (LOADER == LD_GATHER_SCALE) {
-              pb[i] = p.fd_rps.div(m);
-              py[i] = 0;
-              px[i] = m;
-            } else {
-              const int t = p.fd_ow.div(m);
-              px[i] = m - t * p.OW;
-              pb[i] = p.fd_oh.div(t);
-              py[i] = t - pb[i] * p.OH;
-            }
+            const int t = p.fd_ow.div(m);
+            px[i] = m - t * p.OW;
+            pb[i] = p.fd_oh.div(t);
+            py[i] = t - pb[i] * p.OH;
           } else {
             pb[i] = -1; py[i] = 0; px[i] = 0;
           }
@@ -1095,64 +1028,34 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           uint8_t* sa = tiles + (size_t)stage * p.stage_bytes;
           const int k = kb * 64 + j * 8;
           const bool kvalid = k < p.Ktot;
-          if (LOADER == LD_GATHER_SCALE) {
-            uint4 g[8];
+          const int tap = kvalid ? p.fd_ct.div(k) : 0;
+          const int c = k - tap * Ct;
+          const int tr = p.fd_s.div(tap), ts = tap - tr * p.S;
+          const __half* src = (c < p.C0) ? p.src0 : p.src1;
+          const int ld = (c < p.C0) ? p.ld0 : p.ld1;
+          const int cc = (c < p.C0) ? c : c - p.C0;
+          // asynchronous gather: 16-byte cp.async per (row, chunk) with zero fill for padding / tails; the mbarrier
+          // arrival fires when this thread's copies have landed, so the builder runs ahead by the ring depth
 #pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              g[i] = make_uint4(0, 0, 0, 0);
-              if (kvalid && pb[i] >= 0) g[i] = __ldg(reinterpret_cast<const uint4*>(p.src0 + (long)px[i] * p.ld0 + k));
-            }
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              uint4 val = make_uint4(0, 0, 0, 0);
-              if (kvalid && pb[i] >= 0) {
-                const float4 s0 = __ldg(reinterpret_cast<const float4*>(p.a_scale + (long)pb[i] * p.ld_scale + k));
-                const float4 s1 = __ldg(reinterpret_cast<const float4*>(p.a_scale + (long)pb[i] * p.ld_scale + k) + 1);
-                const __half2* ph = reinterpret_cast<const __half2*>(&g[i]);
-                __half2* po = reinterpret_cast<__half2*>(&val);
-                float2 f;
-                f = __half22float2(ph[0]); f.x *= s0.x; f.y *= s0.y; po[0] = __float22half2_rn(f);
-                f = __half22float2(ph[1]); f.x *= s0.z; f.y *= s0.w; po[1] = __float22half2_rn(f);
-                f = __half22float2(ph[2]); f.x *= s1.x; f.y *= s1.y; po[2] = __float22half2_rn(f);
-                f = __half22float2(ph[3]); f.x *= s1.z; f.y *= s1.w; po[3] = __float22half2_rn(f);
+          for (int i = 0; i < 8; ++i) {
+            const __half* gsrc = p.src0;   // always a valid address (no bytes are read when nbytes == 0)
+            uint32_t nbytes = 0;
+            if (kvalid && pb[i] >= 0) {
+              int iy = py[i] * p.stride + tr - p.pad;
+              int ix = px[i] * p.stride + ts - p.pad;
+              bool ok = true;
+              if (p.pad_mode == 1) {
+                iy = reflect_idx(iy, p.IH);
+                ix = reflect_idx(ix, p.IW);
+              } else {
+                ok = (iy >= 0) && (iy < p.IH) && (ix >= 0) && (ix < p.IW);
               }
-              const int r = rg + 16 * i;
-              *reinterpret_cast<uint4*>(sa + r * 128 + ((j ^ (r & 7)) << 4)) = val;
+              if (ok) { gsrc = src + (((long)pb[i] * p.IH + iy) * p.IW + ix) * ld + cc; nbytes = 16; }
             }
-          } else {
-            const int tap = kvalid ? p.fd_ct.div(k) : 0;
-            const int c = k - tap * Ct;
-            const int tr = p.fd_s.div(tap), ts = tap - tr * p.S;
-            const __half* src = (c < p.C0) ? p.src0 : p.src1;
-            const int ld = (c < p.C0) ? p.ld0 : p.ld1;
-            const int cc = (c < p.C0) ? c : c - p.C0;
-            // asynchronous gather: 16-byte cp.async per (row, chunk) with zero fill for padding / tails; the mbarrier
-            // arrival fires when this thread's copies have landed, so the builder runs ahead by the ring depth
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const __half* gsrc = p.src0;   // always a valid address (no bytes are read when nbytes == 0)
-              uint32_t nbytes = 0;
-              if (kvalid && pb[i] >= 0) {
-                int iy = py[i] * p.stride + tr - p.pad;
-                int ix = px[i] * p.stride + ts - p.pad;
-                bool ok = true;
-                if (p.pad_mode == 1) {
-                  iy = reflect_idx(iy, p.IH);
-                  ix = reflect_idx(ix, p.IW);
-                } else {
-                  ok = (iy >= 0) && (iy < p.IH) && (ix >= 0) && (ix < p.IW);
-                }
-                if (ok) { gsrc = src + (((long)pb[i] * p.IH + iy) * p.IW + ix) * ld + cc; nbytes = 16; }
-              }
-              const int r = rg + 16 * i;
-              cp_async16_zfill(sa + r * 128 + ((j ^ (r & 7)) << 4), gsrc, nbytes);
-            }
-            cp_async_mbar_arrive_noinc(&full_bar[stage]);
-            if (++stage == p.stages) { stage = 0; phase ^= 1u; }
-            continue;
+            const int r = rg + 16 * i;
+            cp_async16_zfill(sa + r * 128 + ((j ^ (r & 7)) << 4), gsrc, nbytes);
           }
-          fence_proxy_async_smem();
-          mbar_arrive(&full_bar[stage]);
+          cp_async_mbar_arrive_noinc(&full_bar[stage]);
           if (++stage == p.stages) { stage = 0; phase ^= 1u; }
         }
        }

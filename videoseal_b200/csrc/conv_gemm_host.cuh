@@ -111,13 +111,10 @@ inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw,
   p.n_tiles = (N + p.block_n - 1) / p.block_n;
   // small-N layers: several consecutive M tiles share one accumulator round (columns g*block_n of the accumulator tile) so that
   // the per-tile barrier handshakes / index math are amortised
-  p.group = 1;
-  if (!getenv("VSB_NO_GROUP")) {
-    p.group = p.block_n <= 32 ? kAccCols / p.block_n : 1;
-    if (p.group > 4) p.group = 4;
-    if (p.group < 1) p.group = 1;
-    if (p.m_tiles < 4 * num_sms) p.group = 1;   // keep enough tiles for load balance
-  }
+  p.group = p.block_n <= 32 ? kAccCols / p.block_n : 1;
+  if (p.group > 4) p.group = 4;
+  if (p.group < 1) p.group = 1;
+  if (p.m_tiles < 4 * num_sms) p.group = 1;   // keep enough tiles for load balance
   p.num_tiles = ((p.m_tiles + p.group - 1) / p.group) * p.n_tiles;
   p.fd_ntiles = make_fastdiv(p.n_tiles); p.fd_tpi = make_fastdiv(p.tiles_per_img); p.fd_tx = make_fastdiv(p.tiles_x);
   p.fd_tw = make_fastdiv(p.tile_w); p.fd_group = make_fastdiv(p.group); p.fd_rps = make_fastdiv(p.rows_per_sample);
@@ -127,12 +124,11 @@ inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw,
   p.b_stage_bytes = (uint32_t)(p.block_n * p.kblk * 2);
   p.stage_bytes = p.a_stage_bytes + ((p.b_stage_bytes + 1023u) & ~1023u);
   VSB_CHECK(p.a_stage_bytes % 1024 == 0, "A stage must be 1024B aligned");
-  // shared memory: [header | stages x (A|B) | halo tiles | upsampled halo | resident weights | residual ring | output staging |
-  // accumulator tile]
+  // shared memory: [header | stages x (A|B) | halo tiles | resident weights | residual ring | output staging | accumulator tile]
   size_t resid_one = 0;
   p.resid_direct = 0;
   if (p.resid16 && op.loader == LD_TMA && p.num_kb >= 24 && (p.ld_res16 % 8) == 0 && N % p.block_n == 0 && (long)p.m_tiles * kBlockM == (long)p.M &&
-      p.out32 == nullptr && p.outc_w == nullptr && !getenv("VSB_RESID_RING"))
+      p.out32 == nullptr && p.outc_w == nullptr)
     p.resid_direct = 1;     // whole tiles only (the lean affine path is the one that implements the direct read)
   if (p.resid16 && !p.resid_direct) resid_one = (size_t)kBlockM * p.block_n * 2;
   if (p.resid32) resid_one = (size_t)kBlockM * p.block_n * 4;
@@ -146,7 +142,6 @@ inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw,
   p.halo_bufs = 2;
   if (p.halo_stride) { p.halo_bufs = (int)(24576 / p.halo_stride); if (p.halo_bufs > kMaxHalo) p.halo_bufs = kMaxHalo; if (p.halo_bufs < 2) p.halo_bufs = 2; }
   const size_t halo_total = (size_t)p.halo_bufs * p.halo_stride;
-  const size_t u_bytes = op.loader == LD_HALO_UPS ? (((size_t)kHaloH * kHaloW * p.cc * 2 + 1023) & ~size_t(1023)) : 0;
   // resident weights: one N tile, whole K slab <= 48 KB -> loaded once per CTA instead of once per tile
   const size_t bslab = (size_t)p.num_kb * p.b_stage_bytes;
   p.b_resident = (p.n_tiles == 1 && bslab <= 48 * 1024 && op.w_samples == 1) ? 1 : 0;
@@ -154,15 +149,14 @@ inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw,
   // so its [block_n x K] weight slab can stay resident too when it fits beside >= 4 A stages.  Without this the slab is re-streamed
   // from L2 for every M tile (res 1x1 384->384: 295 KB of weights per M tile against 98 KB of activations).
   p.b_fixed_ntile = 0;
-  if (!p.b_resident && p.n_tiles > 1 && p.n_tiles <= 8 && op.w_samples == 1 && op.loader == LD_TMA && !getenv("VSB_NO_BRES2") &&
+  if (!p.b_resident && p.n_tiles > 1 && p.n_tiles <= 8 && op.w_samples == 1 && op.loader == LD_TMA &&
       kHeaderBytes + resid_bytes + bslab + kAccBytes + 4 * (size_t)p.a_stage_bytes + 64 * 1024 <= 225 * 1024 && p.num_tiles >= 2 * num_sms) {
     p.b_resident = 1;
     p.b_fixed_ntile = 1;
   }
-  if (getenv("VSB_NO_BRES")) { p.b_resident = 0; p.b_fixed_ntile = 0; }
   // a resident slab that leaves fewer than 2 pipeline stages beside the rest is streamed instead
   if (p.b_resident && !p.b_fixed_ntile &&
-      kHeaderBytes + resid_bytes + halo_total + u_bytes + bslab + kAccBytes + 2 * (size_t)p.a_stage_bytes + 1024 > 225 * 1024)
+      kHeaderBytes + resid_bytes + halo_total + bslab + kAccBytes + 2 * (size_t)p.a_stage_bytes + 1024 > 225 * 1024)
     p.b_resident = 0;
   const size_t bres_bytes = p.b_resident ? bslab : 0;
   if (p.b_resident) p.stage_bytes = p.a_stage_bytes;
@@ -172,11 +166,11 @@ inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw,
   {
     const int nchunks = p.block_n / 16, epw = kEpiWarps / 4;     // epilogue warps per 32-row quadrant
     const bool common = op.loader == LD_TMA && p.outc_w == nullptr && p.epi == EPI_AFFINE && (long)p.m_tiles * kBlockM == (long)p.M &&
-                        N % p.block_n == 0 && p.num_kb <= 12 && !getenv("VSB_NO_TMA_STORE");
+                        N % p.block_n == 0 && p.num_kb <= 12;
     if (common && p.out16 != nullptr && p.out32 == nullptr && (p.ld_out16 % 8) == 0 && (reinterpret_cast<uintptr_t>(p.out16) & 15) == 0)
       p.tma_store = 1;
     else if (common && p.out32 != nullptr && p.out16 == nullptr && p.act == ACT_NONE && p.resid32 != nullptr && p.grn_stats == nullptr &&
-             (p.ld_out32 % 4) == 0 && (reinterpret_cast<uintptr_t>(p.out32) & 15) == 0 && !getenv("VSB_NO_TMA_STORE32"))
+             (p.ld_out32 % 4) == 0 && (reinterpret_cast<uintptr_t>(p.out32) & 15) == 0)
       p.tma_store = 2;
     if (p.tma_store) {
       p.cpw = (nchunks + epw - 1) / epw;
@@ -187,12 +181,11 @@ inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw,
       p.ost_cpb = (nchunks % epw == 0 && p.cpw * cb <= 128u) ? p.cpw : 1;
       p.ost_rowb = (uint32_t)p.ost_cpb * cb;
       p.ost_swz = p.ost_rowb == 128u ? 3 : (p.ost_rowb == 64u ? 2 : (p.ost_rowb == 32u ? 1 : 0));
-      if (getenv("VSB_TMA_STORE_NOSWZ")) p.ost_swz = 0;
       p.ostage_bytes = (uint32_t)p.cpw * 32u * cb;               // per warp: multiples of 1024 bytes (swizzle atoms stay aligned)
     }
   }
   size_t ostage_total = p.tma_store ? (size_t)kEpiWarps * p.ostage_bytes + 1024 : 0;
-  size_t fixed = kHeaderBytes + resid_bytes + halo_total + u_bytes + bres_bytes + ostage_total + kAccBytes;
+  size_t fixed = kHeaderBytes + resid_bytes + halo_total + bres_bytes + ostage_total + kAccBytes;
   if (p.tma_store && fixed + 2 * (size_t)p.stage_bytes > 225 * 1024) {   // no room for the staging boxes: plain stores
     fixed -= ostage_total;
     ostage_total = 0;
@@ -204,8 +197,7 @@ inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw,
   if (stages > kMaxStages) stages = kMaxStages;
   p.stages = stages;
   p.halo_off = (uint32_t)(kHeaderBytes + (size_t)stages * p.stage_bytes);
-  p.u_off = (uint32_t)(p.halo_off + halo_total);
-  p.bres_off = (uint32_t)(p.u_off + u_bytes);
+  p.bres_off = (uint32_t)(p.halo_off + halo_total);
   p.resid_off = (uint32_t)(p.bres_off + bres_bytes);
   p.ostage_off = (uint32_t)((p.resid_off + resid_bytes + 1023) & ~size_t(1023));   // swizzle atoms of the staging boxes need 1024-byte alignment
   p.acc_off = (uint32_t)(p.ostage_off + ostage_total);
@@ -237,7 +229,7 @@ inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw,
   // whole tiles and an aligned bias vector: the epilogue warps read it from global memory and never meet at a barrier (the fused
   // 1x1 outc epilogue keeps its own barrier, so it keeps the shared copy)
   p.bias_global = (p.bias != nullptr && N % p.block_n == 0 && p.epi == EPI_AFFINE && p.outc_w == nullptr &&
-                   (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0 && !getenv("VSB_NO_BIAS_GLOBAL")) ? 1 : 0;
+                   (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0) ? 1 : 0;
   op.grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
   if (p.b_fixed_ntile) op.grid = (num_sms / p.n_tiles) * p.n_tiles;
   // 8 epilogue warps (LD_TMA) or 4 epilogue + 4 builder warps, 2 MMA warpgroups, the producer warp
@@ -314,28 +306,6 @@ inline void setup_halo_conv3(ConvGemmOp& op, const __half* src, int B, int H, in
   encode_map(&op.tmA, src, 4, dims, strides, box, 64, /*no_swizzle=*/true);
 }
 
-// UBlock up-conv (modules/common.py:45-52 after the skip concat of unet.py:187-190): conv3x3(valid) o ReflectionPad2d(1) o
-// bilinear x2 of the virtual concat [src0 (C0) | src1 (C1)], both NHWC fp16 at IH x IW; output at 2IH x 2IW.
-inline void setup_halo_ups(ConvGemmOp& op, const __half* src0, int C0, int ld0, const __half* src1, int C1, int ld1, int B, int IH, int IW) {
-  ConvGemmParams& p = op.p;
-  op.loader = LD_HALO_UPS;
-  VSB_CHECK(C1 == 0 || C1 == C0, "halo ups: both sources must have the same channel count");
-  setup_halo_common(p, C0, C1, B, 2 * IH, 2 * IW);
-  p.IH = IH; p.IW = IW; p.OH = 2 * IH; p.OW = 2 * IW;
-  p.halo_bytes = (uint32_t)(6 * 10 * p.cc * 2);
-  uint32_t box[4] = {(uint32_t)p.cc, 10u, 6u, 1u};
-  {
-    uint64_t dims[4] = {(uint64_t)C0, (uint64_t)IW, (uint64_t)IH, (uint64_t)B};
-    uint64_t strides[3] = {(uint64_t)ld0 * 2, (uint64_t)IW * ld0 * 2, (uint64_t)IH * IW * ld0 * 2};
-    encode_map(&op.tmA, src0, 4, dims, strides, box, 64, true);
-  }
-  if (C1 > 0) {
-    uint64_t dims[4] = {(uint64_t)C1, (uint64_t)IW, (uint64_t)IH, (uint64_t)B};
-    uint64_t strides[3] = {(uint64_t)ld1 * 2, (uint64_t)IW * ld1 * 2, (uint64_t)IH * IW * ld1 * 2};
-    encode_map(&op.tmA2, src1, 4, dims, strides, box, 64, true);
-  }
-}
-
 // A = [M, K] fp16 row-major (row pitch ld elements)
 inline void setup_tma_gemm(ConvGemmOp& op, const __half* A, long M, int K, int ld) {
   ConvGemmParams& p = op.p;
@@ -392,36 +362,19 @@ inline void setup_gather_conv(ConvGemmOp& op, int loader, const __half* src0, in
   p.num_kb = (p.Ktot + 63) / 64;
 }
 
-// A[m, k] = G[m, k] * scale[m / rows_per_sample, k]   (ConvNeXt pwconv2 with the GRN factor folded in)
-inline void setup_gather_scale(ConvGemmOp& op, const __half* G, long M, int K, int ld, const float* scale, int ld_scale, int rows_per_sample) {
-  ConvGemmParams& p = op.p;
-  op.loader = LD_GATHER_SCALE;
-  p.kblk = 64;
-  p.src0 = G; p.ld0 = ld; p.C0 = K; p.C1 = 0;
-  VSB_CHECK(K % 8 == 0 && ld % 8 == 0 && ld_scale % 4 == 0, "gather scale: K must be a multiple of 8");
-  p.Ktot = K;
-  p.a_scale = scale; p.ld_scale = ld_scale; p.rows_per_sample = rows_per_sample;
-  p.M = (int)M;
-  p.m_tiles = (int)((M + kBlockM - 1) / kBlockM);
-  p.num_kb = (K + 63) / 64;
-}
-
-#ifdef VSB_PDL
 // launch with programmatic stream serialization: the kernel may begin while its predecessor drains and synchronises
-// itself with pdl_wait() (ptx.cuh).  VSB_NO_PDL=1 falls back to classic launches at run time (A/B in one build).
+// itself with pdl_wait() (ptx.cuh).
 template <class... KArgs, class... Args>
 inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
-  static const bool off = getenv("VSB_NO_PDL") != nullptr;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = off ? 0 : 1;
+  cfg.attrs = attr; cfg.numAttrs = 1;
   VSB_CUDA(cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...));
 }
-#endif
 
 template <int LOADER, int ACT>
 inline void launch_one(const ConvGemmOp& op, cudaStream_t st) {
@@ -430,11 +383,7 @@ inline void launch_one(const ConvGemmOp& op, cudaStream_t st) {
     VSB_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<LOADER, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
-#ifdef VSB_PDL
   launch_pdl(conv_gemm_kernel<LOADER, ACT>, dim3(op.grid), dim3(op.threads), op.smem, st, op.tmA, op.tmA2, op.tmB, op.tmO, op.p);
-#else
-  conv_gemm_kernel<LOADER, ACT><<<op.grid, op.threads, op.smem, st>>>(op.tmA, op.tmA2, op.tmB, op.tmO, op.p);
-#endif
 }
 
 // instantiated (loader, activation) pairs: only what the networks need, to bound compile time
@@ -451,17 +400,9 @@ inline void launch(const ConvGemmOp& op, cudaStream_t st) {
       else if (a == ACT_RELU) launch_one<LD_GATHER_CONV, ACT_RELU>(op, st);
       else throw Error("gather conv: unsupported activation", kErrUnsupported);
       break;
-    case LD_HALO_UPS:
-      if (a == ACT_RELU) launch_one<LD_HALO_UPS, ACT_RELU>(op, st);
-      else throw Error("halo ups: unsupported activation", kErrUnsupported);
-      break;
     case LD_HALO_CONV3:
       if (a == ACT_RELU) launch_one<LD_HALO_CONV3, ACT_RELU>(op, st);
       else throw Error("halo conv3: unsupported activation", kErrUnsupported);
-      break;
-    case LD_GATHER_SCALE:
-      if (a == ACT_NONE) launch_one<LD_GATHER_SCALE, ACT_NONE>(op, st);
-      else throw Error("gather scale: unsupported activation", kErrUnsupported);
       break;
     default: throw Error("bad loader");
   }

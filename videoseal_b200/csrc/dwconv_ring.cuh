@@ -13,7 +13,7 @@
 //   * a finished output row is normalised in registers: the per-pixel sums over the channel pairs are reduced with a halving
 //     butterfly over 16-lane segments, combined across the segments through a few floats of shared memory (one named barrier of the
 //     compute warps per row, double-buffered partials), one-pass variance.
-// Requires dense x / out (pixel pitch C), H % R == 0, W % (NS*SX) == 0, (NS * C/2) % 32 == 0.
+// Requires dense x / out (pixel pitch C), H % R == 0, W % (NS*SX) == 0, (NS * C/2) % 32 == 0, C <= 256 (one TMA box per row).
 #pragma once
 #include <type_traits>
 #include "ptx.cuh"
@@ -21,37 +21,23 @@
 namespace vsb {
 
 
-template <int C> struct DwRingCfg {
-  static constexpr int CB = C <= 256 ? C : 192;      // channels per TMA box (<= 256 elements per box dimension)
-  static constexpr int NOPS = C / CB;
-  static_assert(C % CB == 0, "channel chunking");
-};
-
 __device__ __forceinline__ void dw_bar_sync(int nthreads) { asm volatile("bar.sync 3, %0;" ::"r"(nthreads) : "memory"); }
 
-// WS = true: the 49 weight pairs of a thread are read from a shared copy ([49][C] floats, one 64-bit shared load per 4 FFMA2) instead
-// of living in 98 registers: ~110 registers per thread, 3-4 blocks per SM instead of 2.
-template <int C, int NS, int SX, int kDwRingSlots, bool WS = false>
-__global__ void __launch_bounds__(NS * C / 2 + 32, WS ? 3 : 1)
+template <int C, int NS, int SX, int kDwRingSlots>
+__global__ void __launch_bounds__(NS * C / 2 + 32, 1)
 dwconv7_ln_ring_kernel(const __grid_constant__ CUtensorMap tmX, int B, int H, int W, const float* __restrict__ wdw /*[49][C]*/,
                        const float* __restrict__ bdw, const float* __restrict__ lnw, const float* __restrict__ lnb,
                        __half* __restrict__ out, int R) {
   constexpr int C2 = C / 2, KSEG = C2 / 16, NV = 2 * SX;      // 16-lane segments per strip; values per thread in the row reduction
   constexpr int BW = NS * SX + 6;                              // band width in pixels incl. the halo
-  constexpr int CB = DwRingCfg<C>::CB, NOPS = DwRingCfg<C>::NOPS;
-  constexpr int SLOT = BW * C;                                 // floats per ring slot, layout [chunk][BW][CB]
+  constexpr int SLOT = BW * C;                                 // floats per ring slot, layout [BW][C]
   constexpr int NCOMP = NS * C2;                               // compute threads
-  static_assert(NCOMP % 32 == 0 && C2 % 16 == 0 && (SX == 2 || SX == 4), "shape");
+  static_assert(NCOMP % 32 == 0 && C2 % 16 == 0 && (SX == 2 || SX == 4) && C <= 256, "shape");
   extern __shared__ __align__(128) float dwr_smem[];
   float* ring = dwr_smem;                                                            // [kDwRingSlots][SLOT]
   float* part = ring + kDwRingSlots * SLOT;                                          // [2][NS][KSEG][NV]
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(part + 2 * NS * KSEG * NV);       // [slots] | empty [slots]
   uint64_t* empty_bar = full_bar + kDwRingSlots;
-  float* wsm = reinterpret_cast<float*>(empty_bar + kDwRingSlots);                   // WS: [49][C]
-  if (WS) {
-    for (int i = threadIdx.x * 4; i < 49 * C; i += (NCOMP + 32) * 4)
-      *reinterpret_cast<float4*>(wsm + i) = __ldg(reinterpret_cast<const float4*>(wdw + i));
-  }
 
   const int cgroups = W / (NS * SX), rgroups = H / R;
   const int cg = blockIdx.x % cgroups;
@@ -79,9 +65,7 @@ dwconv7_ln_ring_kernel(const __grid_constant__ CUtensorMap tmX, int B, int H, in
         const int slot = q % kDwRingSlots;
         mbar_wait(&empty_bar[slot], (((uint32_t)(q / kDwRingSlots)) & 1u) ^ 1u);
         mbar_arrive_expect_tx(&full_bar[slot], (uint32_t)(SLOT * sizeof(float)));
-#pragma unroll
-        for (int ch = 0; ch < NOPS; ++ch)
-          tma_load_4d(&tmX, &full_bar[slot], ring + (size_t)slot * SLOT + ch * BW * CB, ch * CB, xb - 3, iy, b);
+        tma_load_4d(&tmX, &full_bar[slot], ring + (size_t)slot * SLOT, 0, xb - 3, iy, b);
         ++q;
       }
     }
@@ -92,16 +76,12 @@ dwconv7_ln_ring_kernel(const __grid_constant__ CUtensorMap tmX, int B, int H, in
   const int s = threadIdx.x / C2, cp = threadIdx.x - s * C2, c = cp * 2;
   const int lane = threadIdx.x & 31, seg = cp >> 4;
   const int x0 = xb + s * SX;
-  // this thread's pixels inside a slot: pixel (s*SX + u) of the band, channel c  ->  [chunk][pixel][CB]
-  const int soff = (c / CB) * BW * CB + (s * SX) * CB + (c % CB);
+  // this thread's pixels inside a slot: pixel (s*SX + u) of the band, channel c  ->  [pixel][C]
+  const int soff = (s * SX) * C + c;
 
-  float2 wt[WS ? 1 : 49];
-  if (!WS) {
+  float2 wt[49];
 #pragma unroll
-    for (int k = 0; k < 49; ++k) wt[WS ? 0 : k] = __ldg(reinterpret_cast<const float2*>(wdw + k * C + c));
-  }
-  const float* wcol = wsm + c;
-  auto WGT = [&](int idx) -> float2 { return WS ? *reinterpret_cast<const float2*>(wcol + idx * C) : wt[WS ? 0 : idx]; };
+  for (int k = 0; k < 49; ++k) wt[k] = __ldg(reinterpret_cast<const float2*>(wdw + k * C + c));
   const float2 bias = __ldg(reinterpret_cast<const float2*>(bdw + c));
   const float2 lg = __ldg(reinterpret_cast<const float2*>(lnw + c)), lb = __ldg(reinterpret_cast<const float2*>(lnb + c));
 
@@ -122,7 +102,7 @@ dwconv7_ln_ring_kernel(const __grid_constant__ CUtensorMap tmX, int B, int H, in
       mbar_wait(&full_bar[slot], ((uint32_t)(q / kDwRingSlots)) & 1u);
       const float* rp = ring + (size_t)slot * SLOT + soff;
 #pragma unroll
-      for (int u = 0; u < SX + 6; ++u) cur[u] = *reinterpret_cast<const float2*>(rp + u * CB);
+      for (int u = 0; u < SX + 6; ++u) cur[u] = *reinterpret_cast<const float2*>(rp + u * C);
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty_bar[slot]);  // the row now lives in this warp's registers
       ++q;
@@ -131,10 +111,10 @@ dwconv7_ln_ring_kernel(const __grid_constant__ CUtensorMap tmX, int B, int H, in
       constexpr int SL = (PH + 7) % 7;
       if (rowok && i < R) {
 #pragma unroll
-        for (int p = 0; p < SX; ++p) acc[SL][p] = f2fma(cur[p], WGT(0), bias);
+        for (int p = 0; p < SX; ++p) acc[SL][p] = f2fma(cur[p], wt[0], bias);
 #pragma unroll
         for (int k = 1; k < 7; ++k) {
-          const float2 wk = WGT(k);
+          const float2 wk = wt[k];
 #pragma unroll
           for (int p = 0; p < SX; ++p) acc[SL][p] = f2fma(cur[p + k], wk, acc[SL][p]);
         }
@@ -152,7 +132,7 @@ dwconv7_ln_ring_kernel(const __grid_constant__ CUtensorMap tmX, int B, int H, in
         for (int k = 0; k < 7; ++k)
 #pragma unroll
           for (int j = 0; j < 6; ++j) {
-            const float2 wk = WGT((6 - j) * 7 + k);
+            const float2 wk = wt[(6 - j) * 7 + k];
 #pragma unroll
             for (int p = 0; p < SX; ++p) acc[(PH + j + 1) % 7][p] = f2fma(cur[p + k], wk, acc[(PH + j + 1) % 7][p]);
           }
@@ -163,7 +143,7 @@ dwconv7_ln_ring_kernel(const __grid_constant__ CUtensorMap tmX, int B, int H, in
           if (o >= 0 && o < R) {
 #pragma unroll
             for (int k = 0; k < 7; ++k) {
-              const float2 wk = WGT((6 - j) * 7 + k);
+              const float2 wk = wt[(6 - j) * 7 + k];
 #pragma unroll
               for (int p = 0; p < SX; ++p) acc[(PH + j + 1) % 7][p] = f2fma(cur[p + k], wk, acc[(PH + j + 1) % 7][p]);
             }
@@ -272,8 +252,8 @@ dwconv7_ln_ring_kernel(const __grid_constant__ CUtensorMap tmX, int B, int H, in
   }
 }
 
-template <int C, int NS, int SX, int kDwRingSlots, bool WS = false> constexpr size_t dw_ring_smem() {
-  return (size_t)(kDwRingSlots * (NS * SX + 6) * C + 2 * NS * (C / 32) * 2 * SX + (WS ? 49 * C : 0)) * sizeof(float) + 2 * kDwRingSlots * sizeof(uint64_t) + 128;
+template <int C, int NS, int SX, int kDwRingSlots> constexpr size_t dw_ring_smem() {
+  return (size_t)(kDwRingSlots * (NS * SX + 6) * C + 2 * NS * (C / 32) * 2 * SX) * sizeof(float) + 2 * kDwRingSlots * sizeof(uint64_t) + 128;
 }
 
 }  // namespace vsb

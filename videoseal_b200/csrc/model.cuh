@@ -197,43 +197,34 @@ struct DwRingOp {
   const float *dww = nullptr, *dwb = nullptr, *lnw = nullptr, *lnb = nullptr;
   __half* out = nullptr;
 };
-template <int C, int NS, int SX, int NSLOT, bool WS = false>
+template <int C, int NS, int SX, int NSLOT>
 inline void launch_dw_ring_t(const DwRingOp& op, cudaStream_t st) {
   static bool attr = false;
-  constexpr size_t smem = dw_ring_smem<C, NS, SX, NSLOT, WS>();
+  constexpr size_t smem = dw_ring_smem<C, NS, SX, NSLOT>();
   if (!attr) {
-    VSB_CUDA(cudaFuncSetAttribute(dwconv7_ln_ring_kernel<C, NS, SX, NSLOT, WS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    VSB_CUDA(cudaFuncSetAttribute(dwconv7_ln_ring_kernel<C, NS, SX, NSLOT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr = true;
   }
   const unsigned blocks = (unsigned)((long)op.B * (op.H / op.R) * (op.H / (NS * SX)));
-#ifdef VSB_PDL
-  launch_pdl(dwconv7_ln_ring_kernel<C, NS, SX, NSLOT, WS>, dim3(blocks), dim3(NS * C / 2 + 32), smem, st, op.tm, op.B, op.H, op.H, op.dww, op.dwb, op.lnw,
+  launch_pdl(dwconv7_ln_ring_kernel<C, NS, SX, NSLOT>, dim3(blocks), dim3(NS * C / 2 + 32), smem, st, op.tm, op.B, op.H, op.H, op.dww, op.dwb, op.lnw,
              op.lnb, op.out, op.R);
-#else
-  dwconv7_ln_ring_kernel<C, NS, SX, NSLOT, WS><<<blocks, NS * C / 2 + 32, smem, st>>>(op.tm, op.B, op.H, op.H, op.dww, op.dwb, op.lnw, op.lnb, op.out, op.R);
-#endif
   VSB_CUDA(cudaGetLastError());
 }
-inline bool dw_ring_ok(int C, int H, int ld) {
-  // (the 384-channel instantiation exists and is correct, but at 16 x 16 maps it runs one 192-thread block per SM with a 14-step
-  //  prologue per 8 rows; the whole-row strip kernel handles those maps)
-  static const bool all = getenv("VSB_DW_RING_384") != nullptr;
-  return ld == C && ((C == 96 && H % 16 == 0) || (C == 192 && H % 16 == 0) || (all && C == 384 && H % 8 == 0));
-}
+// (384 channels take the whole-row strip kernel: at 16 x 16 maps a ring block would run one 192-thread block per SM with a
+//  14-step prologue per 8 rows)
+inline bool dw_ring_ok(int C, int H, int ld) { return ld == C && (C == 96 || C == 192) && H % 16 == 0; }
 inline void setup_dw_ring(DwRingOp& op, const float* x, int B, int H, int C) {
   op.C = C; op.B = B; op.H = H;
-  op.R = C == 384 ? 8 : (H % 32 == 0 ? 32 : 16);    // rows per block: 6 halo rows + the block prologue are amortised over R
-  const int BW = (C == 96 ? 8 : 4) + 6, CB = C <= 256 ? C : 192;
+  op.R = H % 32 == 0 ? 32 : 16;    // rows per block: 6 halo rows + the block prologue are amortised over R
+  const int BW = (C == 96 ? 8 : 4) + 6;
   uint64_t dims[4] = {(uint64_t)C, (uint64_t)H, (uint64_t)H, (uint64_t)B};
   uint64_t strides[3] = {(uint64_t)C * 4, (uint64_t)H * C * 4, (uint64_t)H * H * C * 4};
-  uint32_t box[4] = {(uint32_t)CB, (uint32_t)BW, 1u, 1u};
+  uint32_t box[4] = {(uint32_t)C, (uint32_t)BW, 1u, 1u};
   encode_map(&op.tm, x, 4, dims, strides, box, 0, true, /*f32=*/true);
 }
 inline void launch_dw_ring(const DwRingOp& op, cudaStream_t st) {
-  static const bool ws = getenv("VSB_DW_WS") != nullptr;     // weights from shared memory (more blocks per SM): A/B switch
-  if (op.C == 96) { if (ws) launch_dw_ring_t<96, 2, 4, 6, true>(op, st); else launch_dw_ring_t<96, 2, 4, 8>(op, st); }
-  else if (op.C == 192) { if (ws) launch_dw_ring_t<192, 1, 4, 4, true>(op, st); else launch_dw_ring_t<192, 1, 4, 8>(op, st); }
-  else launch_dw_ring_t<384, 1, 4, 8>(op, st);
+  if (op.C == 96) launch_dw_ring_t<96, 2, 4, 8>(op, st);
+  else launch_dw_ring_t<192, 1, 4, 8>(op, st);
 }
 
 class Model {
@@ -418,14 +409,7 @@ class Model {
     VSB_CUDA(cudaStreamSynchronize(0));
     return wd;
   }
-  int halo_max_c = -1;
-  bool use_halo(int C) {
-    if (halo_max_c < 0) {
-      const char* e = getenv("VSB_HALO_MAXC");
-      halo_max_c = e ? atoi(e) : 16;
-    }
-    return C <= halo_max_c;
-  }
+  static bool use_halo(int C) { return C <= 16; }
   ConvW pack_conv3(const std::string& wkey, const std::vector<float>* out_scale, const std::vector<float>& bias) {
     const int C = (int)get(wkey).shape[1], N = (int)get(wkey).shape[0];
     ConvW cw = use_halo(C) ? pack_conv_halo(wkey, out_scale, bias, C, 0) : pack_conv(wkey, out_scale, bias);
@@ -501,7 +485,7 @@ class Model {
     }
     for (int i = 0; i < L - 1; ++i) {
       down_conv.push_back(pack_conv(P + "downs." + std::to_string(i) + ".down.weight", nullptr, get(P + "downs." + std::to_string(i) + ".down.bias").data));
-      if (z[i] == 16 && z[i + 1] == 32 && conv3_direct_ok(64, 32, 64, 0, 3) && !getenv("VSB_NO_S2D"))
+      if (z[i] == 16 && z[i + 1] == 32 && conv3_direct_ok(64, 32, 64, 0, 3))
         down_conv.back().wd = pack_down_s2d(P + "downs." + std::to_string(i) + ".down.weight");
       down_rb.push_back(pack_resblock(P + "downs." + std::to_string(i) + ".conv"));
     }
@@ -517,7 +501,7 @@ class Model {
         for (int c = zz[ii + 1]; c < 2 * zz[ii + 1]; ++c) in_scale[c] = 0.70710678118654752440f;
         up_conv.push_back(pack_upconv_taps(U + ".up.upsample_block.2.weight", in_scale));
         __half* pw = nullptr; float* bw = nullptr;
-        if (zz[ii] == 16 && 2 * zz[ii + 1] == 64 && conv3_direct_ok(64, 64, 64, 0, 3) && !getenv("VSB_NO_UPPHASE"))
+        if (zz[ii] == 16 && 2 * zz[ii + 1] == 64 && conv3_direct_ok(64, 64, 64, 0, 3))
           pack_upconv_phase(U + ".up.upsample_block.2.weight", in_scale, &pw, &bw);
         up_phase_w.push_back(pw); up_border_w.push_back(bw);
         up_lnw.push_back(wpool.upload(get(U + ".up.upsample_block.3.weight").data));
@@ -611,8 +595,8 @@ class Model {
     pl.steps.push_back(Step{[op](cudaStream_t st) { launch(op, st); }, 1, name});
   }
   // 3x3 stride-1 zero-padded conv: on-chip im2col from a shared-memory halo tile (input crosses L2->SM once) up to
-  // `halo_max_c` input channels, one TMA load per tap above (VSB_HALO_MAXC overrides, for experiments); the weight layout
-  // was chosen by the same rule at pack time (pack_conv3)
+  // 16 input channels, one TMA load per tap above (use_halo); the weight layout was chosen by the same rule at pack time
+  // (pack_conv3)
   void setup_conv3(ConvGemmOp& op, const __half* x, int B, int H, int W, int C, int ld) {
     if (use_halo(C)) setup_halo_conv3(op, x, B, H, W, C, ld);
     else setup_tma_conv(op, x, B, H, W, C, ld, 3, 3, 1);
@@ -708,11 +692,7 @@ class Model {
       float *w1 = first_w1, *b1 = first_b1, *wr = first_wr, *br = first_br;
       pl.steps.push_back(Step{[=](cudaStream_t st) {
         dim3 grid((S + 31) / 32, (S + 15) / 16, B);
-        // frame stride lets image-size inputs be read in place (key frames of a video are `step` frames apart)
         const float* src = plp->in_imgs;
-        if (plp->in_frame_stride != (long)3 * S * S) {
-          // strided key frames: launch per frame group is avoided by passing the stride through the batch index
-        }
         if (cin == 1) unet_first_kernel<1><<<grid, 256, 0, st>>>(src, B, S, S, Z, w1, b1, wr, br, h1, r0, yuv);
         else unet_first_kernel<3><<<grid, 256, 0, st>>>(src, B, S, S, Z, w1, b1, wr, br, h1, r0, yuv);
         VSB_CUDA(cudaGetLastError());
@@ -821,8 +801,7 @@ class Model {
         const int gthreads = Cc / (8 * vpt);          // threads per output pixel
         VSB_CHECK(Cc % (8 * vpt) == 0 && gthreads <= 32 && (gthreads & (gthreads - 1)) == 0, "up conv: C_out must be 8 * 2^k <= 512");
         const size_t tsmem = (size_t)100 * 9 * Cc * sizeof(__half);
-        static const bool no_tiled = getenv("VSB_UPS_UNTILED") != nullptr;
-        if (!no_tiled && IH % 8 == 0 && tsmem <= 160 * 1024) {
+        if (IH % 8 == 0 && tsmem <= 160 * 1024) {
           // low-resolution taps of a 16 x 16 output tile staged in shared memory (ups_gather_ln_tiled_kernel)
           pl.steps.push_back(Step{[=](cudaStream_t st) {
             const unsigned blocks = (unsigned)((long)B * (IH / 8) * (IH / 8));
@@ -933,8 +912,6 @@ class Model {
         part_n = std::max(part_n, (size_t)((Ms + kBlockM - 1) / kBlockM * 4) * 4 * d.ext_dims[s]);
       }
     }
-    static const bool no_part = getenv("VSB_GRN_ATOMIC") != nullptr;
-    if (no_part) all_part = false;
     float* part_buf = all_part ? pl.pool.alloc_n<float>(part_n) : nullptr;
     if (!all_part)
       pl.steps.push_back(Step{[=](cudaStream_t st) { VSB_CUDA(cudaMemsetAsync(stats_all, 0, 2 * stats_n * sizeof(float), st)); }, 0,
@@ -974,8 +951,7 @@ class Model {
       __half* g = pl.pool.alloc_n<__half>(M * 4 * C);   // 4C is a multiple of 8 for every even width
       // GRN multiplier: folded into per-sample pwconv2 weights where a sample has many more rows than W2 has output
       // channels (stages 0-1 of the tiny trunk), applied to g in place otherwise
-      static const bool no_wscale = getenv("VSB_NO_WSCALE") != nullptr;
-      const bool wscale = !no_wscale && 4 * C <= rows_per_sample && rows_per_sample % kBlockM == 0 && C % 16 == 0;
+      const bool wscale = 4 * C <= rows_per_sample && rows_per_sample % kBlockM == 0 && C % 16 == 0;
       __half* w2s = wscale ? pl.pool.alloc_n<__half>((size_t)B * C * 4 * C) : nullptr;
       for (int jb = 0; jb < d.ext_depths[s]; ++jb) {
         const CnBlockW& w = cn[s][jb];
@@ -983,9 +959,8 @@ class Model {
           const int H = hs, Cc = C, ldc = Cp;
           const float* xin = x;
           float *dww = w.dww, *dwb = w.dwb, *lw = w.lnw, *lb = w.lnb;
-          static const bool no_ring = getenv("VSB_DW_NO_RING") != nullptr;
-          if (!no_ring && dw_ring_ok(Cc, H, ldc)) {
-            // TMA-ring register-rolling kernel (dwconv_ring.cuh) for the 96 / 192 / 384-channel stages of the tiny trunk
+          if (dw_ring_ok(Cc, H, ldc)) {
+            // TMA-ring register-rolling kernel (dwconv_ring.cuh) for the 96 / 192-channel stages of the tiny trunk
             DwRingOp rop;
             setup_dw_ring(rop, xin, B, H, Cc);
             rop.dww = dww; rop.dwb = dwb; rop.lnw = lw; rop.lnb = lb; rop.out = a;
@@ -993,7 +968,7 @@ class Model {
                                     "cnx.dwconv7_ln." + std::to_string(C) + "@" + std::to_string(hs)});
           } else
           pl.steps.push_back(Step{[=](cudaStream_t st) {
-            if (!(Cc == 96 || Cc == 192 || Cc == 384 || Cc == 768) || getenv("VSB_DW_WIDE")) {
+            if (!(Cc == 96 || Cc == 192 || Cc == 384 || Cc == 768)) {
               // any even width / odd map size (chunkyseal's proportional trunk): threads loop over the channel pairs
               const long nstrips = (long)B * H * ((H + kDwStrip - 1) / kDwStrip);
               const int threads = std::min(512, (Cc / 2 + 31) / 32 * 32);
@@ -1011,22 +986,17 @@ class Model {
             int spb = 1;
             for (int s2 = 1; s2 <= 4; s2 *= 2) if ((s2 * C2) % 32 == 0 && s2 * C2 <= 512) { spb = s2; break; }
             if (spb * C2 > 512) throw Error("dwconv7: C/2 > 512 threads is not implemented (unsupported chunky extractor width)", kErrUnsupported);
-#define VSB_DWC(CC, ST, FR, SPB, NGR, RPB) dwconv7_ln_c_kernel<CC, ST, FR><<<(unsigned)(((NGR) + (SPB) - 1) / (SPB)), (SPB) * (CC) / 2, \
-    (size_t)(SPB) * (ST) * (CC) * sizeof(float), st>>>(xin, B, H, H, dww, dwb, lw, lb, a, Cc, SPB, (int)(NGR), RPB)
+#define VSB_DWC(CC, ST, FR, SPB, NGR) dwconv7_ln_c_kernel<CC, ST, FR><<<(unsigned)(((NGR) + (SPB) - 1) / (SPB)), (SPB) * (CC) / 2, \
+    (size_t)(SPB) * (ST) * (CC) * sizeof(float), st>>>(xin, B, H, H, dww, dwb, lw, lb, a, Cc, SPB, (int)(NGR))
             {
-              // rows per block: 1.  Walking 2-4 consecutive rows per block (L1 reuse of the 7-row input window) gives fewer,
-              // longer blocks with two block barriers per row, which hide less of this latency-bound kernel's stalls;
-              // VSB_DW_RPB selects it
-              int rpb = 1;
-              if (const char* e = getenv("VSB_DW_RPB")) { const int r2 = atoi(e); if (r2 > 0 && H % r2 == 0) rpb = r2; }
               // narrow maps: one strip = the whole row, so no column is ever out of the image
               const long nrows = (long)B * H;
-              if (Cc == 384 && H == 16) VSB_DWC(384, 16, true, 1, nrows, 1);
-              else if (Cc == 768 && H == 8) VSB_DWC(768, 8, true, 1, nrows, 1);
-              else if (Cc == 96) VSB_DWC(96, 8, false, spb, nstrips / rpb, rpb);
-              else if (Cc == 192) VSB_DWC(192, 8, false, spb, nstrips / rpb, rpb);
-              else if (Cc == 384) VSB_DWC(384, 8, false, spb, nstrips / rpb, rpb);
-              else VSB_DWC(768, 8, false, spb, nstrips / rpb, rpb);
+              if (Cc == 384 && H == 16) VSB_DWC(384, 16, true, 1, nrows);
+              else if (Cc == 768 && H == 8) VSB_DWC(768, 8, true, 1, nrows);
+              else if (Cc == 96) VSB_DWC(96, 8, false, spb, nstrips);
+              else if (Cc == 192) VSB_DWC(192, 8, false, spb, nstrips);
+              else if (Cc == 384) VSB_DWC(384, 8, false, spb, nstrips);
+              else VSB_DWC(768, 8, false, spb, nstrips);
             }
 #undef VSB_DWC
             VSB_CUDA(cudaGetLastError());
@@ -1186,17 +1156,10 @@ class Model {
     // slice as soon as its copy has landed, the D2H of a slice's watermarked frames starts as soon as its embed() is done and
     // runs under the following compute; detect() runs once 64 frames have accumulated (full-size extractor batches) and on the tail.
     // Exposed copies: the first slice in and the last group's logits out.
-    // Slice sizes: the FIRST slice's copy is the exposed one, so it may be shorter than the rest (VSB_E2E_SL0 / VSB_E2E_SL1, read per
-    // call so that one process can compare settings).  Measured at 64 x 3x256x256 (tests/e2e_ab.py, results bit-identical for every
-    // setting): 32/32 7 165 f/s, 24/40 7 207, 16/48 7 317, 8/56 7 310, 16/24 7 020 -> defaults 16 / 48.
+    // Slice sizes: the FIRST slice's copy is the exposed one, so it is shorter than the rest.  Measured at 64 x 3x256x256 (results
+    // bit-identical for every setting): first/rest 32/32 7 165 f/s, 24/40 7 207, 16/48 7 317, 8/56 7 310, 16/24 7 020 -> 16 / 48.
     const int unit = (video_mode == VSB_VIDEO_INTERPOLATE && step > 1) ? step * std::max(1, chunk_keys) : step;
-    auto knob = [&](const char* name, int dflt) {
-      const char* e = getenv(name);
-      int v = e ? atoi(e) : dflt;
-      if (v < 1 || v > kMaxBatch) v = dflt;
-      return ((v + unit - 1) / unit) * unit;
-    };
-    const int sl0 = knob("VSB_E2E_SL0", 16), sl1 = knob("VSB_E2E_SL1", 48);
+    const int sl0 = (16 + unit - 1) / unit * unit, sl1 = (48 + unit - 1) / unit * unit;
     std::vector<std::pair<int, int>> slices;   // (first frame, frames)
     for (int f0 = 0; f0 < F;) {
       const int n = std::min(slices.empty() ? sl0 : sl1, F - f0);
@@ -1410,10 +1373,9 @@ class Model {
     const bool fastup = bp.identity_resample || (bp.tab.maxt_x <= 2 && bp.tab.maxt_y <= 2 && bp.H >= bp.PH && bp.W >= bp.PW);
     VSB_CHECK(bp.CD == 1 || bp.CD == 3, "delta must have 1 or 3 channels");
     // TMA-fed kernel (jnd_blend3_kernel): vector layout, delta in place or <= 2 taps per axis; the delta tile needs a TMA-legal row pitch
-    static const bool blend_old = getenv("VSB_BLEND_OLD") != nullptr;
     const bool delta_tma = bp.identity_resample || (bp.PW % 4 == 0 && reinterpret_cast<uintptr_t>(bp.delta) % 16 == 0);
     // (boxes never exceed the tensor they are cut from: tiny frames / processing sizes take the load-then-compute kernel)
-    const bool tma = vec && fastup && delta_tma && !blend_old && bp.W >= kB2LP && bp.H >= kB2TH + 4 &&
+    const bool tma = vec && fastup && delta_tma && bp.W >= kB2LP && bp.H >= kB2TH + 4 &&
                      (bp.identity_resample || (bp.PW >= kB3DW && bp.PH >= kB2DH)) &&
                      (!bp.identity_resample || (bp.PW % 4 == 0 && reinterpret_cast<uintptr_t>(bp.delta) % 16 == 0));
     CUtensorMap tmI, tmD;

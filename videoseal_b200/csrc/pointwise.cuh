@@ -6,7 +6,6 @@
 //   K9  stem_ln_kernel         ConvNeXt stem conv k4 (stride 4 / 2) + channels-first LayerNorm
 //   K4  dwconv7_ln_kernel      depthwise 7x7 + channels-last LayerNorm -> fp16 GEMM operand
 //   K4b ln_rows_kernel         per-pixel LayerNorm over C (downsample layers) -> fp16
-//   K2c grn_scale_kernel       GRN statistics -> per-(sample, channel) multiplier
 //   K8  head_pool_kernel / head_linear_kernel   LN + GELU + spatial mean, then Linear(C -> 1 + nbits)
 #pragma once
 #include <type_traits>
@@ -753,23 +752,18 @@ template <int C, int STRIP, bool FULLROW>
 __global__ void __launch_bounds__(768) dwconv7_ln_c_kernel(const float* __restrict__ x, int B, int H, int W,
                                                            const float* __restrict__ wdw /*[49][C]*/, const float* __restrict__ bdw,
                                                            const float* __restrict__ lnw, const float* __restrict__ lnb,
-                                                           __half* __restrict__ out, int ld_out, int spb, int ngroups, int rpb) {
+                                                           __half* __restrict__ out, int ld_out, int spb, int ngroups) {
   constexpr int C2 = C / 2, KP = (C + 63) / 64;
   extern __shared__ float pre[];  // [spb][STRIP][C]
   const int strips_x = (W + STRIP - 1) / STRIP;
   const int ls = threadIdx.x / C2;                 // local strip
   const int cp = threadIdx.x - ls * C2;            // channel pair
-  // A block owns `spb` strip columns and walks `rpb` consecutive output rows of each: 6 of the 7 input rows of a strip are
-  // those of the row above, so they come out of L1 instead of L2 (the one-row-per-block version re-read every input 12x
-  // from L2, 3.6 TB/s of L2->SM traffic at 96@64^2)
-  const int ygroups = H / rpb;
+  // A block owns `spb` strips of one output row each (group = (b*H + oy) * strips_x + strip column)
   const unsigned group = blockIdx.x * (unsigned)spb + (unsigned)ls;
   const unsigned tg = group / (unsigned)strips_x;
   const int sx = (int)(group - tg * (unsigned)strips_x);
-  const int b = (int)(tg / (unsigned)ygroups), yg = (int)(tg - (unsigned)b * (unsigned)ygroups);
-  for (int it = 0; it < rpb; ++it) {
+  const int b = (int)(tg / (unsigned)H), oy = (int)(tg - (unsigned)b * (unsigned)H);
   if (ls < spb && group < (unsigned)ngroups) {
-    const int oy = yg * rpb + it;
     const int ox0 = sx * STRIP;
     const int c = cp * 2;
     float2 acc[STRIP];
@@ -804,10 +798,8 @@ __global__ void __launch_bounds__(768) dwconv7_ln_c_kernel(const float* __restri
     const int l2 = item / STRIP, i = item - l2 * STRIP;
     const unsigned st2 = blockIdx.x * (unsigned)spb + (unsigned)l2;
     if (st2 >= (unsigned)ngroups) continue;
-    const unsigned tg2 = st2 / (unsigned)strips_x;
-    const int sx2 = (int)(st2 - tg2 * (unsigned)strips_x);
-    const int b2 = (int)(tg2 / (unsigned)ygroups);
-    const unsigned t2 = (unsigned)b2 * (unsigned)H + (tg2 - (unsigned)b2 * (unsigned)ygroups) * (unsigned)rpb + (unsigned)it;   // b*H + oy
+    const unsigned t2 = st2 / (unsigned)strips_x;   // b*H + oy
+    const int sx2 = (int)(st2 - t2 * (unsigned)strips_x);
     const int ox = sx2 * STRIP + i;
     if (ox >= W) continue;
     const float2* pr2 = reinterpret_cast<const float2*>(pre + ((size_t)l2 * STRIP + i) * C);
@@ -842,8 +834,6 @@ __global__ void __launch_bounds__(768) dwconv7_ln_c_kernel(const float* __restri
       }
     }
   }
-  __syncthreads();   // `pre` is rewritten by the next row
-  }  // rows of the block
 }
 
 
@@ -864,34 +854,6 @@ __global__ void __launch_bounds__(256) ln_rows_kernel(const float* __restrict__ 
     for (int o = 16; o; o >>= 1) var += __shfl_xor_sync(0xffffffffu, var, o);
     const float rstd = 1.0f / sqrtf(var / (float)C + eps);
     for (int c = lane; c < C; c += 32) out[m * ld_out + c] = __float2half_rn((r[c] - mean) * rstd * __ldg(w + c) + __ldg(bvec + c));
-  }
-}
-
-// K2c: GRN (common.py:166-169) folded into a per-(sample, k) multiplier of pwconv2's A operand:
-//   Gx = sqrt(sum_{h,w} g^2);  Nx = Gx / (mean_k Gx + 1e-6);  scale = gamma * Nx + 1   (beta is folded into pwconv2's bias)
-// stats: [B, K] sums of squares (zeroed again here for the next use).  One block per sample.
-__global__ void __launch_bounds__(256) grn_scale_kernel(float* __restrict__ stats, const float* __restrict__ gamma, int K,
-                                                        float* __restrict__ scale, int ld_scale) {
-  __shared__ float red[8];
-  __shared__ float mean_s;
-  const int b = blockIdx.x;
-  float* st = stats + (long)b * K;
-  float sum = 0.f;
-  for (int k = threadIdx.x; k < K; k += blockDim.x) sum += sqrtf(st[k]);
-#pragma unroll
-  for (int o = 16; o; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = sum;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float t = 0.f;
-    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) t += red[i];
-    mean_s = t / (float)K;
-  }
-  __syncthreads();
-  const float inv = 1.0f / (mean_s + 1e-6f);
-  for (int k = threadIdx.x; k < K; k += blockDim.x) {
-    scale[(long)b * ld_scale + k] = __ldg(gamma + k) * (sqrtf(st[k]) * inv) + 1.0f;
-    st[k] = 0.f;
   }
 }
 

@@ -28,22 +28,14 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
-// ---------------------------------------------------------------- programmatic dependent launch (build with -DVSB_PDL)
+// ---------------------------------------------------------------- programmatic dependent launch
 // A kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may start while its predecessor on the stream
 // is still draining: everything before pdl_wait() (barrier init, descriptor prefetch, constant weights)
 // overlaps the predecessor's tail; pdl_wait() returns once the predecessor grid has completed and its writes are
 // visible (immediately when the kernel was launched the classic way).  pdl_launch_dependents() lets the successor
 // start its own prologue as soon as every CTA of this grid has passed it.
-__device__ __forceinline__ void pdl_wait() {
-#ifdef VSB_PDL
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-#endif
-}
-__device__ __forceinline__ void pdl_launch_dependents() {
-#ifdef VSB_PDL
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-#endif
-}
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {

@@ -251,7 +251,7 @@ int vsb_debug_conv(const vsb_conv_test* t, void* stream) {
   ConvGemmOp op;
   const int Ct = t->C0 + t->C1;
   int K = t->R * t->S * Ct;
-  if (t->loader == LD_HALO_UPS || t->loader == LD_HALO_CONV3) K = halo_kpad(t->C0, t->C1);  // weights in halo layout
+  if (t->loader == LD_HALO_CONV3) K = halo_kpad(t->C0, t->C1);  // weights in halo layout
   int OH, OW;
   const int ld0 = t->ld0 ? t->ld0 : t->C0, ld_out = t->ld_out ? t->ld_out : t->N;
   if (t->loader == LD_TMA) {
@@ -263,15 +263,10 @@ int vsb_debug_conv(const vsb_conv_test* t, void* stream) {
     OW = (t->IW + 2 * t->pad - t->S) / t->stride + 1;
     setup_gather_conv(op, LD_GATHER_CONV, (const __half*)t->src0, t->C0, ld0, (const __half*)t->src1, t->C1, t->C1, t->B, t->IH, t->IW, OH, OW,
                       t->R, t->S, t->stride, t->pad, t->pad_mode);
-  } else if (t->loader == LD_HALO_UPS) {
-    OH = 2 * t->IH; OW = 2 * t->IW;
-    setup_halo_ups(op, (const __half*)t->src0, t->C0, t->C0, (const __half*)t->src1, t->C1, t->C1, t->B, t->IH, t->IW);
-  } else if (t->loader == LD_HALO_CONV3) {
+  } else {
+    VSB_CHECK(t->loader == LD_HALO_CONV3, "bad loader");
     OH = t->IH; OW = t->IW;
     setup_halo_conv3(op, (const __half*)t->src0, t->B, t->IH, t->IW, t->C0, t->C0);
-  } else {
-    OH = t->IH; OW = t->IW;
-    setup_gather_scale(op, (const __half*)t->src0, (long)t->B * t->IH * t->IW, t->C0, t->C0, t->a_scale, t->C0, t->rows_per_sample);
   }
   ConvGemmParams& p = op.p;
   p.epi = t->epi; p.act = t->act; p.bias = t->bias;
