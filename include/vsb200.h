@@ -72,6 +72,12 @@ int vsb_version(void);
 int vsb_model_create(const vsb_model_desc* desc, vsb_model** out);
 /* one state_dict entry, fp32, host memory, contiguous; `name` is the reference state_dict key */
 int vsb_model_set_tensor(vsb_model* m, const char* name, const float* data, const int64_t* shape, int32_t ndim);
+/* Pixel-wise extractor head (modules/pixel_decoder.py:44-83 with pixelwise=True), called between create and finalize.  Without
+ * this call the model has the pooled head (one [1+nbits] logit vector per frame).  pixelwise = 1 needs 1..8 stage factors, each 2
+ * or 4, and a ConvNeXt trunk with ext_stem_stride 4; stage i maps C -> C / factors[i] channels (bilinear up-sampling, reflect-padded
+ * 3x3 conv, LayerNorm, GELU), then a 1x1 conv gives 1+nbits maps.  pixelwise = 0 accepts only n_stages = 1, factors = {1} (the
+ * pooled head).  VSB_ERR_STATE after finalize; VSB_ERR_INVALID / VSB_ERR_UNSUPPORTED for other values. */
+int vsb_model_set_pixel_decoder(vsb_model* m, int32_t n_stages, const int32_t* factors, int32_t pixelwise);
 /* fold BN, pack to fp16 KRSC, upload to `device`, build nothing else (plans are built lazily per batch shape) */
 int vsb_model_finalize(vsb_model* m, int32_t device);
 void vsb_model_destroy(vsb_model* m);
@@ -91,7 +97,11 @@ int vsb_embed(vsb_model* m, const float* imgs_dev, const uint8_t* msgs_dev, int3
 int vsb_embedder_forward(vsb_model* m, const float* x_dev, const uint8_t* msgs_dev, int32_t n_msgs, float* delta_dev,
                          int32_t B, void* stream);
 
-/* imgs_dev [F,3,H,W] -> logits_dev [F, 1+nbits] */
+/* imgs_dev [F,3,H,W] -> logits_dev [F, 1+nbits]; for a pixel-wise model (vsb_model_set_pixel_decoder) logits_dev is
+ * [F, 1+nbits, P, P] fp32 NCHW with P = (img_size / 32) * prod(factors), i.e. img_size for upscale_stages [4, 4, 2]:
+ * channel 0 is the detection map, channels 1.. the per-pixel message bits (the reference's "b (1+nbits) h w").
+ * The same shape applies to vsb_detect_host.  vsb_embed_detect_host and vsb_frames_host_u8 with logits_host != NULL
+ * return VSB_ERR_UNSUPPORTED for pixel-wise models. */
 int vsb_detect(vsb_model* m, const float* imgs_dev, float* logits_dev, int32_t F, int32_t H, int32_t W, int32_t flags,
                void* stream);
 

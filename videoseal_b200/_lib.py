@@ -10,7 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("VSB200_LIB") or os.path.join(_HERE, "libvsb200.so")
 
 EXPORTS = [
-    "vsb_last_error", "vsb_version", "vsb_model_create", "vsb_model_set_tensor", "vsb_model_finalize",
+    "vsb_last_error", "vsb_version", "vsb_model_create", "vsb_model_set_tensor", "vsb_model_set_pixel_decoder", "vsb_model_finalize",
     "vsb_model_destroy", "vsb_embed", "vsb_embedder_forward", "vsb_detect", "vsb_jnd_heatmaps", "vsb_embed_host",
     "vsb_detect_host", "vsb_embed_detect_host", "vsb_frames_host_u8", "vsb_launch_count", "vsb_profile_enable", "vsb_profile_read", "vsb_debug_get_tensor", "vsb_debug_conv",
     "vsb_debug_resample_table",
@@ -61,6 +61,7 @@ def lib():
     L.vsb_version.restype = C.c_int
     L.vsb_model_create.argtypes = [C.POINTER(ModelDesc), C.POINTER(C.c_void_p)]
     L.vsb_model_set_tensor.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.POINTER(C.c_int64), C.c_int32]
+    L.vsb_model_set_pixel_decoder.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_int32]
     L.vsb_model_finalize.argtypes = [C.c_void_p, C.c_int32]
     L.vsb_model_destroy.argtypes = [C.c_void_p]
     L.vsb_model_destroy.restype = None

@@ -81,15 +81,28 @@ def spec_from_card(card: dict) -> dict:
         raise NotImplementedError("only additive blending is implemented (all shipped cards use it)")
     ep = card["extractor"]["params"]
     pd = ep.get("pixel_decoder", {})
-    if pd.get("pixelwise", False) or list(pd.get("upscale_stages", [1])) != [1] or pd.get("sigmoid_output", False):
-        raise NotImplementedError("pixel decoder: only pixelwise=False, upscale_stages=[1], sigmoid_output=False")
+    pixelwise = bool(pd.get("pixelwise", False))
+    stages = [int(f) for f in pd.get("upscale_stages", [1])]
+    if pd.get("sigmoid_output", False):
+        raise NotImplementedError("pixel decoder: sigmoid_output=True is not implemented")
+    if not pixelwise and stages != [1]:
+        raise NotImplementedError("pixel decoder: a pooled (pixelwise=False) decoder needs upscale_stages=[1]")
+    if pixelwise and (not stages or any(f not in (2, 4) for f in stages)):
+        raise NotImplementedError(f"pixel decoder: pixel-wise upscale_stages must be factors of 2 or 4, got {stages}")
+    # modules/common.py:36-66: 'nearest', 'conv' and 'pixelshuffle' have other arithmetic (the first even the same weights)
+    if pixelwise and str(pd.get("upscale_type", "bilinear")) != "bilinear":
+        raise NotImplementedError(f"pixel decoder: upscale_type '{pd.get('upscale_type')}' is not implemented (only 'bilinear')")
     enc = ep["encoder"]
+    if pixelwise and (ep.get("proportional_dim", False) or int(enc.get("stem_stride", 4)) != 4):
+        raise NotImplementedError("pixel decoder: pixel-wise maps need a non-proportional ConvNeXt trunk with stem_stride 4")
     dims = [int(x) for x in enc["dims"]]
     if ep.get("proportional_dim", False):
         mult = math.sqrt(nbits / 128)
         dims = [int(x * mult) for x in dims]
     if enc.get("temporal_convs", False) or enc.get("temporal_attention", False):
         raise NotImplementedError("temporal ConvNeXt variants are out of scope")
+    if pixelwise:
+        check_pixel_decoder(dims[-1], stages, int(img_size), nbits)
     att = str(a.get("attenuation", "None"))
     jnd = (0, 0)
     if att.lower().startswith("jnd"):
@@ -107,8 +120,37 @@ def spec_from_card(card: dict) -> dict:
             "last_tanh": bool(u.get("last_tanh", True)),
         },
         "convnext": {"depths": [int(x) for x in enc["depths"]], "dims": dims, "stem_stride": int(enc.get("stem_stride", 4))},
+        "pixel_decoder": {"pixelwise": pixelwise, "upscale_stages": stages},
         "jnd": jnd, "attenuation": att,
     }
+
+
+def check_pixel_decoder(c: int, stages: list, img_size: int, nbits: int) -> None:
+    """Widths and sizes the native pixel-wise decoder implements (model.cuh:add_pixel_decoder), checked at load time.  Stage i maps
+    c -> c // f_i channels (pixel_decoder.py:44-50).  The stage GEMM takes c in {16, 32} or >= 64 as its first input; every output
+    width is a multiple of 8, of the form 8 * {1, 3} * 2^k (k <= 5) for a middle stage, and at most 32 for the last one, whose
+    kernel holds one pixel's channels in registers.  The last stage's map must tile by 16 / f pixels, and its shared memory (the
+    staged taps plus the fp32 head weights) must fit in one H100 block."""
+    if not (c in (16, 32) or c >= 64):
+        raise NotImplementedError(f"pixel decoder: a trunk width of {c} is not implemented (16, 32 or >= 64)")
+    h = (img_size - 4) // 4 + 1
+    for _ in range(3):
+        h = (h - 2) // 2 + 1
+    for i, f in enumerate(stages):
+        co, last = c // f, i == len(stages) - 1
+        if c % f or co % 8:
+            raise NotImplementedError(f"pixel decoder: stage {i} maps {c} -> {c / f:g} channels; widths must be multiples of 8")
+        if last:
+            if co > 32:
+                raise NotImplementedError(f"pixel decoder: the last stage has {co} channels; at most 32 are implemented")
+            t = 16 // f
+            smem = (t + 2) ** 2 * 9 * co * 2 + (1 + nbits) * (co + 1) * 4
+            if h % t or smem > 227 * 1024:
+                raise NotImplementedError(f"pixel decoder: a last stage on a {h}-pixel map with {co} channels and {nbits} bits is not "
+                                          "implemented (the map must be a multiple of 16 / f; head weights must fit in shared memory)")
+        elif not any(co % (8 * v) == 0 and co // (8 * v) <= 32 and (co // (8 * v)) & (co // (8 * v) - 1) == 0 for v in (1, 3)):
+            raise NotImplementedError(f"pixel decoder: stage {i} has {co} channels; middle stages take 8 * {{1, 3}} * 2^k, k <= 5")
+        c, h = co, h * f
 
 
 def setup_model(card: dict, ckpt_path):

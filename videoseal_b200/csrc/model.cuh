@@ -96,6 +96,7 @@ struct Plan {
   float* x_res = nullptr;   // [B,3,S,S] resized RGB when the input is not at processing size
   float* delta = nullptr;   // [B,CD,S,S]
   float* logits = nullptr;  // [B,1+K]
+  float* out_maps = nullptr;  // pixel-wise detect plans: the caller's [B,1+K,P,P] slice, set per call
   void run(cudaStream_t st) {
     if (!g_profile.enabled) {
       for (auto& s : steps) { s.fn(st); g_launches += s.launches; }
@@ -227,6 +228,52 @@ inline void launch_dw_ring(const DwRingOp& op, cudaStream_t st) {
   else launch_dw_ring_t<192, 1, 4, 8>(op, st);
 }
 
+// Pixel-decoder gather launches (pointwise.cuh K3 with F in {2, 4} and GELU).  kPdMaxSmem: the opt-in shared memory of one H100 block.
+constexpr size_t kPdMaxSmem = 227 * 1024;
+template <int VPT, int F>
+inline void launch_pd_stage_t(bool tiled, size_t smem, const __half* y, int B, int IH, int C, const float* lw, const float* lb, __half* out,
+                              int ld_out, int num_sms, cudaStream_t st) {
+  if (tiled) {
+    static bool attr = false;
+    if (!attr) { VSB_CUDA(cudaFuncSetAttribute(ups_gather_ln_tiled_kernel<VPT, F, kUpGelu, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPdMaxSmem)); attr = true; }
+    const int tiles = IH / (16 / F);
+    ups_gather_ln_tiled_kernel<VPT, F, kUpGelu, false><<<(unsigned)((long)B * tiles * tiles), 256, smem, st>>>(y, B, IH, IH, C, lw, lb, 1e-6f, out, ld_out);
+  } else {
+    const int ppb = 256 / (C / (8 * VPT));
+    const long npix = (long)B * F * IH * F * IH;
+    const unsigned grid = (unsigned)std::min<long>((npix + ppb - 1) / ppb, (long)num_sms * 32);
+    ups_gather_ln_kernel<VPT, F, kUpGelu><<<grid, 256, 0, st>>>(y, B, IH, IH, C, lw, lb, 1e-6f, out, ld_out);
+  }
+  VSB_CUDA(cudaGetLastError());
+}
+inline void launch_pd_stage(int F, int vpt, bool tiled, size_t smem, const __half* y, int B, int IH, int C, const float* lw, const float* lb,
+                            __half* out, int ld_out, int num_sms, cudaStream_t st) {
+  if (F == 2 && vpt == 1) launch_pd_stage_t<1, 2>(tiled, smem, y, B, IH, C, lw, lb, out, ld_out, num_sms, st);
+  else if (F == 2 && vpt == 3) launch_pd_stage_t<3, 2>(tiled, smem, y, B, IH, C, lw, lb, out, ld_out, num_sms, st);
+  else if (F == 4 && vpt == 1) launch_pd_stage_t<1, 4>(tiled, smem, y, B, IH, C, lw, lb, out, ld_out, num_sms, st);
+  else if (F == 4 && vpt == 3) launch_pd_stage_t<3, 4>(tiled, smem, y, B, IH, C, lw, lb, out, ld_out, num_sms, st);
+  else throw Error("pixel decoder: no gather kernel for this stage", kErrUnsupported);
+}
+template <int VPT, int F>
+inline void launch_pd_head_t(size_t smem, const __half* y, int B, int IH, int C, const float* lw, const float* lb, const float* hw,
+                             const float* hb, int NO, float* maps, cudaStream_t st) {
+  static bool attr = false;
+  if (!attr) { VSB_CUDA(cudaFuncSetAttribute(ups_gather_ln_tiled_kernel<VPT, F, kUpGelu, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPdMaxSmem)); attr = true; }
+  const int tiles = IH / (16 / F);
+  ups_gather_ln_tiled_kernel<VPT, F, kUpGelu, true><<<(unsigned)((long)B * tiles * tiles), 256, smem, st>>>(
+      y, B, IH, IH, C, lw, lb, 1e-6f, nullptr, 0, hw, hb, NO, maps);
+  VSB_CUDA(cudaGetLastError());
+}
+// the last stage: C = 8 * VPT channels (G = 1: one thread per output pixel), VPT 1..4
+inline void launch_pd_head(int F, int vpt, size_t smem, const __half* y, int B, int IH, int C, const float* lw, const float* lb, const float* hw,
+                           const float* hb, int NO, float* maps, cudaStream_t st) {
+#define VSB_PDH(V, FF) if (F == FF && vpt == V) return launch_pd_head_t<V, FF>(smem, y, B, IH, C, lw, lb, hw, hb, NO, maps, st)
+  VSB_PDH(1, 2); VSB_PDH(2, 2); VSB_PDH(3, 2); VSB_PDH(4, 2);
+  VSB_PDH(1, 4); VSB_PDH(2, 4); VSB_PDH(3, 4); VSB_PDH(4, 4);
+#undef VSB_PDH
+  throw Error("pixel-wise head: no kernel for this width", kErrUnsupported);
+}
+
 class Model {
  public:
   vsb_model_desc d;
@@ -259,6 +306,13 @@ class Model {
   std::vector<std::vector<CnBlockW>> cn;
   ConvW head_conv;
   float *head_lnw = nullptr, *head_lnb = nullptr, *head_lw = nullptr, *head_lb = nullptr;
+  // pixel-wise decoder (vsb_model_set_pixel_decoder; pixel_decoder.py:44-83): stage i = bilinear x pd_factors[i], reflect-padded 3x3
+  // conv C -> C / f, LayerNorm, GELU; then the 1x1 conv head C_last -> 1 + nbits per pixel
+  bool pixelwise = false;
+  std::vector<int> pd_factors;
+  struct PdStageW { ConvW taps; float* lnw; float* lnb; int cin, cout, kin; };
+  std::vector<PdStageW> pd;
+  float *pd_hw = nullptr, *pd_hb = nullptr;   // fp32 [1+nbits][C_last], [1+nbits]
 
   // grow-only device staging for the host-buffer entry points (no cudaMalloc on the steady-state path)
   struct Staging { void* p = nullptr; size_t cap = 0; };
@@ -285,6 +339,51 @@ class Model {
   Plan* last_plan = nullptr;
 
   explicit Model(const vsb_model_desc& desc) : d(desc) {}
+
+  void set_pixel_decoder(int n, const int32_t* f, int pw) {
+    if (finalized) throw Error("model already finalized", kErrState);
+    VSB_CHECK(pw == 0 || pw == 1, "pixelwise must be 0 or 1");
+    VSB_CHECK(n >= 1 && n <= 8, "pixel decoder: 1 to 8 upscale stages");
+    for (int i = 0; i < n; ++i) VSB_CHECK(f[i] >= 1, "pixel decoder: upscale factors must be positive");
+    if (!pw) {
+      if (n != 1 || f[0] != 1) throw Error("pooled pixel decoder: only upscale_stages [1] is implemented", kErrUnsupported);
+      pixelwise = false;
+      pd_factors.clear();
+      return;
+    }
+    for (int i = 0; i < n; ++i)
+      if (f[i] != 2 && f[i] != 4) throw Error("pixel-wise decoder: upscale factors must be 2 or 4", kErrUnsupported);
+    if (d.ext_stem_stride != 4) throw Error("pixel-wise decoder: needs a ConvNeXt trunk with stem stride 4", kErrUnsupported);
+    pixelwise = true;
+    pd_factors.assign(f, f + n);
+  }
+  // side of the trunk's last feature map: stem k4 / stride st, then three k2 s2 downsampling layers
+  int trunk_map() const {
+    int h = (d.img_size - 4) / d.ext_stem_stride + 1;
+    for (int s = 1; s < 4; ++s) h = (h - 2) / 2 + 1;
+    return h;
+  }
+  // floats vsb_detect writes per frame: 1+nbits logits, or 1+nbits maps of P x P for a pixel-wise model
+  size_t detect_out_per_frame() const {
+    size_t P = (size_t)trunk_map();
+    for (int f : pd_factors) P *= f;
+    return pixelwise ? (size_t)(1 + d.nbits) * P * P : (size_t)(1 + d.nbits);
+  }
+  void check_pooled_head(const std::string& what) const {
+    if (pixelwise) throw Error(what + ": per-pixel maps of a streamed video are not implemented (use vsb_detect / vsb_detect_host)", kErrUnsupported);
+  }
+  // K of a pixel-decoder stage GEMM over C input channels: the TMA GEMM loader takes K in {16, 32} or >= 64, narrower widths
+  // are zero-padded (in the packed weights and in the pitch of the activation buffer, whose pad channels are zeroed once)
+  static int pd_gemm_k(int C) { return (C == 16 || C == 32 || C >= 64) ? C : (C < 16 ? 16 : (C < 32 ? 32 : 64)); }
+  // 16-byte channel vectors per gather thread for a non-final stage of C channels: C = 8 * VPT * G, G a power of two <= 32
+  static int pd_vpt(int C) {
+    for (int v : {1, 3}) {
+      if (C % (8 * v)) continue;
+      const int g = C / (8 * v);
+      if (g <= 32 && (g & (g - 1)) == 0) return v;
+    }
+    return 0;
+  }
 
   const HostTensor& get(const std::string& k) const {
     auto it = sd.find(k);
@@ -349,16 +448,18 @@ class Model {
     return cw;
   }
   // UBlock up-conv as a low-resolution tap GEMM (see ups_gather_ln_kernel): rows n' = tap*Cout + co, K = concat channels
-  ConvW pack_upconv_taps(const std::string& wkey, const std::vector<float>& in_scale) {
+  // (zero-padded to Kp columns when Kp > Ct: the pixel decoder's narrow stage inputs, see pd_gemm_k)
+  ConvW pack_upconv_taps(const std::string& wkey, const std::vector<float>& in_scale, int Kp = 0) {
     const HostTensor& w = get(wkey);
     VSB_CHECK(w.shape.size() == 4 && w.shape[2] == 3 && w.shape[3] == 3, "up conv weight shape");
     const int Co = (int)w.shape[0], Ct = (int)w.shape[1];
-    std::vector<float> p((size_t)9 * Co * Ct);
+    if (Kp < Ct) Kp = Ct;
+    std::vector<float> p((size_t)9 * Co * Kp, 0.f);
     for (int co = 0; co < Co; ++co)
       for (int c = 0; c < Ct; ++c)
-        for (int t = 0; t < 9; ++t) p[((size_t)t * Co + co) * Ct + c] = w.data[((size_t)co * Ct + c) * 9 + t] * in_scale[c];
+        for (int t = 0; t < 9; ++t) p[((size_t)t * Co + co) * Kp + c] = w.data[((size_t)co * Ct + c) * 9 + t] * in_scale[c];
     ConvW cw;
-    cw.N = 9 * Co; cw.K = Ct;
+    cw.N = 9 * Co; cw.K = Kp;
     cw.w = wpool.upload(to_half(p));
     return cw;
   }
@@ -572,7 +673,33 @@ class Model {
         cn[s].push_back(w);
       }
     }
-    {
+    if (pixelwise) {
+      const std::string D = "detector.pixel_decoder.";
+      int c = d.ext_dims[3];
+      for (size_t i = 0; i < pd_factors.size(); ++i) {
+        const std::string K = D + "output_upscaling." + std::to_string(i) + ".upsample_block.";
+        const int f = pd_factors[i], co = c / f;
+        const bool last = i + 1 == pd_factors.size();
+        const HostTensor& w = get(K + "2.weight");
+        VSB_CHECK(w.shape.size() == 4 && (int)w.shape[0] == co && (int)w.shape[1] == c && w.shape[2] == 3 && w.shape[3] == 3,
+                  "pixel decoder stage " + std::to_string(i) + ": weight must be [C/f, C, 3, 3]");
+        if (co % 8 != 0 || (last ? co > 32 : pd_vpt(co) == 0) || (i == 0 && pd_gemm_k(c) != c))
+          throw Error("pixel decoder: stage width " + std::to_string(c) + " -> " + std::to_string(co) + " is not implemented (widths must be "
+                      "multiples of 8 of the form 8 * {1,3} * 2^k, the last one at most 32)", kErrUnsupported);
+        PdStageW sw;
+        sw.cin = c; sw.cout = co; sw.kin = pd_gemm_k(c);
+        sw.taps = pack_upconv_taps(K + "2.weight", std::vector<float>(c, 1.f), sw.kin);
+        sw.lnw = wpool.upload(get(K + "3.weight").data);
+        sw.lnb = wpool.upload(get(K + "3.bias").data);
+        pd.push_back(sw);
+        c = co;
+      }
+      const HostTensor& lw = get(D + "linear.weight");
+      VSB_CHECK(lw.shape.size() == 4 && (int)lw.shape[0] == 1 + d.nbits && (int)lw.shape[1] == c && lw.shape[2] == 1 && lw.shape[3] == 1,
+                "pixel-wise head: linear.weight must be [1+nbits, C, 1, 1]");
+      pd_hw = wpool.upload(lw.data);
+      pd_hb = wpool.upload(get(D + "linear.bias").data);
+    } else {
       const std::string D = "detector.pixel_decoder.";
       head_conv = pack_conv(D + "output_upscaling.0.upsample_block.2.weight", nullptr, {}, nullptr, /*pad_taps=*/true);
       head_lnw = wpool.upload(get(D + "output_upscaling.0.upsample_block.3.weight").data);
@@ -1058,7 +1185,9 @@ class Model {
       dbg(pl, "stage" + std::to_string(s), x, 0, B, hs, hs, C, Cp);
     }
     // ---- head (pixel_decoder.py:61-83)
-    {
+    if (pixelwise) {
+      add_pixel_decoder(pl, x16, B, hs, Cp);
+    } else {
       const long M = (long)B * hs * hs;
       float* y = pl.pool.alloc_n<float>(M * Cp);
       ConvGemmOp op;
@@ -1084,6 +1213,53 @@ class Model {
     detect_plans[B] = std::move(up);
     evict_plans(detect_plans, ret);
     return ret;
+  }
+
+  // Pixel-wise decoder stages.  Each stage is one tensor-core GEMM at the LOW resolution, Y[p, tap*C_out + co] (the tap trick of the
+  // U-Net's up-convolutions: bilinear up-sampling, reflection padding and the 3x3 taps are linear, so the channel mixing commutes
+  // with the spatial gather), then ups_gather_ln_*_kernel forms each output pixel from 9 taps x 4 bilinear corners + LN + GELU.
+  // The last stage's kernel also applies the 1x1 head and writes the 1+K NCHW maps straight into the caller's buffer (plp->out_maps):
+  // the full-resolution activation never goes to HBM.
+  void add_pixel_decoder(Plan& pl, const __half* x, int B, int h, int ldx) {
+    Plan* plp = &pl;
+    const int NO = 1 + d.nbits, nsm = num_sms;
+    for (size_t i = 0; i < pd.size(); ++i) {
+      const PdStageW& s = pd[i];
+      const int F = pd_factors[i], ho = F * h, Co = s.cout, IH = h, T = 16 / F;
+      const bool last = i + 1 == pd.size();
+      const long Mi = (long)B * h * h;
+      __half* ytap = pl.pool.alloc_n<__half>(Mi * 9 * Co);
+      ConvGemmOp op; setup_tma_gemm(op, x, Mi, s.kin, ldx);
+      op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.out16 = ytap; op.p.ld_out16 = 9 * Co;
+      add_conv(pl, op, s.taps, "pd.uptap1x1." + std::to_string(s.cin) + "-" + std::to_string(9 * Co) + "@" + std::to_string(h));
+      const float *lw = s.lnw, *lb = s.lnb;
+      const size_t tsmem = (size_t)(T + 2) * (T + 2) * 9 * Co * sizeof(__half);
+      const std::string tag = std::to_string(Co) + "x" + std::to_string(F) + "@" + std::to_string(ho);
+      if (last) {
+        const size_t smem = tsmem + (size_t)NO * (Co + 1) * sizeof(float);
+        if (IH % T != 0 || smem > kPdMaxSmem)
+          throw Error("pixel-wise head: a " + std::to_string(IH) + "-pixel map with " + std::to_string(NO) + " outputs is not implemented", kErrUnsupported);
+        const float *hw = pd_hw, *hb = pd_hb;
+        pl.steps.push_back(Step{[=](cudaStream_t st) {
+          launch_pd_head(F, Co / 8, smem, ytap, B, IH, Co, lw, lb, hw, hb, NO, plp->out_maps, st);
+        }, 1, "pd.gather_head." + tag});
+      } else {
+        const int ldo = pd_gemm_k(Co);
+        __half* u = pl.pool.alloc_n<__half>((long)B * ho * ho * ldo);
+        if (ldo != Co) {   // pad channels stay zero: the gather writes [0, Co)
+          VSB_CUDA(cudaMemset(u, 0, (size_t)B * ho * ho * ldo * sizeof(__half)));
+          VSB_CUDA(cudaDeviceSynchronize());
+        }
+        const bool tiled = IH % T == 0 && tsmem <= kPdMaxSmem;
+        const int vpt = pd_vpt(Co);
+        pl.steps.push_back(Step{[=](cudaStream_t st) {
+          launch_pd_stage(F, vpt, tiled, tiled ? tsmem : 0, ytap, B, IH, Co, lw, lb, u, ldo, nsm, st);
+        }, 1, std::string(tiled ? "pd.upgather." : "pd.upgather_untiled.") + tag});
+        dbg(pl, "pd" + std::to_string(i), u, 1, B, ho, ho, Co, ldo);
+        x = u; ldx = ldo;
+      }
+      h = ho;
+    }
   }
 
   ResampleDev* get_resampler(int ih, int iw, int oh, int ow, bool aa) {
@@ -1434,16 +1610,18 @@ class Model {
     const bool same = (H == S && W == S);
     const bool aa = !(flags & VSB_FLAG_RESIZE_NO_AA);
     const long fstride = (long)3 * H * W;
-    const int NO = 1 + d.nbits;
+    const size_t NO = detect_out_per_frame();
     for (int f0 = 0; f0 < F; f0 += kMaxBatch) {
       const int n = std::min(kMaxBatch, F - f0);
       Plan* pl = get_detect_plan(n);
       const float* x = imgs + (size_t)f0 * fstride;
       if (!same) { resize_frames(x, fstride, n, H, W, pl->x_res, aa, st); x = pl->x_res; }
       pl->in_imgs = x;
+      pl->out_maps = pixelwise ? logits + (size_t)f0 * NO : nullptr;   // the maps are written in place, at this sub-batch's offset
       pl->run(st);
       last_plan = pl;
-      VSB_CUDA(cudaMemcpyAsync(logits + (size_t)f0 * NO, pl->logits, (size_t)n * NO * sizeof(float), cudaMemcpyDeviceToDevice, st));
+      if (!pixelwise)
+        VSB_CUDA(cudaMemcpyAsync(logits + (size_t)f0 * NO, pl->logits, (size_t)n * NO * sizeof(float), cudaMemcpyDeviceToDevice, st));
     }
   }
 };

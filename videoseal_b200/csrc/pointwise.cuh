@@ -261,13 +261,33 @@ __global__ void __launch_bounds__(256) jnd_lowres_kernel(const float* __restrict
 //   out[b,oy,ox,co] = act(LN_c( sum_{r,s} bilinear_x2( y[.., (3r+s)*C + co] )(reflect(oy+r-1), reflect(ox+s-1)) ))
 // One group of C/8 threads per output pixel (8 channels = one 16-byte load per thread and tap corner).
 // VPT = 16-byte channel vectors per thread: C = 8 * VPT * G with G <= 32 threads per pixel (C <= 256: VPT 1; chunkyseal's
-// 512-channel first up-conv: VPT 2); thread lane_g owns the vectors lane_g + G*j.
-template <int VPT>
+// 512-channel first up-conv: VPT 2; the pixel decoder's 192 / 48 / 24: VPT 3); thread lane_g owns the vectors lane_g + G*j.
+// F = up-sampling factor (2: U-Net; 2 or 4: pixel decoder, pixel_decoder.py:44-50), ACT = kUpRelu (U-Net) or kUpGelu (pixel decoder).
+constexpr int kUpRelu = 0, kUpGelu = 1;
+
+// Source rows of row u (already reflected into [0, 4*IH)) of a bilinear x4 up-sampling with align_corners=False: rows a <= b and
+// the weight of a (src = (u + 0.5) / 4 - 0.5 clamped at 0; the weights are multiples of 1/8, exact in fp16).  Factor 2 is written
+// out in the kernels themselves, as the U-Net has always had it.
+template <int F>
+__device__ __forceinline__ void up_src(int u, int IH, int& a, int& b, float& wa) {
+  static_assert(F == 4, "factor 2 is inlined in the kernels");
+  const int i = u >> 2, p = u & 3;
+  if (p < 2) { a = max(i - 1, 0); b = i; wa = (float)(3 - 2 * p) * 0.125f; }
+  else       { a = i; b = min(i + 1, IH - 1); wa = (float)(11 - 2 * p) * 0.125f; }
+}
+
+template <int ACT>
+__device__ __forceinline__ float up_act(float v) {
+  if constexpr (ACT == kUpRelu) return fmaxf(v, 0.f);
+  else return 0.5f * v * (1.f + erff(v * 0.70710678118654752f));    // nn.GELU (exact erf), pixel_decoder.py:24
+}
+
+template <int VPT, int F = 2, int ACT = kUpRelu>
 __global__ void __launch_bounds__(256) ups_gather_ln_kernel(const __half* __restrict__ y, int B, int IH, int IW, int C,
                                                             const float* __restrict__ lnw, const float* __restrict__ lnb, float eps,
                                                             __half* __restrict__ out, int ld_out) {
   const int G = C / (8 * VPT);                // threads per pixel (power of two, <= 32)
-  const int OH = 2 * IH, OW = 2 * IW;
+  const int OH = F * IH, OW = F * IW;
   const long npix = (long)B * OH * OW;
   const int ppb = 256 / G;                    // pixels per block
   const int lane_g = threadIdx.x % G;
@@ -284,15 +304,23 @@ __global__ void __launch_bounds__(256) ups_gather_ln_kernel(const __half* __rest
       int u = oy + r - 1;
       if (u < 0) u = -u;
       if (u >= OH) u = 2 * OH - 2 - u;
-      const int i = u >> 1;
-      if (u & 1) { ya[r] = i; yb[r] = min(i + 1, IH - 1); wy[r] = 0.75f; }
-      else       { ya[r] = max(i - 1, 0); yb[r] = i; wy[r] = 0.25f; }
+      if constexpr (F == 2) {
+        const int i = u >> 1;
+        if (u & 1) { ya[r] = i; yb[r] = min(i + 1, IH - 1); wy[r] = 0.75f; }
+        else       { ya[r] = max(i - 1, 0); yb[r] = i; wy[r] = 0.25f; }
+      } else {
+        up_src<F>(u, IH, ya[r], yb[r], wy[r]);
+      }
       int v = ox + r - 1;
       if (v < 0) v = -v;
       if (v >= OW) v = 2 * OW - 2 - v;
-      const int jx = v >> 1;
-      if (v & 1) { xa[r] = jx; xb[r] = min(jx + 1, IW - 1); wx[r] = 0.75f; }
-      else       { xa[r] = max(jx - 1, 0); xb[r] = jx; wx[r] = 0.25f; }
+      if constexpr (F == 2) {
+        const int jx = v >> 1;
+        if (v & 1) { xa[r] = jx; xb[r] = min(jx + 1, IW - 1); wx[r] = 0.75f; }
+        else       { xa[r] = max(jx - 1, 0); xb[r] = jx; wx[r] = 0.25f; }
+      } else {
+        up_src<F>(v, IW, xa[r], xb[r], wx[r]);
+      }
     }
     float acc[8 * VPT];
 #pragma unroll
@@ -344,7 +372,7 @@ __global__ void __launch_bounds__(256) ups_gather_ln_kernel(const __half* __rest
 #pragma unroll
       for (int k = 0; k < 8; ++k) {
         const int c = (lane_g + j * G) * 8 + k;
-        h[k] = __float2half_rn(fmaxf((acc[8 * j + k] - mean) * rstd * __ldg(lnw + c) + __ldg(lnb + c), 0.f));
+        h[k] = __float2half_rn(up_act<ACT>((acc[8 * j + k] - mean) * rstd * __ldg(lnw + c) + __ldg(lnb + c)));
       }
       *reinterpret_cast<uint4*>(out + pix * ld_out + (lane_g + j * G) * 8) = *reinterpret_cast<const uint4*>(h);
     }
@@ -355,26 +383,38 @@ __global__ void __launch_bounds__(256) ups_gather_ln_kernel(const __half* __rest
 // the (8 + 2) x (8 + 2) low-resolution pixels x 9C channels its 36 bilinear corners touch are copied once (16-byte cp.async, rows /
 // columns clamped at the image border), then every corner is a 128-bit shared load.  The untiled kernel above re-read each
 // low-resolution vector ~16 times through L1/L2 (2.4 GB of L1 traffic for 151 MB of input at 32@128: 203 us against a 34 us bound).
-// Requires IH, IW multiples of 8.  Dynamic shared memory: 100 * 9C halves.
-template <int VPT>
+// Factor F: the tile is 16 x 16 output pixels = T x T low-resolution pixels with T = 16 / F, (T + 2)^2 of them staged.
+// Requires IH, IW multiples of T.  Dynamic shared memory: (T + 2)^2 * 9C halves (+ the head below).
+// HEAD (last pixel-decoder stage, pixel_decoder.py:76-78): the activated C = 8 * VPT channels of each pixel (G = 1) stay in
+// registers and the 1x1 conv head (hw fp32 [NO][C], hb [NO], staged in shared memory after the taps) writes the NO fp32 NCHW
+// planes `maps` [B][NO][OH][OW] directly: a warp's 32 pixels are two 16-pixel rows, i.e. two full 64-byte segments per plane.
+template <int VPT, int F = 2, int ACT = kUpRelu, bool HEAD = false>
 __global__ void __launch_bounds__(256) ups_gather_ln_tiled_kernel(const __half* __restrict__ y, int B, int IH, int IW, int C,
                                                                   const float* __restrict__ lnw, const float* __restrict__ lnb, float eps,
-                                                                  __half* __restrict__ out, int ld_out) {
+                                                                  __half* __restrict__ out, int ld_out, const float* __restrict__ hw = nullptr,
+                                                                  const float* __restrict__ hb = nullptr, int NO = 0,
+                                                                  float* __restrict__ maps = nullptr) {
+  constexpr int T = 16 / F, TS = T + 2, LT = F == 2 ? 3 : 2;   // low-resolution tile, staged tile side, log2(T)
   extern __shared__ __align__(16) uint8_t ugt_smem[];
-  __half* tile = reinterpret_cast<__half*>(ugt_smem);       // [10][10][9C]
+  __half* tile = reinterpret_cast<__half*>(ugt_smem);       // [TS][TS][9C]
   const int G = C / (8 * VPT);                // threads per pixel (power of two, <= 32)
-  const int OH = 2 * IH, OW = 2 * IW;
-  const int tiles_x = IW >> 3, tiles_y = IH >> 3;
+  const int OH = F * IH, OW = F * IW;
+  const int tiles_x = IW >> LT, tiles_y = IH >> LT;
   int t = blockIdx.x;
   const int tx = t % tiles_x; t /= tiles_x;
   const int ty = t % tiles_y;
   const int b = t / tiles_y;
-  const int I0 = ty * 8, J0 = tx * 8;          // low-resolution origin of the tile; the staged region starts at (I0 - 1, J0 - 1)
+  const int I0 = ty * T, J0 = tx * T;          // low-resolution origin of the tile; the staged region starts at (I0 - 1, J0 - 1)
   const int ldy = 9 * C, cpp = ldy >> 3;       // 16-byte chunks per low-resolution pixel
   const __half* yb_ = y + (long)b * IH * IW * ldy;
-  for (int i = threadIdx.x; i < 100 * cpp; i += 256) {
+  float* hws = reinterpret_cast<float*>(ugt_smem + (size_t)TS * TS * ldy * sizeof(__half));   // HEAD: [NO][C] then [NO]
+  if constexpr (HEAD) {
+    for (int i = threadIdx.x; i < NO * C; i += 256) hws[i] = __ldg(hw + i);
+    for (int i = threadIdx.x; i < NO; i += 256) hws[NO * C + i] = __ldg(hb + i);
+  }
+  for (int i = threadIdx.x; i < TS * TS * cpp; i += 256) {
     const int px = i / cpp, ch = i - px * cpp;
-    const int ly = px / 10, lx = px - ly * 10;
+    const int ly = px / TS, lx = px - ly * TS;
     const int gy = min(max(I0 - 1 + ly, 0), IH - 1), gx = min(max(J0 - 1 + lx, 0), IW - 1);
     cp_async16(tile + (long)px * ldy + ch * 8, yb_ + ((long)gy * IW + gx) * ldy + ch * 8);
   }
@@ -385,7 +425,7 @@ __global__ void __launch_bounds__(256) ups_gather_ln_tiled_kernel(const __half* 
   const int ppb = 256 / G;
   for (int lp = threadIdx.x / G; lp < 256; lp += ppb) {      // local output pixel of the 16 x 16 tile
     const int loy = lp >> 4, lox = lp & 15;
-    const int oy = 2 * I0 + loy, ox = 2 * J0 + lox;
+    const int oy = F * I0 + loy, ox = F * J0 + lox;
     int ya[3], yb[3], xa[3], xb[3];
     float wy[3], wx[3];
 #pragma unroll
@@ -393,16 +433,24 @@ __global__ void __launch_bounds__(256) ups_gather_ln_tiled_kernel(const __half* 
       int u = oy + r - 1;
       if (u < 0) u = -u;
       if (u >= OH) u = 2 * OH - 2 - u;
-      const int i = u >> 1;
-      if (u & 1) { ya[r] = i; yb[r] = min(i + 1, IH - 1); wy[r] = 0.75f; }
-      else       { ya[r] = max(i - 1, 0); yb[r] = i; wy[r] = 0.25f; }
+      if constexpr (F == 2) {
+        const int i = u >> 1;
+        if (u & 1) { ya[r] = i; yb[r] = min(i + 1, IH - 1); wy[r] = 0.75f; }
+        else       { ya[r] = max(i - 1, 0); yb[r] = i; wy[r] = 0.25f; }
+      } else {
+        up_src<F>(u, IH, ya[r], yb[r], wy[r]);
+      }
       ya[r] -= I0 - 1; yb[r] -= I0 - 1;           // tile rows (the clamped copies make the border rows valid)
       int v = ox + r - 1;
       if (v < 0) v = -v;
       if (v >= OW) v = 2 * OW - 2 - v;
-      const int jx = v >> 1;
-      if (v & 1) { xa[r] = jx; xb[r] = min(jx + 1, IW - 1); wx[r] = 0.75f; }
-      else       { xa[r] = max(jx - 1, 0); xb[r] = jx; wx[r] = 0.25f; }
+      if constexpr (F == 2) {
+        const int jx = v >> 1;
+        if (v & 1) { xa[r] = jx; xb[r] = min(jx + 1, IW - 1); wx[r] = 0.75f; }
+        else       { xa[r] = max(jx - 1, 0); xb[r] = jx; wx[r] = 0.25f; }
+      } else {
+        up_src<F>(v, IW, xa[r], xb[r], wx[r]);
+      }
       xa[r] -= J0 - 1; xb[r] -= J0 - 1;
     }
     float acc[8 * VPT];
@@ -418,10 +466,10 @@ __global__ void __launch_bounds__(256) ups_gather_ln_tiled_kernel(const __half* 
 #pragma unroll
         for (int j = 0; j < VPT; ++j) {
           const __half* base = tb + (r * 3 + s2) * C + j * G * 8;
-          const uint4 v00 = *reinterpret_cast<const uint4*>(base + (ya[r] * 10 + xa[s2]) * ldy);
-          const uint4 v01 = *reinterpret_cast<const uint4*>(base + (ya[r] * 10 + xb[s2]) * ldy);
-          const uint4 v10 = *reinterpret_cast<const uint4*>(base + (yb[r] * 10 + xa[s2]) * ldy);
-          const uint4 v11 = *reinterpret_cast<const uint4*>(base + (yb[r] * 10 + xb[s2]) * ldy);
+          const uint4 v00 = *reinterpret_cast<const uint4*>(base + (ya[r] * TS + xa[s2]) * ldy);
+          const uint4 v01 = *reinterpret_cast<const uint4*>(base + (ya[r] * TS + xb[s2]) * ldy);
+          const uint4 v10 = *reinterpret_cast<const uint4*>(base + (yb[r] * TS + xa[s2]) * ldy);
+          const uint4 v11 = *reinterpret_cast<const uint4*>(base + (yb[r] * TS + xb[s2]) * ldy);
           const __half2* p00 = reinterpret_cast<const __half2*>(&v00);
           const __half2* p01 = reinterpret_cast<const __half2*>(&v01);
           const __half2* p10 = reinterpret_cast<const __half2*>(&v10);
@@ -446,6 +494,24 @@ __global__ void __launch_bounds__(256) ups_gather_ln_tiled_kernel(const __half* 
     for (int k = 0; k < 8 * VPT; ++k) { const float d = acc[k] - mean; var += d * d; }
     for (int o = G >> 1; o; o >>= 1) var += __shfl_xor_sync(0xffffffffu, var, o);
     const float rstd = 1.0f / sqrtf(var / (float)C + eps);
+    if constexpr (HEAD) {
+      constexpr int CH = 8 * VPT;             // G == 1: this thread holds all channels of its pixel
+#pragma unroll
+      for (int k = 0; k < CH; ++k) acc[k] = up_act<ACT>((acc[k] - mean) * rstd * __ldg(lnw + k) + __ldg(lnb + k));
+      const long plane = (long)OH * OW;
+      float* dst = maps + (long)b * NO * plane + (long)oy * OW + ox;
+      for (int o = 0; o < NO; ++o) {
+        const float4* w4 = reinterpret_cast<const float4*>(hws + o * CH);
+        float a0 = hws[NO * CH + o], a1 = 0.f;
+#pragma unroll
+        for (int k = 0; k < CH / 4; ++k) {
+          const float4 w = w4[k];
+          a0 = fmaf(w.x, acc[4 * k], a0); a1 = fmaf(w.y, acc[4 * k + 1], a1);
+          a0 = fmaf(w.z, acc[4 * k + 2], a0); a1 = fmaf(w.w, acc[4 * k + 3], a1);
+        }
+        __stcs(dst + o * plane, a0 + a1);      // streamed: the maps are not read again by this library
+      }
+    } else {
     const long pix = ((long)b * OH + oy) * OW + ox;
 #pragma unroll
     for (int j = 0; j < VPT; ++j) {
@@ -453,9 +519,10 @@ __global__ void __launch_bounds__(256) ups_gather_ln_tiled_kernel(const __half* 
 #pragma unroll
       for (int k = 0; k < 8; ++k) {
         const int c = (lane_g + j * G) * 8 + k;
-        h[k] = __float2half_rn(fmaxf((acc[8 * j + k] - mean) * rstd * __ldg(lnw + c) + __ldg(lnb + c), 0.f));
+        h[k] = __float2half_rn(up_act<ACT>((acc[8 * j + k] - mean) * rstd * __ldg(lnw + c) + __ldg(lnb + c)));
       }
       *reinterpret_cast<uint4*>(out + pix * ld_out + (lane_g + j * G) * 8) = *reinterpret_cast<const uint4*>(h);
+    }
     }
   }
 }

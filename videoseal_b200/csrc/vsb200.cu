@@ -65,6 +65,15 @@ int vsb_model_set_tensor(vsb_model* m, const char* name, const float* data, cons
   VSB_API_END
 }
 
+int vsb_model_set_pixel_decoder(vsb_model* m, int32_t n_stages, const int32_t* factors, int32_t pixelwise) {
+  VSB_API_BEGIN
+  VSB_CHECK(m != nullptr && (factors != nullptr || n_stages == 0), "null argument");
+  std::lock_guard<std::recursive_mutex> lk(m->impl.mu);
+  m->impl.set_pixel_decoder(n_stages, factors, pixelwise);
+  return VSB_OK;
+  VSB_API_END
+}
+
 int vsb_model_finalize(vsb_model* m, int32_t device) {
   VSB_API_BEGIN
   VSB_CHECK(m != nullptr, "null model");
@@ -150,7 +159,7 @@ int vsb_detect_host(vsb_model* m, const float* imgs_h, float* logits_h, int32_t 
   VSB_MODEL_SCOPE(m);
   m->impl.check_ready();
   const size_t n = (size_t)F * 3 * H * W;
-  const size_t nl = (size_t)F * (1 + m->impl.d.nbits);
+  const size_t nl = (size_t)F * m->impl.detect_out_per_frame();
   float* imgs = (float*)m->impl.stage(0, n * sizeof(float));
   float* lg = (float*)m->impl.stage(2, nl * sizeof(float));
   cudaStream_t st = 0;
@@ -168,6 +177,7 @@ int vsb_embed_detect_host(vsb_model* m, const float* imgs_h, const uint8_t* msgs
   VSB_API_BEGIN
   VSB_CHECK(m && imgs_h && msgs_h && imgs_w_h && logits_h, "null argument");
   VSB_MODEL_SCOPE(m);
+  m->impl.check_pooled_head("vsb_embed_detect_host");
   m->impl.embed_detect_host(imgs_h, msgs_h, n_msgs, imgs_w_h, logits_h, F, H, W, step, video_mode, chunk_keys, scaling_i, scaling_w,
                             flags);
   return VSB_OK;
@@ -181,6 +191,7 @@ int vsb_frames_host_u8(vsb_model* m, const uint8_t* frames_h, const uint8_t* msg
   VSB_CHECK(m && frames_h && (frames_w_h || logits_h) && (msgs_h || !frames_w_h), "null argument");
   VSB_MODEL_SCOPE(m);
   VSB_CHECK(F > 0 && H > 0 && W > 0 && step >= 1, "bad shape");
+  if (logits_h) m->impl.check_pooled_head("vsb_frames_host_u8 with logits");
   m->impl.frames_host_u8(frames_h, msgs_h, n_msgs, frames_w_h, logits_h, F, H, W, step, video_mode, chunk_keys, scaling_i, scaling_w,
                          flags);
   return VSB_OK;

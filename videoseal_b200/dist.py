@@ -87,6 +87,9 @@ def embed_detect_sharded(embed_fn: Callable, detect_fn: Callable, frames: torch.
 def extract_message_sharded(logits_local: torch.Tensor, group=None) -> torch.Tensor:
     """`extract_message(aggregation='avg')` over a sharded clip (models/videoseal.py:411-428): local sum of bit logits +
     frame count, one all-reduce of K+1 floats, threshold at 0."""
+    if logits_local.dim() != 2:
+        raise NotImplementedError("extract_message_sharded takes pooled logits [F, 1+K]; per-pixel maps of a pixel-wise model "
+                                  "are not sharded")
     k = logits_local.shape[1] - 1
     buf = torch.zeros(k + 1, device=logits_local.device, dtype=torch.float32)
     if logits_local.shape[0]:

@@ -89,7 +89,8 @@ class _Embedder:
 
 
 class _Detector:
-    """models/extractor.py:140-167 ConvnextExtractor seam: forward(imgs [B,3,S,S] in [0,1]) -> logits [B,1+K]"""
+    """models/extractor.py:140-167 ConvnextExtractor seam: forward(imgs [B,3,S,S] in [0,1]) -> logits [B,1+K] (pixel-wise
+    extractors: maps [B,1+K,S,S])"""
 
     def __init__(self, owner: "Videoseal"):
         self._owner = owner
@@ -132,6 +133,10 @@ class Videoseal(nn.Module):
         if v != self.spec["img_size"]:
             if v <= 0 or v % 128 != 0:
                 raise ValueError(f"img_size={v}: the native path needs a processing size that is a positive multiple of 128")
+            if self.pixelwise:
+                from .cfg import check_pixel_decoder
+                check_pixel_decoder(self.spec["convnext"]["dims"][-1], self.spec["pixel_decoder"]["upscale_stages"], v,
+                                    self.spec["nbits"])
             self._respec(img_size=v)
 
     @property
@@ -215,6 +220,10 @@ class Videoseal(nn.Module):
         h = C.c_void_p()
         _lib.check(L.vsb_model_create(C.byref(d), C.byref(h)))
         try:
+            pd = s.get("pixel_decoder", {"pixelwise": False})
+            if pd["pixelwise"]:
+                f = pd["upscale_stages"]
+                _lib.check(L.vsb_model_set_pixel_decoder(h, len(f), (C.c_int32 * len(f))(*f), 1))
             for k, v in self._sd.items():
                 if k.startswith(("attenuation.", "rgb2yuv.")) or v.dim() > 4:
                     continue
@@ -289,8 +298,19 @@ class Videoseal(nn.Module):
             return {"imgs_w": imgs_w.to(imgs.device), "msgs": msgs[0:1].repeat(F_, 1)}
         return {"msgs": msgs, "preds_w": preds_w.to(imgs.device), "imgs_w": imgs_w.to(imgs.device)}
 
+    @property
+    def pixelwise(self) -> bool:
+        """True when detect() returns per-pixel maps [F, 1+K, P, P] (pixel_decoder.pixelwise of the card)."""
+        return bool(self.spec.get("pixel_decoder", {}).get("pixelwise", False))
+
     def _detect_dev(self, x: torch.Tensor, antialias: bool) -> torch.Tensor:
-        out = torch.empty((x.shape[0], 1 + self.spec["nbits"]), device=x.device, dtype=torch.float32)
+        shape = (x.shape[0], 1 + self.spec["nbits"])
+        if self.pixelwise:   # trunk map (img_size / 32) x the product of the stage factors: img_size for [4, 4, 2]
+            P = self.spec["img_size"] // 32
+            for f in self.spec["pixel_decoder"]["upscale_stages"]:
+                P *= f
+            shape += (P, P)
+        out = torch.empty(shape, device=x.device, dtype=torch.float32)
         flags = 0 if antialias else _lib.FLAG_RESIZE_NO_AA
         _lib.check(_lib.lib().vsb_detect(self._handle(), x.data_ptr(), out.data_ptr(), x.shape[0], x.shape[2], x.shape[3], flags,
                                          self._stream()))

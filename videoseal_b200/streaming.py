@@ -23,6 +23,9 @@ def _as_u8_clip(clip) -> np.ndarray:
 
 def _run(model: Videoseal, clip: np.ndarray, msgs, want_frames: bool, want_logits: bool, lowres_attenuation: bool, is_video: bool):
     F_, H, W = clip.shape[0], clip.shape[1], clip.shape[2]
+    if want_logits and model.pixelwise:
+        raise NotImplementedError("streaming detection returns one logit vector per frame; a pixel-wise model's maps come from "
+                                  "model.detect()")
     nbits = model.spec["nbits"]
     out = np.empty_like(clip) if want_frames else None
     logits = np.empty((F_, 1 + nbits), dtype=np.float32) if want_logits else None

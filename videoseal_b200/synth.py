@@ -83,9 +83,16 @@ def synth_state_dict(spec: dict, seed: int = 0) -> dict:
             sd[B + "grn.beta"] = 0.1 * torch.randn(1, 1, 1, 4 * dims[s], generator=g)
             linear(B + "pwconv2", dims[s], 4 * dims[s])
     D = "detector.pixel_decoder."
-    conv(D + "output_upscaling.0.upsample_block.2", dims[-1], dims[-1], 3, False)
-    affine(D + "output_upscaling.0.upsample_block.3", dims[-1])
-    linear(D + "linear", 1 + spec["nbits"], dims[-1])
+    pd = spec.get("pixel_decoder", {"pixelwise": False, "upscale_stages": [1]})
+    c = dims[-1]
+    for i, f in enumerate(pd["upscale_stages"]):      # pixel_decoder.py:44-50: widths c, c // f, ...
+        conv(D + f"output_upscaling.{i}.upsample_block.2", c // f, c, 3, False)
+        affine(D + f"output_upscaling.{i}.upsample_block.3", c // f)
+        c //= f
+    if pd["pixelwise"]:
+        conv(D + "linear", 1 + spec["nbits"], c, 1, True)
+    else:
+        linear(D + "linear", 1 + spec["nbits"], c)
     return sd
 
 
