@@ -143,6 +143,13 @@ int64_t vsb_profile_read(char* buf, int64_t capacity);
 /* copy a named intermediate activation of the most recent embed/detect sub-batch to the host as fp32.
  * shape4 receives [B, H, W, C] (NHWC) or [M, C, 1, 1]-style dims; returns the element count or <0. */
 int64_t vsb_debug_get_tensor(vsb_model* m, const char* name, float* host_out, int64_t capacity, int64_t* shape4);
+/* which compiled variant the most recent launch of each full-resolution kernel used (host state, no synchronisation):
+ *   out[0..4]  resize_sep_kernel:  MT (x taps in registers: 2, 8, or 0 = any count), GST (input rows per staging round: 4, 2, 1),
+ *              vec (1 = bulk copies, 0 = 4-byte cp.async), toy (output rows per block), OW (output width = img_size)
+ *   out[5..9]  blend:  3 = jnd_blend3_kernel (TMA-fed) or 2 = jnd_blend2_kernel, VEC (4 or 1), FASTUP (1 = delta read in place or
+ *              through <= 2 taps per axis), CD (delta channels), JIN (heat-map inputs: 1 luminance, 3 per RGB channel)
+ * Entries are -1 until that kernel has run on this handle.  capacity >= 10; returns 10, or < 0. */
+int32_t vsb_debug_last_dispatch(vsb_model* m, int32_t* out, int32_t capacity);
 /* standalone conv/GEMM on the wgmma kernels for unit tests: see tests/test_conv_gemm_gpu.py */
 typedef struct vsb_conv_test {
   int32_t loader;            /* 0 TMA per tap, 1 gather conv, 4 halo conv3x3, 5 direct 3x3 ring conv */

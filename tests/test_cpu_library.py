@@ -69,10 +69,17 @@ def test_unsupported_card_features_raise_at_load():
 
 
 @pytest.mark.parametrize("n_in,n_out,aa", [(768, 256, True), (300, 256, True), (480, 256, True), (257, 256, True), (200, 256, True),
-                                            (256, 768, True), (256, 768, False), (256, 300, False), (17, 256, False), (1080, 256, False)])
+                                            (256, 768, True), (256, 768, False), (256, 300, False), (17, 256, False), (1080, 256, False),
+                                            # anti-aliased down-scales above 3x (maxt 9 .. 61: resize_sep_kernel's any-tap-count path)
+                                            (769, 256, True), (1080, 256, True), (1920, 256, True), (2160, 256, True), (3840, 256, True),
+                                            (1280, 256, True), (1920, 384, True), (3840, 128, True),
+                                            # large up-scales (the delta of the blend at 1080p / 4K)
+                                            (256, 1920, True), (256, 2160, False), (512, 1080, True)])
 def test_resample_tables_match_aten_interpolate(built_lib, n_in, n_out, aa):
     """the host-built separable tables of the resize kernels (model.cuh:make_resample) against F.interpolate applied to the
-    identity: every output sample's tap positions and weights (wam.py:163,184,224 call sites; bilinear, align_corners=False)"""
+    identity: every output sample's tap positions and weights (wam.py:163,184,224 call sites; bilinear, align_corners=False).
+    Anti-aliased down-scales are computed in double and rounded once to fp32, so they are held to float64 ATen; the plain
+    bilinear tables take their source coordinate in fp32 (as ATen's fp32 kernels do), so they are held to fp32 ATen."""
     import ctypes as C
     import numpy as np
     import torch.nn.functional as F
@@ -87,12 +94,16 @@ def test_resample_tables_match_aten_interpolate(built_lib, n_in, n_out, aa):
     for o in range(n_out):
         assert 0 <= start[o] and start[o] + cnt[o] <= n_in and 1 <= cnt[o] <= maxt
         op[o, start[o]:start[o] + cnt[o]] = w[o, :cnt[o]]
-    eye = torch.eye(n_in, dtype=torch.float32).reshape(1, n_in, 1, n_in)          # n_in "channels", each a one-hot row of width n_in
+    down_aa = aa and n_in > n_out
+    assert (maxt == 2 * int(np.ceil(n_in / n_out)) + 1) if down_aa else maxt == 2
+    dt = torch.float64 if down_aa else torch.float32
+    eye = torch.eye(n_in, dtype=dt).reshape(1, n_in, 1, n_in)          # n_in "channels", each a one-hot row of width n_in
     ref = F.interpolate(eye, size=(1, n_out), mode="bilinear", align_corners=False, antialias=aa)
     ref = ref.reshape(n_in, n_out).t().double().numpy()
     # up-scaling with antialias=True: ATen routes it through its anti-aliasing code (triangle filter of support 1 == plain bilinear
-    # mathematically), whose source coordinate is rounded once more than the plain kernel's: one float ulp of a coordinate < 256
-    tol = 8e-6 if (aa and n_out > n_in) else 2e-6
+    # mathematically), whose source coordinate is rounded once more than the plain kernel's: half a float ulp of a coordinate < 512
+    # (7.6e-6 at 256 -> 1920 and 512 -> 1080).  Anti-aliased down-scales: one fp32 rounding of a weight <= 1 (measured <= 1.5e-8).
+    tol = 1e-7 if down_aa else (8e-6 if aa and n_out > n_in else 2e-6)
     assert np.abs(op - ref).max() < tol
     assert np.allclose(op.sum(1), 1.0, atol=1e-5)
 

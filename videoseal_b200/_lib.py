@@ -13,7 +13,7 @@ EXPORTS = [
     "vsb_last_error", "vsb_version", "vsb_model_create", "vsb_model_set_tensor", "vsb_model_set_pixel_decoder", "vsb_model_finalize",
     "vsb_model_destroy", "vsb_embed", "vsb_embedder_forward", "vsb_detect", "vsb_jnd_heatmaps", "vsb_embed_host",
     "vsb_detect_host", "vsb_embed_detect_host", "vsb_frames_host_u8", "vsb_launch_count", "vsb_profile_enable", "vsb_profile_read", "vsb_debug_get_tensor", "vsb_debug_conv",
-    "vsb_debug_resample_table",
+    "vsb_debug_resample_table", "vsb_debug_last_dispatch",
 ]
 
 FLAG_CLAMP, FLAG_LOWRES_ATTN, FLAG_NO_ATTENUATION, FLAG_RESIZE_NO_AA = 1, 2, 4, 8
@@ -86,6 +86,8 @@ def lib():
     L.vsb_debug_get_tensor.restype = C.c_int64
     L.vsb_debug_conv.argtypes = [C.POINTER(ConvTest), C.c_void_p]
     L.vsb_debug_resample_table.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
+    L.vsb_debug_last_dispatch.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int32]
+    L.vsb_debug_last_dispatch.restype = C.c_int32
     _lib = L
     return L
 

@@ -187,7 +187,6 @@ struct ResampleDev {
       smem = ((((size_t)rin_max * ow + 3) & ~(size_t)3) + kRsStages * (((size_t)gstage * iw + 8 + 3) & ~(size_t)3)) * sizeof(float);
       if (smem <= 100 * 1024 || toy == 1) break;
     }
-    if (smem > 200 * 1024) throw Error("resize: image too wide for the shared-memory resample kernel (not implemented)", kErrUnsupported);
   }
 };
 
@@ -337,6 +336,10 @@ class Model {
   std::map<int, std::unique_ptr<Plan>> embed_plans, detect_plans;
   std::map<uint64_t, std::unique_ptr<ResampleDev>> resamplers;
   Plan* last_plan = nullptr;
+  // test seam (vsb_debug_last_dispatch): the variant of the most recent launch of each full-resolution kernel, -1 before the first
+  //   resize: MT, GST, vec, toy, OW       blend: 3 (jnd_blend3_kernel) or 2 (jnd_blend2_kernel), VEC, FASTUP, CD, JIN
+  int32_t last_resize[5] = {-1, -1, -1, -1, -1};
+  int32_t last_blend[5] = {-1, -1, -1, -1, -1};
 
   explicit Model(const vsb_model_desc& desc) : d(desc) {}
 
@@ -808,6 +811,7 @@ class Model {
     const int S = d.img_size, L = d.unet_levels;
     std::vector<int> z(d.unet_z, d.unet_z + L);
     pl.x_res = pl.pool.alloc_n<float>((size_t)B * 3 * S * S);
+    dbg(pl, "x_res", pl.x_res, 0, B, 3, S, S, S);
     pl.delta = pl.pool.alloc_n<float>((size_t)B * d.unet_out_ch * S * S);
     Plan* plp = &pl;
     // ---- inc
@@ -974,6 +978,7 @@ class Model {
     Plan* plp = &pl;
     const int S = d.img_size;
     pl.x_res = pl.pool.alloc_n<float>((size_t)B * 3 * S * S);
+    dbg(pl, "x_res", pl.x_res, 0, B, 3, S, S, S);
     pl.logits = pl.pool.alloc_n<float>((size_t)B * (1 + d.nbits));
     const int st_ = d.ext_stem_stride;
     int hs = (S - 4) / st_ + 1;
@@ -1288,6 +1293,8 @@ class Model {
   void resize_frames(const float* src, long frame_stride, int n, int H, int W, float* dst, bool aa, cudaStream_t st) {
     const int S = d.img_size;
     ResampleDev* r = get_resampler(H, W, S, S, aa);
+    // (checked here, not when the table is built: the blend only reads the delta up-sampler's table, whatever its width)
+    if (r->smem > 200 * 1024) throw Error("resize: image too wide for the shared-memory resample kernel (not implemented)", kErrUnsupported);
     const int vec = (W % 4 == 0) && (reinterpret_cast<uintptr_t>(src) % 16 == 0) && (frame_stride % 4 == 0);
     if (n > 16384) {   // gridDim.y limit: split very long frame ranges
       for (int i = 0; i < n; i += 16384)
@@ -1295,8 +1302,10 @@ class Model {
       return;
     }
     const dim3 grid((S + r->toy - 1) / r->toy, n * 3);
+    const int mt = r->tab.maxt_x <= 2 ? 2 : (r->tab.maxt_x <= 8 ? 8 : 0);
+    const int32_t rec[5] = {mt, r->gstage, vec, r->toy, S};
+    std::copy(rec, rec + 5, last_resize);
     prof_scope("pw.resize." + std::to_string(H) + "x" + std::to_string(W) + "@" + std::to_string(n), st, 1, [&] {
-      const int mt = r->tab.maxt_x <= 2 ? 2 : (r->tab.maxt_x <= 8 ? 8 : 0);
 #define VSB_RS(MT, GS) do { static bool attr_ = false; \
         if (!attr_) { VSB_CUDA(cudaFuncSetAttribute(resize_sep_kernel<MT, GS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr_ = true; } \
         resize_sep_kernel<MT, GS><<<grid, 256, r->smem, st>>>(src, frame_stride, dst, H, W, S, S, r->tab, r->toy, r->rin_max, vec); } while (0)
@@ -1540,7 +1549,7 @@ class Model {
     }
   }
 
-  static void launch_blend(const BlendParams& bp, cudaStream_t st) {
+  void launch_blend(const BlendParams& bp, cudaStream_t st) {
     VSB_CHECK(bp.F <= 65535, "too many frames per blend launch");
     dim3 grid((bp.W + kB2TW - 1) / kB2TW, (bp.H + kB2TH - 1) / kB2TH, bp.F);
     const bool vec = (bp.W % 4 == 0) && ((reinterpret_cast<uintptr_t>(bp.imgs) | reinterpret_cast<uintptr_t>(bp.imgs_w) |
@@ -1569,6 +1578,8 @@ class Model {
         encode_map(&tmD, bp.delta, 3, ddims, dstr, dbox, 0, true, /*f32=*/true);
       }
     }
+    const int32_t rec[5] = {tma ? 3 : 2, vec ? 4 : 1, fastup ? 1 : 0, bp.CD, (bp.use_jnd && bp.jnd_in == 3) ? 3 : 1};
+    std::copy(rec, rec + 5, last_blend);
     prof_scope(std::string(bp.use_jnd ? "pw.jnd_blend." : "pw.blend.") + std::to_string(bp.H) + "x" + std::to_string(bp.W) + "@" + std::to_string(bp.F) +
                    (bp.preds_w ? "+preds" : ""), st, 1, [&] {
 #define VSB_BL(V, FU, CDV, JI) do { static bool attr_ = false; \

@@ -233,6 +233,20 @@ int64_t vsb_debug_get_tensor(vsb_model* m, const char* name, float* host_out, in
   }
 }
 
+int32_t vsb_debug_last_dispatch(vsb_model* m, int32_t* out, int32_t capacity) {
+  try {
+    VSB_CHECK(m && out, "null argument");
+    VSB_CHECK(capacity >= 10, "dispatch buffer too small");
+    std::lock_guard<std::recursive_mutex> lk(m->impl.mu);
+    std::copy(m->impl.last_resize, m->impl.last_resize + 5, out);
+    std::copy(m->impl.last_blend, m->impl.last_blend + 5, out + 5);
+    return 10;
+  } catch (const std::exception& e) {
+    g_err = e.what();
+    return -1;
+  }
+}
+
 int vsb_debug_conv(const vsb_conv_test* t, void* stream) {
   VSB_API_BEGIN
   VSB_CHECK(t != nullptr, "null argument");
