@@ -103,6 +103,7 @@ def spec_from_card(card: dict) -> dict:
         raise NotImplementedError("temporal ConvNeXt variants are out of scope")
     if pixelwise:
         check_pixel_decoder(dims[-1], stages, int(img_size), nbits)
+    check_unet([int(u["z_channels"]) * int(m) for m in u["z_channels_mults"]], int(img_size))
     att = str(a.get("attenuation", "None"))
     jnd = (0, 0)
     if att.lower().startswith("jnd"):
@@ -151,6 +152,24 @@ def check_pixel_decoder(c: int, stages: list, img_size: int, nbits: int) -> None
         elif not any(co % (8 * v) == 0 and co // (8 * v) <= 32 and (co // (8 * v)) & (co // (8 * v) - 1) == 0 for v in (1, 3)):
             raise NotImplementedError(f"pixel decoder: stage {i} has {co} channels; middle stages take 8 * {{1, 3}} * 2^k, k <= 5")
         c, h = co, h * f
+
+
+def check_unet(z: list, img_size: int) -> None:
+    """U-Net widths and sizes the native embedder implements (model.cuh: Model::finalize), checked at load time.  A level is 16, 32
+    or a multiple of 64 channels wide, or 8 in a leading run of levels that stops before the last one (the 8-channel direct-conv
+    kernels; unet_tiny_*).  The bottleneck map, img_size / 2^(levels - 1), is at least 16 pixels: the tensor-core convs tile
+    maps by 128 pixels.  An 8-channel U-Net runs at processing sizes up to 768, where its 8-channel rings still fit in shared
+    memory."""
+    L = len(z)
+    for i, c in enumerate(z):
+        if not ((c == 8 and i < L - 1 and (i == 0 or z[i - 1] == 8)) or c in (16, 32) or (c > 0 and c % 64 == 0)):
+            raise NotImplementedError(f"U-Net width {c} at level {i} is not implemented (8 in the leading levels, 16, 32 or a "
+                                      "multiple of 64)")
+    if img_size >> (L - 1) < 16:
+        raise NotImplementedError(f"img_size={img_size}: the U-Net's {L} levels leave a {img_size >> (L - 1)}-pixel bottleneck map; "
+                                  "at least 16 is implemented")
+    if z[0] == 8 and img_size > 768:
+        raise NotImplementedError(f"img_size={img_size}: an 8-channel U-Net runs at processing sizes up to 768")
 
 
 def setup_model(card: dict, ckpt_path):

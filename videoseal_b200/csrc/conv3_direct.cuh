@@ -75,7 +75,10 @@ __global__ void pack_direct_weights_kernel(const __half* __restrict__ w, int N, 
 
 // MODE 0: plain conv; MODE 1 ("UP"): phase-folded up-conv (two sources, replicate padding, LN + pixel-shuffle epilogue);
 // MODE 2 ("S2"): stride-2 3x3 conv, pad 1, as a 2x2-tap conv over the space-to-depth view of the input (C = 4*C_in planes
-// gathered by the producers straight from the [B,2H,2W,C_in] tensor; taps with an offset of +1 have no weights and are skipped)
+// gathered by the producers straight from the [B,2H,2W,C_in] tensor; taps with an offset of +1 have no weights and are skipped).
+// KS = C / 16 k16 steps per tap; KS = 0 is the 8-channel input (C = 8, one plane, MODE 0 only): a k16 MMA then covers two
+// horizontally adjacent taps, and the weights are packed as (R * ceil(R/2)) virtual 16-channel taps (direct8_weights).
+// N = 8 (m64n8k16) takes C = 8 in MODE 0 or C = 32 (4 x 8) in MODE 2.
 template <int N, int KS, int R, int MODE>
 __global__ void __launch_bounds__(kD3Threads, 1) conv3_direct_kernel(const Conv3DirectParams p) {
   constexpr bool UP = MODE == 1, S2 = MODE == 2;
@@ -122,7 +125,7 @@ __global__ void __launch_bounds__(kD3Threads, 1) conv3_direct_kernel(const Conv3
     // extent does the same split, but every 16-byte line is its own request and the TMA unit's request window, not
     // bandwidth, then bounds the kernel.)
     const int pw = warp >> 1;
-    const int planes = p.C >> 3, pshift = planes == 2 ? 1 : (planes == 4 ? 2 : 3);
+    const int planes = p.C >> 3, pshift = KS == 0 ? 0 : (planes == 2 ? 1 : (planes == 4 ? 2 : 3));
     int tiles_conf = 0;
     int slot = pw;   // NR >= 8 > 2 producers
     for (int k = pw; k <= row_hi - row_lo && nt > 0; k += 2, slot = slot + 2 >= NR ? slot + 2 - NR : slot + 2) {
@@ -197,7 +200,8 @@ __global__ void __launch_bounds__(kD3Threads, 1) conv3_direct_kernel(const Conv3
     float* xp = reinterpret_cast<float*>(smem + kD3XposeOff) + (size_t)(warp - 4) * 32 * kD3XposePitch;
     // no-swizzle K-major descriptors: LBO = byte distance between the two core matrices along K (next 8 channels), SBO = byte
     // distance between consecutive 8-row groups (next 8 positions / output channels)
-    const uint32_t a_lbo = p.plane_stride, a_sbo = 128u;
+    // (KS = 0, one 8-channel plane: LBO = 16 B, so the second core matrix along K is the NEXT position, i.e. tap (r, s + 1))
+    const uint32_t a_lbo = KS == 0 ? 16u : p.plane_stride, a_sbo = 128u;
     const uint32_t b_lbo = (uint32_t)N * 16u, b_sbo = 128u;
     const uint32_t a_lo = (((a_lbo >> 4) & 0x3FFFu) << 16) + (smem_u32(ring) >> 4);
     const uint32_t b_lo = (((b_lbo >> 4) & 0x3FFFu) << 16) + (smem_u32(wsm) >> 4);
@@ -274,6 +278,22 @@ __global__ void __launch_bounds__(kD3Threads, 1) conv3_direct_kernel(const Conv3
         wgmma_fence_regs(acc[0]);
         wgmma_fence_regs(acc[1]);
         wgmma_fence();
+        if constexpr (KS == 0) {
+          // C = 8: per kernel row, taps (r, 0) + (r, 1) in one k16 MMA and (r, 2) + a zero-weight (r, 3) in the next (1x1: the
+          // tap and a zero-weight neighbour).  The neighbour of a valid output is always in its own padded row (rw >= W + R).
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int r = 0; r < R; ++r) {
+#pragma unroll
+              for (int t = 0; t < (R + 1) / 2; ++t) {
+                const uint64_t adesc = a_hi | (uint64_t)(arow[r] + (uint32_t)(64 * h + 2 * t));
+                const uint64_t bdesc = b_hi | (uint64_t)(b_lo + (uint32_t)((r * ((R + 1) / 2) + t) * 2 * N));
+                Wgmma<N>::mma(acc[h], adesc, bdesc, (r | t) != 0 ? 1u : 0u);
+              }
+            }
+          }
+        } else {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
 #pragma unroll
@@ -289,6 +309,7 @@ __global__ void __launch_bounds__(kD3Threads, 1) conv3_direct_kernel(const Conv3
             }
           }
         }
+        }
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_fence_regs(acc[0]);
@@ -297,6 +318,60 @@ __global__ void __launch_bounds__(kD3Threads, 1) conv3_direct_kernel(const Conv3
       __syncwarp();
       if (lane == 0) mbar_arrive(&hd->tile_done[i & (kD3TileBars - 1)]);   // this warp's reads of the ring are complete
       advance(kD3EpiSets);
+      if constexpr (N == 8) {
+        // m64n8 fragments -> one row (8 columns) per lane; + bias, ReLU, + residual, one 16-byte store, optional fused outc + tanh
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int j = 0; j < 4; j += 2) {
+            const int lr = (lane >> 2) + 8 * (j >> 1) + 16 * h, lc = 2 * (lane & 3);
+            *reinterpret_cast<float2*>(xp + lr * kD3XposePitch + lc) = make_float2(acc[h][j], acc[h][j + 1]);
+          }
+        }
+        __syncwarp();
+        float f[8];
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          const float4 t = *reinterpret_cast<const float4*>(xp + lane * kD3XposePitch + 4 * u);
+          const float4 bq = *reinterpret_cast<const float4*>(&hd->bias[4 * u]);
+          f[4 * u + 0] = t.x + bq.x; f[4 * u + 1] = t.y + bq.y; f[4 * u + 2] = t.z + bq.z; f[4 * u + 3] = t.w + bq.w;
+        }
+        __syncwarp();
+        if (valid) {
+          if (p.relu) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) f[j] = fmaxf(f[j], 0.f);
+          }
+          if (p.resid != nullptr) {
+            __align__(16) __half hr[8];
+            *reinterpret_cast<uint4*>(hr) = rr[0];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) f[j] += __half2float(hr[j]);
+          }
+          if (p.out != nullptr) {
+            __align__(16) __half2 h2[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+              h2[j] = __floats2half2_rn(fminf(fmaxf(f[2 * j], -65504.f), 65504.f), fminf(fmaxf(f[2 * j + 1], -65504.f), 65504.f));
+            *reinterpret_cast<uint4*>(p.out + pix * 8) = *reinterpret_cast<const uint4*>(h2);
+          }
+          if (p.outc_w != nullptr) {
+            const long hw = (long)p.H * p.W;
+            const long o0 = (long)b * p.n_out * hw + (long)y * p.W + x;
+#pragma unroll
+            for (int o = 0; o < 3; ++o) {
+              if (o < p.n_out) {
+                float d = 0.f;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) d += f[j] * hd->ocw[o][j];
+                d += __ldg(p.outc_b + o);
+                if (p.outc_tanh) d = tanhf(d);
+                p.delta[o0 + o * hw] = d;
+              }
+            }
+          }
+        }
+      } else {
       // fragments -> one row per lane, 16 columns at a time
       uint32_t v[N / 16][16];
 #pragma unroll
@@ -401,6 +476,7 @@ __global__ void __launch_bounds__(kD3Threads, 1) conv3_direct_kernel(const Conv3
         }
       }
       }  // valid
+      }  // N > 8
       if constexpr (kDeep) {
         cur = nxt;
 #pragma unroll

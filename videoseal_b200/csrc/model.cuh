@@ -513,9 +513,37 @@ class Model {
     VSB_CUDA(cudaStreamSynchronize(0));
     return wd;
   }
+  // 8-channel convs (unet_tiny_*) run only on the direct kernel's 8-channel instantiation (conv3_direct.cuh, KS = 0):
+  // [N][8][R][R] (x out_scale) -> its virtual-tap weight layout (direct8_weights)
+  __half* pack_direct8(const std::string& wkey, const std::vector<float>* out_scale) {
+    const HostTensor& w = get(wkey);
+    const int N = (int)w.shape[0], R = w.shape.size() == 4 ? (int)w.shape[2] : 1;
+    VSB_CHECK((int)w.shape[1] == 8 && N == 8, "8-channel conv weight shape");
+    std::vector<float> t((size_t)N * R * R * 8);
+    for (int n = 0; n < N; ++n)
+      for (int c = 0; c < 8; ++c)
+        for (int k = 0; k < R * R; ++k) {
+          float v = w.data[((size_t)n * 8 + c) * R * R + k];
+          if (out_scale) v *= (*out_scale)[n];
+          t[((size_t)n * R * R + k) * 8 + c] = v;
+        }
+    const std::vector<float> v = direct8_weights(t, N, R);
+    __half* plain = wpool.upload(to_half(v));
+    __half* wd = wpool.alloc_n<__half>(v.size());
+    pack_direct_weights(plain, N, 16, wd, 0, R * ((R + 1) / 2));
+    VSB_CUDA(cudaStreamSynchronize(0));
+    return wd;
+  }
   static bool use_halo(int C) { return C <= 16; }
   ConvW pack_conv3(const std::string& wkey, const std::vector<float>* out_scale, const std::vector<float>& bias) {
     const int C = (int)get(wkey).shape[1], N = (int)get(wkey).shape[0];
+    if (C == 8) {
+      ConvW cw;
+      cw.N = N; cw.K = 9 * C;
+      cw.bias = wpool.upload(bias);
+      cw.wd = pack_direct8(wkey, out_scale);
+      return cw;
+    }
     ConvW cw = use_halo(C) ? pack_conv_halo(wkey, out_scale, bias, C, 0) : pack_conv(wkey, out_scale, bias);
     if (conv3_direct_ok(C, N, C)) {
       ConvW plain = use_halo(C) ? pack_conv(wkey, out_scale, {}) : cw;   // [N][9*C], K order (r, s, c)
@@ -544,7 +572,9 @@ class Model {
     bn_fold(key + ".double_conv.4", s, b);
     rb.c2 = pack_conv3(key + ".double_conv.3.weight", &s, b);
     rb.res = pack_conv(key + ".res_conv.weight", nullptr, get(key + ".res_conv.bias").data);
-    if (conv3_direct_ok(rb.res.K, rb.res.N, rb.res.K, 0, 1)) {   // narrow 1x1: same ring kernel with a single tap
+    if (rb.res.K == 8) {
+      rb.res.wd = pack_direct8(key + ".res_conv.weight", nullptr);
+    } else if (conv3_direct_ok(rb.res.K, rb.res.N, rb.res.K, 0, 1)) {   // narrow 1x1: same ring kernel with a single tap
       rb.res.wd = wpool.alloc_n<__half>((size_t)rb.res.N * rb.res.K);
       pack_direct_weights(rb.res.w, rb.res.N, rb.res.K, rb.res.wd, 0, 1);
       VSB_CUDA(cudaStreamSynchronize(0));
@@ -577,7 +607,17 @@ class Model {
       bn_fold(P + "inc.double_conv.1", s, b);
       const HostTensor& w = get(P + "inc.double_conv.0.weight");
       VSB_CHECK((int)w.shape[0] == z[0] && (int)w.shape[1] == d.unet_in_ch, "inc conv shape");
-      VSB_CHECK(z[0] % 16 == 0, "z0 must be a multiple of 16");
+      for (int i = 0; i < L; ++i) {
+        // widths the kernels implement: 8 (a leading run of levels, not the last: the direct conv's 8-channel instantiations),
+        // 16, 32 and multiples of 64 (cfg.check_unet has the same rule)
+        const bool ok8 = z[i] == 8 && i < L - 1 && (i == 0 || z[i - 1] == 8);
+        if (!(ok8 || z[i] == 16 || z[i] == 32 || (z[i] > 0 && z[i] % 64 == 0)))
+          throw Error("U-Net width " + std::to_string(z[i]) + " at level " + std::to_string(i) + " is not implemented (8 in the "
+                      "leading levels, 16, 32 or a multiple of 64)", kErrUnsupported);
+      }
+      if ((d.img_size >> (L - 1)) < 16)
+        throw Error("U-Net bottleneck map " + std::to_string(d.img_size >> (L - 1)) + "^2 is below 16^2 (processing size " +
+                    std::to_string(d.img_size) + ", " + std::to_string(L) + " levels): not implemented", kErrUnsupported);
       std::vector<float> w1(w.data);
       const size_t per = (size_t)d.unet_in_ch * 9;
       for (int n = 0; n < z[0]; ++n) for (size_t k = 0; k < per; ++k) w1[n * per + k] *= s[n];
@@ -589,7 +629,7 @@ class Model {
     }
     for (int i = 0; i < L - 1; ++i) {
       down_conv.push_back(pack_conv(P + "downs." + std::to_string(i) + ".down.weight", nullptr, get(P + "downs." + std::to_string(i) + ".down.bias").data));
-      if (z[i] == 16 && z[i + 1] == 32 && conv3_direct_ok(64, 32, 64, 0, 3))
+      if (conv3_direct_s2d_ok(z[i], z[i + 1]))
         down_conv.back().wd = pack_down_s2d(P + "downs." + std::to_string(i) + ".down.weight");
       down_rb.push_back(pack_resblock(P + "downs." + std::to_string(i) + ".conv"));
     }
@@ -603,7 +643,8 @@ class Model {
         // virtual concat (x | skip * 2^-1/2): fold the skip scale into the second half of the input channels
         std::vector<float> in_scale(2 * zz[ii + 1], 1.0f);
         for (int c = zz[ii + 1]; c < 2 * zz[ii + 1]; ++c) in_scale[c] = 0.70710678118654752440f;
-        up_conv.push_back(pack_upconv_taps(U + ".up.upsample_block.2.weight", in_scale));
+        // 8-channel sources go through the gather loader, whose K block is 64: pad K to one block
+        up_conv.push_back(pack_upconv_taps(U + ".up.upsample_block.2.weight", in_scale, zz[ii + 1] == 8 ? 64 : 0));
         __half* pw = nullptr; float* bw = nullptr;
         if (zz[ii] == 16 && 2 * zz[ii + 1] == 64 && conv3_direct_ok(64, 64, 64, 0, 3))
           pack_upconv_phase(U + ".up.upsample_block.2.weight", in_scale, &pw, &bw);
@@ -742,6 +783,9 @@ class Model {
     __half* r = pl.pool.alloc_n<__half>(M * Cout);
     __half* h = pl.pool.alloc_n<__half>(M * Cout);
     if (!out && !fuse_outc) { out = pl.pool.alloc_n<__half>(M * Cout); ld_out = Cout; }
+    if (Cout == 8 && !(conv3_direct_ok(8, 8, ldx, W) && conv3_direct_ok(8, 8, ldx, W, 1) && (out == nullptr || ld_out == 8)))
+      throw Error("8-channel ResnetBlock on a " + std::to_string(W) + "-wide map: the direct conv's ring does not fit (processing "
+                  "size too large for an 8-channel U-Net)", kErrUnsupported);
     if (w.res.wd && conv3_direct_ok(Cin, Cout, ldx, W, 1)) {  // res 1x1, narrow layers
       Conv3DirectOp op; setup_conv3_direct(op, x, B, H, W, Cin, Cout, w.res.wd, num_sms, 1);
       op.p.bias = w.res.bias; op.p.out = r; op.p.relu = 0;
@@ -824,7 +868,11 @@ class Model {
       pl.steps.push_back(Step{[=](cudaStream_t st) {
         dim3 grid((S + 31) / 32, (S + 15) / 16, B);
         const float* src = plp->in_imgs;
-        if (cin == 1) unet_first_kernel<1><<<grid, 256, 0, st>>>(src, B, S, S, Z, w1, b1, wr, br, h1, r0, yuv);
+        if (Z == 8) {
+          const dim3 grid8((S + 63) / 64, (S + 15) / 16, B);
+          if (cin == 1) unet_first_z8_kernel<1><<<grid8, 256, 0, st>>>(src, B, S, S, w1, b1, wr, br, h1, r0, yuv);
+          else unet_first_z8_kernel<3><<<grid8, 256, 0, st>>>(src, B, S, S, w1, b1, wr, br, h1, r0, yuv);
+        } else if (cin == 1) unet_first_kernel<1><<<grid, 256, 0, st>>>(src, B, S, S, Z, w1, b1, wr, br, h1, r0, yuv);
         else unet_first_kernel<3><<<grid, 256, 0, st>>>(src, B, S, S, Z, w1, b1, wr, br, h1, r0, yuv);
         VSB_CUDA(cudaGetLastError());
       }, 1, "unet.first"});
@@ -839,6 +887,7 @@ class Model {
                               "unet.conv3x3d." + std::to_string(z[0]) + "-" + std::to_string(z[0]) + "@" + std::to_string(S)});
       dbg(pl, "inc", x, 1, B, S, S, z[0], z[0]);
     } else {
+      if (z[0] == 8) throw Error("8-channel inc block on a " + std::to_string(S) + "-wide map: the direct conv's ring does not fit", kErrUnsupported);
       ConvGemmOp op; setup_conv3(op, h1, B, S, S, z[0], z[0]);
       op.p.epi = EPI_AFFINE; op.p.act = ACT_RELU; op.p.bias = inc_c2.bias; op.p.resid16 = r0; op.p.ld_res16 = z[0];
       op.p.out16 = x; op.p.ld_out16 = z[0];
@@ -852,12 +901,13 @@ class Model {
       const int ho = hs / 2;
       const long Mo = (long)B * ho * ho;
       __half* dn = pl.pool.alloc_n<__half>(Mo * z[i + 1]);
-      if (down_conv[i].wd && ldx == z[i] && hs % 2 == 0 && conv3_direct_ok(4 * z[i], z[i + 1], 4 * z[i], ho, 3)) {
+      if (down_conv[i].wd && ldx == z[i] && hs % 2 == 0 && conv3_direct_s2d_ok(z[i], z[i + 1], ho)) {
         Conv3DirectOp op;
         setup_down_s2d_direct(op, x, z[i], B, ho, ho, z[i + 1], down_conv[i].wd, down_conv[i].bias, dn, num_sms);
         pl.steps.push_back(Step{[op](cudaStream_t st) { launch_direct(op, st); }, 1,
                                 "unet.down3x3s2d." + std::to_string(z[i]) + "-" + std::to_string(z[i + 1]) + "@" + std::to_string(ho)});
       } else {
+        if (z[i + 1] == 8) throw Error("8-channel stride-2 conv on a " + std::to_string(ho) + "-wide map: the direct conv's ring does not fit", kErrUnsupported);
         ConvGemmOp op;
         setup_gather_conv(op, LD_GATHER_CONV, x, z[i], ldx, nullptr, 0, 0, B, hs, hs, ho, ho, 3, 3, 2, 1, 0);
         op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.bias = down_conv[i].bias; op.p.out16 = dn; op.p.ld_out16 = z[i + 1];
@@ -922,7 +972,10 @@ class Model {
         const long Mi = (long)B * hs * hs;
         __half* ytap = pl.pool.alloc_n<__half>(Mi * 9 * Cout);
         ConvGemmOp op;
-        setup_tma_gemm2(op, x, Cin, ldx, skip, Cin, ld_skip, Mi);
+        if (Cin == 8)   // 8-channel sources: a 1x1 gathered conv over [x | skip] (the TMA GEMM's K block is at least 16 per source)
+          setup_gather_conv(op, LD_GATHER_CONV, x, Cin, ldx, skip, Cin, ld_skip, B, hs, hs, hs, hs, 1, 1, 1, 0, 0);
+        else
+          setup_tma_gemm2(op, x, Cin, ldx, skip, Cin, ld_skip, Mi);
         op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.out16 = ytap; op.p.ld_out16 = 9 * Cout;
         add_conv(pl, op, up_conv[j], "unet.uptap1x1." + std::to_string(2 * Cin) + "-" + std::to_string(9 * Cout) + "@" + std::to_string(hs));
         // then bilinear x2 + reflect pad + 3x3 tap sum + LayerNorm + ReLU (CUDA cores, memory-bound)

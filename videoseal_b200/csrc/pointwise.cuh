@@ -116,6 +116,83 @@ __global__ void __launch_bounds__(256) unet_first_kernel(const float* __restrict
   }
 }
 
+// K0 for Z = 8 (unet_tiny_*): the same arithmetic with the whole 16-byte pixel per thread.  Thread = 4 horizontally adjacent
+// pixels x all 8 channels (block = 16 rows x 64 columns); the 16 lanes of a half-warp store 64 consecutive pixels' 1 KB.
+template <int CIN>
+__global__ void __launch_bounds__(256) unet_first_z8_kernel(const float* __restrict__ imgs, int B, int H, int W,
+                                                            const float* __restrict__ w1 /*[8][CIN][3][3]*/, const float* __restrict__ b1,
+                                                            const float* __restrict__ wr /*[8][CIN]*/, const float* __restrict__ br,
+                                                            __half* __restrict__ h1, __half* __restrict__ res, int yuv) {
+  constexpr int NP = 4, TW = 16 * NP, TH = 16;
+  __shared__ float tile[CIN][TH + 2][TW + 2 + 2];
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+  const int x0 = blockIdx.x * TW, y0 = blockIdx.y * TH, b = blockIdx.z;
+  const float* img = imgs + (long)b * 3 * H * W;
+  for (int i = threadIdx.x; i < (TH + 2) * (TW + 2); i += 256) {
+    const int ly = i / (TW + 2), lx = i - ly * (TW + 2);
+    const int gy = y0 + ly - 1, gx = x0 + lx - 1;
+    const bool in = gy >= 0 && gy < H && gx >= 0 && gx < W;
+    if (CIN == 1) {
+      float v = 0.f;
+      if (in) {
+        const long o = (long)gy * W + gx;
+        const float y = 0.299f * __ldg(img + o) + 0.587f * __ldg(img + (long)H * W + o) + 0.114f * __ldg(img + 2L * H * W + o);
+        v = 2.f * y - 1.f;
+      }
+      tile[0][ly][lx] = v;
+    } else {
+#pragma unroll
+      for (int c = 0; c < CIN; ++c) tile[c][ly][lx] = in ? 2.f * __ldg(img + (long)c * H * W + (long)gy * W + gx) - 1.f : 0.f;
+    }
+  }
+  __syncthreads();
+  const int gx = x0 + tx * NP, gy = y0 + ty;
+  if (gx >= W || gy >= H) return;
+  const long pix = ((long)b * H + gy) * W + gx;
+  const int npx = min(NP, W - gx);
+  float a[8][NP], rr[8][NP];
+#pragma unroll
+  for (int q = 0; q < 8; ++q) {
+    const float bz = __ldg(b1 + q), brz = __ldg(br + q);
+#pragma unroll
+    for (int p = 0; p < NP; ++p) { a[q][p] = bz; rr[q][p] = brz; }
+  }
+#pragma unroll
+  for (int c = 0; c < CIN; ++c) {
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      float xr[NP + 2];
+#pragma unroll
+      for (int s = 0; s < NP + 2; ++s) xr[s] = tile[c][ty + r][tx * NP + s];
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+#pragma unroll
+        for (int s = 0; s < 3; ++s) {
+          const float wv = __ldg(w1 + (q * CIN + c) * 9 + r * 3 + s);
+#pragma unroll
+          for (int p = 0; p < NP; ++p) a[q][p] = fmaf(xr[p + s], wv, a[q][p]);
+        }
+        if (r == 1) {
+          const float wv = __ldg(wr + q * CIN + c);
+#pragma unroll
+          for (int p = 0; p < NP; ++p) rr[q][p] = fmaf(xr[p + 1], wv, rr[q][p]);
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int p = 0; p < NP; ++p) {
+    if (p < npx) {
+      __align__(16) __half ho[8];
+      __align__(16) __half ro[8];
+#pragma unroll
+      for (int q = 0; q < 8; ++q) { ho[q] = __float2half_rn(fmaxf(a[q][p], 0.f)); ro[q] = __float2half_rn(rr[q][p]); }
+      *reinterpret_cast<uint4*>(h1 + (pix + p) * 8) = *reinterpret_cast<const uint4*>(ho);
+      *reinterpret_cast<uint4*>(res + (pix + p) * 8) = *reinterpret_cast<const uint4*>(ro);
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // K6: modules/msg_processor.py:88-115 (binary + concat).  msgs: [B, K] uint8 {0,1}; table: [2K, hidden] fp32.
 // Writes the `hidden` message channels (constant over the h x w map) into channels [c_off, c_off+hidden) of the

@@ -257,15 +257,35 @@ int vsb_debug_conv(const vsb_conv_test* t, void* stream) {
     VSB_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
   }
   if (t->loader == 5) {
-    // direct 3x3 conv (conv3_direct.cuh): weights arrive as [N][9*C0] and are re-packed here
-    VSB_CHECK(((t->R == 3 && t->S == 3 && t->pad == 1) || (t->R == 1 && t->S == 1 && t->pad == 0)) && t->stride == 1 && t->C1 == 0,
-              "direct conv: 3x3 pad 1 or 1x1, stride 1");
-    // (one scratch buffer, never freed: test-only path; the small pack kernel runs on every call)
+    // direct 3x3 conv (conv3_direct.cuh): weights arrive as [N][9*C0] and are re-packed here.  Stride 2 (3x3, pad 1) runs the
+    // space-to-depth mode of the model's down convs; 8-channel inputs and stride 2 re-index the weights on the host first.
+    const bool s2 = t->stride == 2;
+    VSB_CHECK(((t->R == 3 && t->S == 3 && t->pad == 1) || (t->R == 1 && t->S == 1 && t->pad == 0 && !s2)) && (t->stride == 1 || s2) &&
+              t->C1 == 0, "direct conv: 3x3 pad 1 or 1x1, stride 1; 3x3 pad 1 stride 2");
+    VSB_CHECK(!s2 || (t->IH % 2 == 0 && t->IW % 2 == 0), "direct conv: stride 2 needs an even input map");
+    // (scratch buffers, never freed: test-only path; the small pack kernel runs on every call)
     static __half* wpk = nullptr;
+    static __half* wtmp = nullptr;
     if (wpk == nullptr) VSB_CUDA(cudaMalloc(&wpk, (size_t)64 * 9 * 64 * sizeof(__half)));
-    pack_direct_weights((const __half*)t->weights, t->N, t->C0, wpk, (cudaStream_t)stream, t->R * t->S);
+    const int T = t->R * t->S;
+    if (s2 || t->C0 == 8) {
+      VSB_CHECK((size_t)t->N * 9 * (s2 ? 4 * t->C0 : 16) <= (size_t)64 * 9 * 64, "direct conv: weights too large for the test path");
+      if (wtmp == nullptr) VSB_CUDA(cudaMalloc(&wtmp, (size_t)64 * 9 * 64 * sizeof(__half)));
+      std::vector<__half> hw((size_t)t->N * T * t->C0);
+      VSB_CUDA(cudaMemcpy(hw.data(), t->weights, hw.size() * sizeof(__half), cudaMemcpyDeviceToHost));
+      std::vector<float> w(hw.size());
+      for (size_t i = 0; i < hw.size(); ++i) w[i] = __half2float(hw[i]);
+      const std::vector<float> v = s2 ? s2d_weights(w, t->N, t->C0) : direct8_weights(w, t->N, t->R);
+      std::vector<__half> vh(v.size());
+      for (size_t i = 0; i < v.size(); ++i) vh[i] = __float2half_rn(v[i]);
+      VSB_CUDA(cudaMemcpy(wtmp, vh.data(), vh.size() * sizeof(__half), cudaMemcpyHostToDevice));
+      pack_direct_weights(wtmp, t->N, s2 ? 4 * t->C0 : 16, wpk, (cudaStream_t)stream, s2 ? 9 : t->R * ((t->R + 1) / 2));
+    } else {
+      pack_direct_weights((const __half*)t->weights, t->N, t->C0, wpk, (cudaStream_t)stream, T);
+    }
     Conv3DirectOp dop;
-    setup_conv3_direct(dop, (const __half*)t->src0, t->B, t->IH, t->IW, t->C0, t->N, wpk, num_sms, t->R);
+    if (s2) setup_down_s2d_direct(dop, (const __half*)t->src0, t->C0, t->B, t->IH / 2, t->IW / 2, t->N, wpk, t->bias, (__half*)t->out16, num_sms);
+    else setup_conv3_direct(dop, (const __half*)t->src0, t->B, t->IH, t->IW, t->C0, t->N, wpk, num_sms, t->R);
     dop.p.relu = t->act == ACT_RELU ? 1 : 0;
     dop.p.bias = t->bias; dop.p.resid = (const __half*)t->resid16; dop.p.out = (__half*)t->out16;
     dop.p.outc_w = t->outc_w; dop.p.outc_b = t->outc_b; dop.p.n_out = t->n_out; dop.p.delta = t->delta; dop.p.outc_tanh = 1;

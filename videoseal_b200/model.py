@@ -133,6 +133,8 @@ class Videoseal(nn.Module):
         if v != self.spec["img_size"]:
             if v <= 0 or v % 128 != 0:
                 raise ValueError(f"img_size={v}: the native path needs a processing size that is a positive multiple of 128")
+            from .cfg import check_unet
+            check_unet(self.spec["unet"]["z"], v)
             if self.pixelwise:
                 from .cfg import check_pixel_decoder
                 check_pixel_decoder(self.spec["convnext"]["dims"][-1], self.spec["pixel_decoder"]["upscale_stages"], v,
