@@ -76,7 +76,7 @@ def test_unsupported_card_features_raise_at_load():
                                             # large up-scales (the delta of the blend at 1080p / 4K)
                                             (256, 1920, True), (256, 2160, False), (512, 1080, True)])
 def test_resample_tables_match_aten_interpolate(built_lib, n_in, n_out, aa):
-    """the host-built separable tables of the resize kernels (model.cuh:make_resample) against F.interpolate applied to the
+    """the host-built separable tables of the resize kernels (resize_blend_host.cuh:make_resample) against F.interpolate applied to the
     identity: every output sample's tap positions and weights (wam.py:163,184,224 call sites; bilinear, align_corners=False).
     Anti-aliased down-scales are computed in double and rounded once to fp32, so they are held to float64 ATen; the plain
     bilinear tables take their source coordinate in fp32 (as ATen's fp32 kernels do), so they are held to fp32 ATen."""

@@ -90,11 +90,7 @@ inline void setup_conv3_direct(Conv3DirectOp& op, const __half* x, int B, int H,
 
 template <int N, int KS, int R, int MODE = 0>
 inline void launch_direct_nkr(const Conv3DirectOp& op, cudaStream_t st) {
-  static bool attr = false;
-  if (!attr) {
-    VSB_CUDA(cudaFuncSetAttribute(conv3_direct_kernel<N, KS, R, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr = true;
-  }
+  smem_optin<conv3_direct_kernel<N, KS, R, MODE>>(227 * 1024);
   launch_pdl(conv3_direct_kernel<N, KS, R, MODE>, dim3(op.grid), dim3(kD3Threads), op.smem, st, op.p);
   VSB_CUDA(cudaGetLastError());
 }

@@ -1,9 +1,11 @@
 // Host-side construction + launch of conv_gemm_kernel instances (tensor maps, tiling, smem budget).
 #pragma once
+#include <atomic>
 #include <cstdio>
 #include <cstring>
 #include <stdexcept>
 #include <string>
+#include <vector>
 
 #include "conv_gemm.cuh"
 
@@ -27,6 +29,33 @@ struct Error : std::runtime_error {
     if (_e != cudaSuccess)                                                                        \
       throw ::vsb::Error(std::string("CUDA error ") + cudaGetErrorString(_e) + " in " #expr " at " __FILE__ ":" + std::to_string(__LINE__), ::vsb::kErrCuda); \
   } while (0)
+
+// device allocations owned by one object, freed together
+struct DevicePool {
+  std::vector<void*> ptrs;
+  void* alloc(size_t n) {
+    void* p = nullptr;
+    n = (n + 255) & ~size_t(255);
+    if (n == 0) n = 256;
+    VSB_CUDA(cudaMalloc(&p, n));
+    ptrs.push_back(p);
+    return p;
+  }
+  template <class T> T* alloc_n(size_t n) { return reinterpret_cast<T*>(alloc(n * sizeof(T))); }
+  // zeroed before it returns: plans run on the caller's stream, which need not be ordered after stream 0
+  template <class T> T* alloc_zeroed(size_t n) {
+    T* p = alloc_n<T>(n);
+    VSB_CUDA(cudaMemset(p, 0, n * sizeof(T)));
+    VSB_CUDA(cudaDeviceSynchronize());
+    return p;
+  }
+  template <class T> T* upload(const std::vector<T>& v) {
+    T* p = alloc_n<T>(v.size());
+    VSB_CUDA(cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+    return p;
+  }
+  ~DevicePool() { for (void* p : ptrs) cudaFree(p); }
+};
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                     const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -376,13 +405,27 @@ inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
   VSB_CUDA(cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...));
 }
 
+// Device the C entry point on this thread runs on (set by its DeviceGuard, vsb200.cu); -1 outside one.
+inline thread_local int t_device = -1;
+
+// Allow kernel K `bytes` of dynamic shared memory on the current device, the first time K is launched there.  The limit is a
+// per-device attribute (cuKernelSetAttribute takes the device), so a process with models on several GPUs opts in on each of
+// them.  One bit per device; threads that race both set the same value.
+template <auto K>
+inline void smem_optin(size_t bytes) {
+  static std::atomic<uint64_t> done{0};
+  int dev = t_device;
+  if (dev < 0) VSB_CUDA(cudaGetDevice(&dev));
+  VSB_CHECK(dev < 64, "device index above 63");
+  const uint64_t bit = 1ull << dev;
+  if (done.load(std::memory_order_acquire) & bit) return;
+  VSB_CUDA(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  done.fetch_or(bit, std::memory_order_release);
+}
+
 template <int LOADER, int ACT>
 inline void launch_one(const ConvGemmOp& op, cudaStream_t st) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    VSB_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<LOADER, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
+  smem_optin<conv_gemm_kernel<LOADER, ACT>>(227 * 1024);
   launch_pdl(conv_gemm_kernel<LOADER, ACT>, dim3(op.grid), dim3(op.threads), op.smem, st, op.tmA, op.tmA2, op.tmB, op.tmO, op.p);
 }
 

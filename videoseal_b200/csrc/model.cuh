@@ -12,9 +12,8 @@
 #include "../../include/vsb200.h"
 #include "conv_gemm_host.cuh"
 #include "conv3_direct_host.cuh"
-#include "pointwise.cuh"
-#include "resize_blend.cuh"
-#include "dwconv_ring.cuh"
+#include "pointwise_host.cuh"
+#include "resize_blend_host.cuh"
 
 namespace vsb {
 
@@ -24,28 +23,6 @@ struct HostTensor {
   std::vector<float> data;
   std::vector<int64_t> shape;
   int64_t numel() const { int64_t n = 1; for (auto s : shape) n *= s; return n; }
-};
-
-// device allocations owned by one object, freed together
-struct DevicePool {
-  std::vector<void*> ptrs;
-  size_t bytes = 0;
-  void* alloc(size_t n) {
-    void* p = nullptr;
-    n = (n + 255) & ~size_t(255);
-    if (n == 0) n = 256;
-    VSB_CUDA(cudaMalloc(&p, n));
-    ptrs.push_back(p);
-    bytes += n;
-    return p;
-  }
-  template <class T> T* alloc_n(size_t n) { return reinterpret_cast<T*>(alloc(n * sizeof(T))); }
-  template <class T> T* upload(const std::vector<T>& v) {
-    T* p = alloc_n<T>(v.size());
-    VSB_CUDA(cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
-    return p;
-  }
-  ~DevicePool() { for (void* p : ptrs) cudaFree(p); }
 };
 
 struct ConvW {          // packed conv / linear weights: fp16 [N][K] (K order r,s,c) + fp32 bias
@@ -83,6 +60,18 @@ struct Profile {
 };
 static Profile g_profile;
 
+// runs `fn`, which makes `launches` kernel launches on `st`, under one profile entry `name` when profiling is on
+template <class Fn> void prof_scope(const std::string& name, cudaStream_t st, int launches, Fn&& fn) {
+  if (!g_profile.enabled) { fn(); g_launches += launches; return; }
+  cudaEvent_t a, b;
+  cudaEventCreate(&a); cudaEventCreate(&b);
+  cudaEventRecord(a, st);
+  fn();
+  cudaEventRecord(b, st);
+  g_launches += launches;
+  g_profile.pending.push_back({name, {a, b}});
+}
+
 struct Plan {
   DevicePool pool;
   uint64_t last_use = 0;    // LRU stamp of the plan cache
@@ -98,180 +87,12 @@ struct Plan {
   float* logits = nullptr;  // [B,1+K]
   float* out_maps = nullptr;  // pixel-wise detect plans: the caller's [B,1+K,P,P] slice, set per call
   void run(cudaStream_t st) {
-    if (!g_profile.enabled) {
-      for (auto& s : steps) { s.fn(st); g_launches += s.launches; }
-      return;
-    }
-    for (auto& s : steps) {
-      cudaEvent_t a, b;
-      cudaEventCreate(&a); cudaEventCreate(&b);
-      cudaEventRecord(a, st);
-      s.fn(st);
-      cudaEventRecord(b, st);
-      g_launches += s.launches;
-      g_profile.pending.push_back({s.name, {a, b}});
-    }
+    for (auto& s : steps) prof_scope(s.name, st, s.launches, [&] { s.fn(st); });
   }
 };
 
-// ATen-compatible separable resample tables (host) ------------------------------------------------
-struct ResampleHost {
-  std::vector<int> start, cnt;
-  std::vector<float> w;
-  int maxt = 0;
-};
-
-// aten/src/ATen/native/cpu/UpSampleKernel.cpp (_compute_indices_weights_aa, bilinear filter) for antialias=True;
-// plain half-pixel bilinear (align_corners=False) otherwise.  Upscaling with antialias=True degenerates to plain bilinear.
-inline ResampleHost make_resample(int in, int out, bool antialias) {
-  ResampleHost t;
-  const double scale = (double)in / (double)out;
-  if (antialias && scale > 1.0) {
-    const double support = scale;  // interp_size/2 * scale with interp_size = 2
-    t.maxt = (int)std::ceil(support) * 2 + 1;
-    t.start.resize(out); t.cnt.resize(out); t.w.assign((size_t)out * t.maxt, 0.f);
-    for (int i = 0; i < out; ++i) {
-      const double center = scale * (i + 0.5);
-      const double invscale = 1.0 / scale;
-      int xmin = (int)(center - support + 0.5); if (xmin < 0) xmin = 0;
-      int xmax = (int)(center + support + 0.5); if (xmax > in) xmax = in;
-      const int n = xmax - xmin;
-      double total = 0.0;
-      std::vector<double> ww(n);
-      for (int j = 0; j < n; ++j) {
-        double x = (j + xmin - center + 0.5) * invscale;
-        if (x < 0) x = -x;
-        ww[j] = x < 1.0 ? 1.0 - x : 0.0;
-        total += ww[j];
-      }
-      t.start[i] = xmin; t.cnt[i] = n;
-      for (int j = 0; j < n; ++j) t.w[(size_t)i * t.maxt + j] = (float)(total != 0.0 ? ww[j] / total : 0.0);
-    }
-  } else {
-    t.maxt = 2;
-    t.start.resize(out); t.cnt.resize(out); t.w.assign((size_t)out * 2, 0.f);
-    for (int i = 0; i < out; ++i) {
-      // area_pixel_compute_source_index(scale, dst, align_corners=false, cubic=false)
-      // single rounding (fused multiply-add), like the vectorised ATen CPU kernel and the CUDA one
-      float src = std::fmaf((float)scale, i + 0.5f, -0.5f);
-      if (src < 0.f) src = 0.f;
-      int x0 = (int)src; if (x0 > in - 1) x0 = in - 1;
-      const int x1 = x0 + ((x0 < in - 1) ? 1 : 0);
-      const float l1 = src - (float)x0, l0 = 1.f - l1;
-      t.start[i] = x0;
-      if (x1 == x0) { t.cnt[i] = 1; t.w[(size_t)i * 2] = 1.f; }
-      else { t.cnt[i] = 2; t.w[(size_t)i * 2] = l0; t.w[(size_t)i * 2 + 1] = l1; }
-    }
-  }
-  return t;
-}
-
-struct ResampleDev {
-  DevicePool pool;
-  ResampleTab tab;
-  // geometry of resize_sep_kernel for this (in -> out) pair: output rows per block, input rows per staging round, the largest
-  // number of input rows one block touches, dynamic shared memory
-  int toy = 8, gstage = 1, rin_max = 1;
-  size_t smem = 0;
-  ResampleDev(int ih, int iw, int oh, int ow, bool aa) {
-    ResampleHost y = make_resample(ih, oh, aa), x = make_resample(iw, ow, aa);
-    tab.ystart = pool.upload(y.start); tab.ycnt = pool.upload(y.cnt); tab.yw = pool.upload(y.w); tab.maxt_y = y.maxt;
-    tab.xstart = pool.upload(x.start); tab.xcnt = pool.upload(x.cnt); tab.xw = pool.upload(x.w); tab.maxt_x = x.maxt;
-    gstage = iw * 4 * 4 <= 16 * 1024 ? 4 : (iw * 4 * 2 <= 16 * 1024 ? 2 : 1);    // rows per staging round (kRsStages - 1 rounds in flight): 4, 2 or 1
-    for (toy = 8; toy >= 1; toy >>= 1) {
-      rin_max = 1;
-      for (int o0 = 0; o0 < oh; o0 += toy) {
-        const int o1 = std::min(oh, o0 + toy) - 1;
-        rin_max = std::max(rin_max, y.start[o1] + y.cnt[o1] - y.start[o0]);
-      }
-      smem = ((((size_t)rin_max * ow + 3) & ~(size_t)3) + kRsStages * (((size_t)gstage * iw + 8 + 3) & ~(size_t)3)) * sizeof(float);
-      if (smem <= 100 * 1024 || toy == 1) break;
-    }
-  }
-};
-
-// K4 v3 launch (dwconv_ring.cuh): tensor map of the fp32 NHWC residual stream + geometry, built once per plan step
-struct DwRingOp {
-  CUtensorMap tm;
-  int C = 0, B = 0, H = 0, R = 0;
-  const float *dww = nullptr, *dwb = nullptr, *lnw = nullptr, *lnb = nullptr;
-  __half* out = nullptr;
-};
-template <int C, int NS, int SX, int NSLOT>
-inline void launch_dw_ring_t(const DwRingOp& op, cudaStream_t st) {
-  static bool attr = false;
-  constexpr size_t smem = dw_ring_smem<C, NS, SX, NSLOT>();
-  if (!attr) {
-    VSB_CUDA(cudaFuncSetAttribute(dwconv7_ln_ring_kernel<C, NS, SX, NSLOT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr = true;
-  }
-  const unsigned blocks = (unsigned)((long)op.B * (op.H / op.R) * (op.H / (NS * SX)));
-  launch_pdl(dwconv7_ln_ring_kernel<C, NS, SX, NSLOT>, dim3(blocks), dim3(NS * C / 2 + 32), smem, st, op.tm, op.B, op.H, op.H, op.dww, op.dwb, op.lnw,
-             op.lnb, op.out, op.R);
-  VSB_CUDA(cudaGetLastError());
-}
-// (384 channels take the whole-row strip kernel: at 16 x 16 maps a ring block would run one 192-thread block per SM with a
-//  14-step prologue per 8 rows)
-inline bool dw_ring_ok(int C, int H, int ld) { return ld == C && (C == 96 || C == 192) && H % 16 == 0; }
-inline void setup_dw_ring(DwRingOp& op, const float* x, int B, int H, int C) {
-  op.C = C; op.B = B; op.H = H;
-  op.R = H % 32 == 0 ? 32 : 16;    // rows per block: 6 halo rows + the block prologue are amortised over R
-  const int BW = (C == 96 ? 8 : 4) + 6;
-  uint64_t dims[4] = {(uint64_t)C, (uint64_t)H, (uint64_t)H, (uint64_t)B};
-  uint64_t strides[3] = {(uint64_t)C * 4, (uint64_t)H * C * 4, (uint64_t)H * H * C * 4};
-  uint32_t box[4] = {(uint32_t)C, (uint32_t)BW, 1u, 1u};
-  encode_map(&op.tm, x, 4, dims, strides, box, 0, true, /*f32=*/true);
-}
-inline void launch_dw_ring(const DwRingOp& op, cudaStream_t st) {
-  if (op.C == 96) launch_dw_ring_t<96, 2, 4, 8>(op, st);
-  else launch_dw_ring_t<192, 1, 4, 8>(op, st);
-}
-
-// Pixel-decoder gather launches (pointwise.cuh K3 with F in {2, 4} and GELU).  kPdMaxSmem: the opt-in shared memory of one H100 block.
+// tiling cap of the pixel decoder's gather kernels: the opt-in shared memory of one H100 block
 constexpr size_t kPdMaxSmem = 227 * 1024;
-template <int VPT, int F>
-inline void launch_pd_stage_t(bool tiled, size_t smem, const __half* y, int B, int IH, int C, const float* lw, const float* lb, __half* out,
-                              int ld_out, int num_sms, cudaStream_t st) {
-  if (tiled) {
-    static bool attr = false;
-    if (!attr) { VSB_CUDA(cudaFuncSetAttribute(ups_gather_ln_tiled_kernel<VPT, F, kUpGelu, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPdMaxSmem)); attr = true; }
-    const int tiles = IH / (16 / F);
-    ups_gather_ln_tiled_kernel<VPT, F, kUpGelu, false><<<(unsigned)((long)B * tiles * tiles), 256, smem, st>>>(y, B, IH, IH, C, lw, lb, 1e-6f, out, ld_out);
-  } else {
-    const int ppb = 256 / (C / (8 * VPT));
-    const long npix = (long)B * F * IH * F * IH;
-    const unsigned grid = (unsigned)std::min<long>((npix + ppb - 1) / ppb, (long)num_sms * 32);
-    ups_gather_ln_kernel<VPT, F, kUpGelu><<<grid, 256, 0, st>>>(y, B, IH, IH, C, lw, lb, 1e-6f, out, ld_out);
-  }
-  VSB_CUDA(cudaGetLastError());
-}
-inline void launch_pd_stage(int F, int vpt, bool tiled, size_t smem, const __half* y, int B, int IH, int C, const float* lw, const float* lb,
-                            __half* out, int ld_out, int num_sms, cudaStream_t st) {
-  if (F == 2 && vpt == 1) launch_pd_stage_t<1, 2>(tiled, smem, y, B, IH, C, lw, lb, out, ld_out, num_sms, st);
-  else if (F == 2 && vpt == 3) launch_pd_stage_t<3, 2>(tiled, smem, y, B, IH, C, lw, lb, out, ld_out, num_sms, st);
-  else if (F == 4 && vpt == 1) launch_pd_stage_t<1, 4>(tiled, smem, y, B, IH, C, lw, lb, out, ld_out, num_sms, st);
-  else if (F == 4 && vpt == 3) launch_pd_stage_t<3, 4>(tiled, smem, y, B, IH, C, lw, lb, out, ld_out, num_sms, st);
-  else throw Error("pixel decoder: no gather kernel for this stage", kErrUnsupported);
-}
-template <int VPT, int F>
-inline void launch_pd_head_t(size_t smem, const __half* y, int B, int IH, int C, const float* lw, const float* lb, const float* hw,
-                             const float* hb, int NO, float* maps, cudaStream_t st) {
-  static bool attr = false;
-  if (!attr) { VSB_CUDA(cudaFuncSetAttribute(ups_gather_ln_tiled_kernel<VPT, F, kUpGelu, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPdMaxSmem)); attr = true; }
-  const int tiles = IH / (16 / F);
-  ups_gather_ln_tiled_kernel<VPT, F, kUpGelu, true><<<(unsigned)((long)B * tiles * tiles), 256, smem, st>>>(
-      y, B, IH, IH, C, lw, lb, 1e-6f, nullptr, 0, hw, hb, NO, maps);
-  VSB_CUDA(cudaGetLastError());
-}
-// the last stage: C = 8 * VPT channels (G = 1: one thread per output pixel), VPT 1..4
-inline void launch_pd_head(int F, int vpt, size_t smem, const __half* y, int B, int IH, int C, const float* lw, const float* lb, const float* hw,
-                           const float* hb, int NO, float* maps, cudaStream_t st) {
-#define VSB_PDH(V, FF) if (F == FF && vpt == V) return launch_pd_head_t<V, FF>(smem, y, B, IH, C, lw, lb, hw, hb, NO, maps, st)
-  VSB_PDH(1, 2); VSB_PDH(2, 2); VSB_PDH(3, 2); VSB_PDH(4, 2);
-  VSB_PDH(1, 4); VSB_PDH(2, 4); VSB_PDH(3, 4); VSB_PDH(4, 4);
-#undef VSB_PDH
-  throw Error("pixel-wise head: no kernel for this width", kErrUnsupported);
-}
 
 class Model {
  public:
@@ -489,68 +310,57 @@ class Model {
                     if (cf != 0.f) p[((size_t)((py * 2 + px) * Co + co) * 9 + (ey * 3 + ex)) * Ct + c] += kv * cf;
                   }
           }
-    __half* plain = wpool.upload(to_half(p));
-    *wd_out = wpool.alloc_n<__half>(p.size());
-    pack_direct_weights(plain, 4 * Co, Ct, *wd_out, 0, 9);
-    VSB_CUDA(cudaStreamSynchronize(0));
+    *wd_out = pack_direct_taps(p, 4 * Co, Ct);
     *wk_out = wpool.upload(wk);
   }
-  // DBlock.down weights [N][Cin][3][3] re-indexed for the space-to-depth ring conv (conv3_direct_host.cuh,
-  // setup_down_s2d_direct): K = (ey*3+ex)*4Cin + (dy*2+dx)*Cin + c with tap r -> (ey, dy) = (0,1), (1,0), (1,1)
-  __half* pack_down_s2d(const std::string& wkey) {
-    const HostTensor& w = get(wkey);
-    const int N = (int)w.shape[0], Ci = (int)w.shape[1], Cs = 4 * Ci;
-    static const int E[3] = {0, 1, 1}, D[3] = {1, 0, 1};
-    std::vector<float> p((size_t)N * 9 * Cs, 0.f);
+  // conv weight [N][C][R][R] (x out_scale) -> fp32 taps [N][R*R][C] (K order r, s, c)
+  std::vector<float> conv_taps(const HostTensor& w, const std::vector<float>* out_scale) const {
+    const int N = (int)w.shape[0], C = (int)w.shape[1], T = w.shape.size() == 4 ? (int)(w.shape[2] * w.shape[3]) : 1;
+    std::vector<float> t((size_t)N * T * C);
     for (int n = 0; n < N; ++n)
-      for (int c = 0; c < Ci; ++c)
-        for (int r = 0; r < 3; ++r)
-          for (int s2 = 0; s2 < 3; ++s2)
-            p[((size_t)n * 9 + (E[r] * 3 + E[s2])) * Cs + (D[r] * 2 + D[s2]) * Ci + c] = w.data[(((size_t)n * Ci + c) * 3 + r) * 3 + s2];
-    __half* plain = wpool.upload(to_half(p));
-    __half* wd = wpool.alloc_n<__half>(p.size());
-    pack_direct_weights(plain, N, Cs, wd, 0, 9);
+      for (int c = 0; c < C; ++c)
+        for (int k = 0; k < T; ++k) {
+          float v = w.data[((size_t)n * C + c) * T + k];
+          if (out_scale) v *= (*out_scale)[n];
+          t[((size_t)n * T + k) * C + c] = v;
+        }
+    return t;
+  }
+  // fp32 taps [N][T][C] -> weights in the direct conv's core-matrix layout (pack_direct_weights_kernel); each value is rounded to
+  // fp16 once, and the fp16 copy the kernel reads is freed once it is done
+  __half* pack_direct_taps(const std::vector<float>& taps, int N, int C, int T = 9) {
+    DevicePool tmp;
+    __half* wd = wpool.alloc_n<__half>(taps.size());
+    pack_direct_weights(tmp.upload(to_half(taps)), N, C, wd, 0, T);
     VSB_CUDA(cudaStreamSynchronize(0));
     return wd;
   }
-  // 8-channel convs (unet_tiny_*) run only on the direct kernel's 8-channel instantiation (conv3_direct.cuh, KS = 0):
-  // [N][8][R][R] (x out_scale) -> its virtual-tap weight layout (direct8_weights)
-  __half* pack_direct8(const std::string& wkey, const std::vector<float>* out_scale) {
+  // stride-1 3x3 / 1x1 conv weights for the direct conv (conv3_direct.cuh); 8 -> 8 channels (unet_tiny_*) run only on its
+  // 8-channel instantiation (KS = 0), through the virtual-tap layout of direct8_weights
+  __half* pack_direct(const std::string& wkey, const std::vector<float>* out_scale) {
     const HostTensor& w = get(wkey);
-    const int N = (int)w.shape[0], R = w.shape.size() == 4 ? (int)w.shape[2] : 1;
-    VSB_CHECK((int)w.shape[1] == 8 && N == 8, "8-channel conv weight shape");
-    std::vector<float> t((size_t)N * R * R * 8);
-    for (int n = 0; n < N; ++n)
-      for (int c = 0; c < 8; ++c)
-        for (int k = 0; k < R * R; ++k) {
-          float v = w.data[((size_t)n * 8 + c) * R * R + k];
-          if (out_scale) v *= (*out_scale)[n];
-          t[((size_t)n * R * R + k) * 8 + c] = v;
-        }
-    const std::vector<float> v = direct8_weights(t, N, R);
-    __half* plain = wpool.upload(to_half(v));
-    __half* wd = wpool.alloc_n<__half>(v.size());
-    pack_direct_weights(plain, N, 16, wd, 0, R * ((R + 1) / 2));
-    VSB_CUDA(cudaStreamSynchronize(0));
-    return wd;
+    const int N = (int)w.shape[0], C = (int)w.shape[1], R = w.shape.size() == 4 ? (int)w.shape[2] : 1;
+    if (C != 8) return pack_direct_taps(conv_taps(w, out_scale), N, C, R * R);
+    VSB_CHECK(N == 8, "8-channel conv weight shape");
+    return pack_direct_taps(direct8_weights(conv_taps(w, out_scale), N, R), N, 16, R * ((R + 1) / 2));
+  }
+  // DBlock.down weights for the space-to-depth ring conv (conv3_direct_host.cuh, setup_down_s2d_direct)
+  __half* pack_down_s2d(const std::string& wkey) {
+    const HostTensor& w = get(wkey);
+    const int N = (int)w.shape[0], Ci = (int)w.shape[1];
+    return pack_direct_taps(s2d_weights(conv_taps(w, nullptr), N, Ci), N, 4 * Ci);
   }
   static bool use_halo(int C) { return C <= 16; }
   ConvW pack_conv3(const std::string& wkey, const std::vector<float>* out_scale, const std::vector<float>& bias) {
     const int C = (int)get(wkey).shape[1], N = (int)get(wkey).shape[0];
-    if (C == 8) {
-      ConvW cw;
+    ConvW cw;
+    if (C == 8) {   // no GEMM path
       cw.N = N; cw.K = 9 * C;
       cw.bias = wpool.upload(bias);
-      cw.wd = pack_direct8(wkey, out_scale);
-      return cw;
+    } else {
+      cw = use_halo(C) ? pack_conv_halo(wkey, out_scale, bias, C, 0) : pack_conv(wkey, out_scale, bias);
     }
-    ConvW cw = use_halo(C) ? pack_conv_halo(wkey, out_scale, bias, C, 0) : pack_conv(wkey, out_scale, bias);
-    if (conv3_direct_ok(C, N, C)) {
-      ConvW plain = use_halo(C) ? pack_conv(wkey, out_scale, {}) : cw;   // [N][9*C], K order (r, s, c)
-      cw.wd = wpool.alloc_n<__half>((size_t)N * 9 * C);
-      pack_direct_weights(plain.w, N, C, cw.wd, 0);
-      VSB_CUDA(cudaStreamSynchronize(0));
-    }
+    if (C == 8 || conv3_direct_ok(C, N, C)) cw.wd = pack_direct(wkey, out_scale);
     return cw;
   }
   // eval-mode BatchNorm2d folded into the preceding bias-free conv: w' = w*g/sqrt(var+eps), b' = beta - mean*g/sqrt(var+eps)
@@ -572,13 +382,8 @@ class Model {
     bn_fold(key + ".double_conv.4", s, b);
     rb.c2 = pack_conv3(key + ".double_conv.3.weight", &s, b);
     rb.res = pack_conv(key + ".res_conv.weight", nullptr, get(key + ".res_conv.bias").data);
-    if (rb.res.K == 8) {
-      rb.res.wd = pack_direct8(key + ".res_conv.weight", nullptr);
-    } else if (conv3_direct_ok(rb.res.K, rb.res.N, rb.res.K, 0, 1)) {   // narrow 1x1: same ring kernel with a single tap
-      rb.res.wd = wpool.alloc_n<__half>((size_t)rb.res.N * rb.res.K);
-      pack_direct_weights(rb.res.w, rb.res.N, rb.res.K, rb.res.wd, 0, 1);
-      VSB_CUDA(cudaStreamSynchronize(0));
-    }
+    if (rb.res.K == 8 || conv3_direct_ok(rb.res.K, rb.res.N, rb.res.K, 0, 1))   // narrow 1x1: same ring kernel with a single tap
+      rb.res.wd = pack_direct(key + ".res_conv.weight", nullptr);
     return rb;
   }
 
@@ -765,12 +570,38 @@ class Model {
     finalize_op(op, w_override ? w_override : w.w, w.N, w.K, w.ld ? w.ld : w.K, num_sms, block_n);
     pl.steps.push_back(Step{[op](cudaStream_t st) { launch(op, st); }, 1, name});
   }
-  // 3x3 stride-1 zero-padded conv: on-chip im2col from a shared-memory halo tile (input crosses L2->SM once) up to
-  // 16 input channels, one TMA load per tap above (use_halo); the weight layout was chosen by the same rule at pack time
-  // (pack_conv3)
-  void setup_conv3(ConvGemmOp& op, const __half* x, int B, int H, int W, int C, int ld) {
-    if (use_halo(C)) setup_halo_conv3(op, x, B, H, W, C, ld);
-    else setup_tma_conv(op, x, B, H, W, C, ld, 3, 3, 1);
+
+  // One U-Net conv step, R x R (3: stride 1, zero pad 1; or 1) over x [B,H,W,Cin] (pitch ldx): the direct ring conv when its
+  // weights were packed and the map allows it, else the tensor-core GEMM.  Epilogue: bias, ReLU (relu), + the fp16 residual
+  // `resid` (pitch w.N), output `out` (pitch ld_out; nullptr: not written) and, fuse_outc, the 1x1 outc + tanh into pl.delta.
+  void add_unet_conv(Plan& pl, const ConvW& w, int R, const __half* x, int B, int H, int W, int Cin, int ldx, bool relu,
+                     const __half* resid, __half* out, int ld_out, bool fuse_outc = false) {
+    const int N = w.N;
+    const bool direct = w.wd && conv3_direct_ok(Cin, N, ldx, W, R) && (out == nullptr || ld_out == N);
+    const std::string name = std::string("unet.conv") + (R == 3 ? "3x3" : "1x1") + (direct ? "d" : "") + (fuse_outc ? "+outc." : ".") +
+                             std::to_string(Cin) + "-" + std::to_string(N) + "@" + std::to_string(H);
+    if (direct) {
+      Conv3DirectOp op; setup_conv3_direct(op, x, B, H, W, Cin, N, w.wd, num_sms, R);
+      op.p.bias = w.bias; op.p.relu = relu ? 1 : 0; op.p.resid = resid; op.p.out = out;
+      if (fuse_outc) {
+        op.p.outc_w = outc_w; op.p.outc_b = outc_b; op.p.n_out = d.unet_out_ch; op.p.delta = pl.delta; op.p.outc_tanh = d.unet_last_tanh;
+      }
+      pl.steps.push_back(Step{[op](cudaStream_t st) { launch_direct(op, st); }, 1, name});
+      return;
+    }
+    // 3x3 up to 16 input channels: on-chip im2col from a shared-memory halo tile (input crosses L2->SM once), one TMA load per tap
+    // above; the weight layout was chosen by the same rule at pack time (pack_conv3)
+    ConvGemmOp op;
+    if (R == 3 && use_halo(Cin)) setup_halo_conv3(op, x, B, H, W, Cin, ldx);
+    else setup_tma_conv(op, x, B, H, W, Cin, ldx, R, R, R / 2);
+    op.p.epi = EPI_AFFINE; op.p.act = relu ? ACT_RELU : ACT_NONE; op.p.bias = w.bias;
+    if (resid) { op.p.resid16 = resid; op.p.ld_res16 = N; }
+    if (out) { op.p.out16 = out; op.p.ld_out16 = ld_out; }
+    if (fuse_outc) {
+      op.p.outc_w = outc_w; op.p.outc_b = outc_b; op.p.n_out = d.unet_out_ch; op.p.delta = pl.delta; op.p.hw = H * W;
+      op.p.outc_tanh = d.unet_last_tanh;
+    }
+    add_conv(pl, op, w, name);
   }
 
   // ResnetBlock on NHWC fp16 (modules/unet.py:17-39):  out = relu(conv3'(relu(conv3'(x)))) + (conv1(x) + b)
@@ -786,46 +617,9 @@ class Model {
     if (Cout == 8 && !(conv3_direct_ok(8, 8, ldx, W) && conv3_direct_ok(8, 8, ldx, W, 1) && (out == nullptr || ld_out == 8)))
       throw Error("8-channel ResnetBlock on a " + std::to_string(W) + "-wide map: the direct conv's ring does not fit (processing "
                   "size too large for an 8-channel U-Net)", kErrUnsupported);
-    if (w.res.wd && conv3_direct_ok(Cin, Cout, ldx, W, 1)) {  // res 1x1, narrow layers
-      Conv3DirectOp op; setup_conv3_direct(op, x, B, H, W, Cin, Cout, w.res.wd, num_sms, 1);
-      op.p.bias = w.res.bias; op.p.out = r; op.p.relu = 0;
-      pl.steps.push_back(Step{[op](cudaStream_t st) { launch_direct(op, st); }, 1,
-                              "unet.conv1x1d." + std::to_string(Cin) + "-" + std::to_string(Cout) + "@" + std::to_string(H)});
-    } else {  // res 1x1
-      ConvGemmOp op; setup_tma_conv(op, x, B, H, W, Cin, ldx, 1, 1, 0);
-      op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.bias = w.res.bias; op.p.out16 = r; op.p.ld_out16 = Cout;
-      add_conv(pl, op, w.res, "unet.conv1x1." + std::to_string(Cin) + "-" + std::to_string(Cout) + "@" + std::to_string(H));
-    }
-    const std::string sfx = "@" + std::to_string(H);
-    if (w.c1.wd && conv3_direct_ok(Cin, Cout, ldx, W)) {  // conv3 + BN + ReLU, narrow layers: straight from a ring of padded rows
-      Conv3DirectOp op; setup_conv3_direct(op, x, B, H, W, Cin, Cout, w.c1.wd, num_sms);
-      op.p.bias = w.c1.bias; op.p.out = h;
-      pl.steps.push_back(Step{[op](cudaStream_t st) { launch_direct(op, st); }, 1, "unet.conv3x3d." + std::to_string(Cin) + "-" + std::to_string(Cout) + sfx});
-    } else {  // conv3 + BN + ReLU
-      ConvGemmOp op; setup_conv3(op, x, B, H, W, Cin, ldx);
-      op.p.epi = EPI_AFFINE; op.p.act = ACT_RELU; op.p.bias = w.c1.bias; op.p.out16 = h; op.p.ld_out16 = Cout;
-      add_conv(pl, op, w.c1, "unet.conv3x3." + std::to_string(Cin) + "-" + std::to_string(Cout) + "@" + std::to_string(H));
-    }
-    if (w.c2.wd && conv3_direct_ok(Cout, Cout, Cout, W) && (out == nullptr || ld_out == Cout)) {
-      Conv3DirectOp op; setup_conv3_direct(op, h, B, H, W, Cout, Cout, w.c2.wd, num_sms);
-      op.p.bias = w.c2.bias; op.p.resid = r; op.p.out = out;
-      if (fuse_outc) {
-        op.p.outc_w = outc_w; op.p.outc_b = outc_b; op.p.n_out = d.unet_out_ch; op.p.delta = pl.delta; op.p.outc_tanh = d.unet_last_tanh;
-      }
-      pl.steps.push_back(Step{[op](cudaStream_t st) { launch_direct(op, st); }, 1,
-                              std::string(fuse_outc ? "unet.conv3x3d+outc." : "unet.conv3x3d.") + std::to_string(Cout) + "-" + std::to_string(Cout) + sfx});
-    } else {  // conv3 + BN + ReLU, + res
-      ConvGemmOp op; setup_conv3(op, h, B, H, W, Cout, Cout);
-      op.p.epi = EPI_AFFINE; op.p.act = ACT_RELU; op.p.bias = w.c2.bias; op.p.resid16 = r; op.p.ld_res16 = Cout;
-      if (fuse_outc) {
-        op.p.outc_w = outc_w; op.p.outc_b = outc_b; op.p.n_out = d.unet_out_ch; op.p.delta = pl.delta; op.p.hw = H * W;
-        op.p.outc_tanh = d.unet_last_tanh;
-        if (out) { op.p.out16 = out; op.p.ld_out16 = ld_out; }
-      } else {
-        op.p.out16 = out; op.p.ld_out16 = ld_out;
-      }
-      add_conv(pl, op, w.c2, std::string(fuse_outc ? "unet.conv3x3+outc." : "unet.conv3x3.") + std::to_string(Cout) + "-" + std::to_string(Cout) + "@" + std::to_string(H));
-    }
+    add_unet_conv(pl, w.res, 1, x, B, H, W, Cin, ldx, false, nullptr, r, Cout);
+    add_unet_conv(pl, w.c1, 3, x, B, H, W, Cin, ldx, true, nullptr, h, Cout);
+    add_unet_conv(pl, w.c2, 3, h, B, H, W, Cout, Cout, true, r, out, ld_out, fuse_outc);
     if (out) dbg(pl, name, out, 1, B, H, W, Cout, ld_out);
     return out;
   }
@@ -835,23 +629,28 @@ class Model {
   // is dropped (its cudaFree calls synchronise the device, so work still in flight on it completes first).
   uint64_t plan_clock = 0;
   int max_plans = [] { const char* e = getenv("VSB_MAX_PLANS"); const int v = e ? atoi(e) : 8; return v < 2 ? 2 : v; }();
-  void evict_plans(std::map<int, std::unique_ptr<Plan>>& m, const Plan* keep) {
+  Plan* get_plan(std::map<int, std::unique_ptr<Plan>>& m, int B, void (Model::*build)(Plan&, int)) {
+    auto it = m.find(B);
+    if (it != m.end()) { it->second->last_use = ++plan_clock; return it->second.get(); }
+    std::unique_ptr<Plan> up(new Plan());
+    (this->*build)(*up, B);
+    Plan* ret = up.get();
+    ret->last_use = ++plan_clock;
+    m[B] = std::move(up);
     while ((int)m.size() > max_plans) {
       auto victim = m.end();
       for (auto it = m.begin(); it != m.end(); ++it)
-        if (it->second.get() != keep && (victim == m.end() || it->second->last_use < victim->second->last_use)) victim = it;
+        if (it->second.get() != ret && (victim == m.end() || it->second->last_use < victim->second->last_use)) victim = it;
       if (victim == m.end()) break;
       if (victim->second.get() == last_plan) last_plan = nullptr;
       m.erase(victim);
     }
+    return ret;
   }
-  size_t cached_plans() const { return embed_plans.size() + detect_plans.size(); }
+  Plan* get_embed_plan(int B) { return get_plan(embed_plans, B, &Model::build_embed_plan); }
+  Plan* get_detect_plan(int B) { return get_plan(detect_plans, B, &Model::build_detect_plan); }
 
-  Plan* get_embed_plan(int B) {
-    auto it = embed_plans.find(B);
-    if (it != embed_plans.end()) { it->second->last_use = ++plan_clock; return it->second.get(); }
-    std::unique_ptr<Plan> up(new Plan());
-    Plan& pl = *up;
+  void build_embed_plan(Plan& pl, int B) {
     const int S = d.img_size, L = d.unet_levels;
     std::vector<int> z(d.unet_z, d.unet_z + L);
     pl.x_res = pl.pool.alloc_n<float>((size_t)B * 3 * S * S);
@@ -864,36 +663,17 @@ class Model {
     __half* r0 = pl.pool.alloc_n<__half>(M0 * z[0]);
     {
       const int Z = z[0], yuv = d.yuv, cin = d.unet_in_ch;
-      float *w1 = first_w1, *b1 = first_b1, *wr = first_wr, *br = first_br;
-      pl.steps.push_back(Step{[=](cudaStream_t st) {
-        dim3 grid((S + 31) / 32, (S + 15) / 16, B);
-        const float* src = plp->in_imgs;
-        if (Z == 8) {
-          const dim3 grid8((S + 63) / 64, (S + 15) / 16, B);
-          if (cin == 1) unet_first_z8_kernel<1><<<grid8, 256, 0, st>>>(src, B, S, S, w1, b1, wr, br, h1, r0, yuv);
-          else unet_first_z8_kernel<3><<<grid8, 256, 0, st>>>(src, B, S, S, w1, b1, wr, br, h1, r0, yuv);
-        } else if (cin == 1) unet_first_kernel<1><<<grid, 256, 0, st>>>(src, B, S, S, Z, w1, b1, wr, br, h1, r0, yuv);
-        else unet_first_kernel<3><<<grid, 256, 0, st>>>(src, B, S, S, Z, w1, b1, wr, br, h1, r0, yuv);
-        VSB_CUDA(cudaGetLastError());
-      }, 1, "unet.first"});
+      const float *w1 = first_w1, *b1 = first_b1, *wr = first_wr, *br = first_br;
+      pl.steps.push_back(Step{[=](cudaStream_t st) { launch_unet_first(plp->in_imgs, B, S, Z, cin, w1, b1, wr, br, h1, r0, yuv, st); }, 1,
+                              "unet.first"});
     }
     std::vector<__half*> skips;  // outputs of inc, downs[0..]
     std::vector<int> skip_ld;
     __half* x = pl.pool.alloc_n<__half>(M0 * z[0]);
-    if (inc_c2.wd && conv3_direct_ok(z[0], z[0], z[0], S)) {
-      Conv3DirectOp op; setup_conv3_direct(op, h1, B, S, S, z[0], z[0], inc_c2.wd, num_sms);
-      op.p.bias = inc_c2.bias; op.p.resid = r0; op.p.out = x;
-      pl.steps.push_back(Step{[op](cudaStream_t st) { launch_direct(op, st); }, 1,
-                              "unet.conv3x3d." + std::to_string(z[0]) + "-" + std::to_string(z[0]) + "@" + std::to_string(S)});
-      dbg(pl, "inc", x, 1, B, S, S, z[0], z[0]);
-    } else {
-      if (z[0] == 8) throw Error("8-channel inc block on a " + std::to_string(S) + "-wide map: the direct conv's ring does not fit", kErrUnsupported);
-      ConvGemmOp op; setup_conv3(op, h1, B, S, S, z[0], z[0]);
-      op.p.epi = EPI_AFFINE; op.p.act = ACT_RELU; op.p.bias = inc_c2.bias; op.p.resid16 = r0; op.p.ld_res16 = z[0];
-      op.p.out16 = x; op.p.ld_out16 = z[0];
-      add_conv(pl, op, inc_c2, "unet.conv3x3." + std::to_string(z[0]) + "-" + std::to_string(z[0]) + "@" + std::to_string(S));
-      dbg(pl, "inc", x, 1, B, S, S, z[0], z[0]);
-    }
+    if (z[0] == 8 && !conv3_direct_ok(8, 8, 8, S))
+      throw Error("8-channel inc block on a " + std::to_string(S) + "-wide map: the direct conv's ring does not fit", kErrUnsupported);
+    add_unet_conv(pl, inc_c2, 3, h1, B, S, S, z[0], z[0], true, r0, x, z[0]);
+    dbg(pl, "inc", x, 1, B, S, S, z[0], z[0]);
     int ldx = z[0], hs = S;
     const int zb = z[L - 1] + d.hidden;
     __half* cat = nullptr;
@@ -926,11 +706,9 @@ class Model {
     // ---- message channels
     {
       const int K = d.nbits, hidden = d.hidden, hw = hs * hs, coff = z[L - 1];
-      float* table = msg_table;
+      const float* table = msg_table;
       pl.steps.push_back(Step{[=](cudaStream_t st) {
-        dim3 grid(B, 8);
-        msg_embed_kernel<<<grid, 256, hidden * sizeof(float), st>>>(plp->in_msgs, table, K, hidden, cat, hw, zb, coff, plp->in_msg_stride);
-        VSB_CUDA(cudaGetLastError());
+        launch_msg_embed(plp->in_msgs, plp->in_msg_stride, table, K, hidden, cat, B, hw, zb, coff, st);
       }, 1, "unet.msg"});
       dbg(pl, "cat", cat, 1, B, hs, hs, zb, zb);
     }
@@ -958,15 +736,10 @@ class Model {
         pl.steps.push_back(Step{[op](cudaStream_t st) { launch_direct(op, st); }, 1,
                                 "unet.upphase." + std::to_string(2 * Cin) + "-" + std::to_string(Cout) + "@" + std::to_string(ho)});
         const __half *x0 = x, *x1 = skip;
-        const int IH = hs, Ci = Cin;
+        const int IH = hs, Ci = Cin, nsm = num_sms;
         const float *wk = up_border_w[j], *lw = up_lnw[j], *lb = up_lnb[j];
-        pl.steps.push_back(Step{[=](cudaStream_t st) {
-          const long nb = (long)B * (2 * (2 * IH) + 2 * (2 * IH - 2));
-          static bool attr = false;
-          if (!attr) { VSB_CUDA(cudaFuncSetAttribute(up_border_fix_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kUpFixSmem)); attr = true; }
-          up_border_fix_kernel<<<(unsigned)std::min<long>((nb + kUpFixPPB - 1) / kUpFixPPB, (long)num_sms * 3), 256, kUpFixSmem, st>>>(x0, Ci, x1, Ci, B, IH, IH, wk, lw, lb, 1e-6f, u);
-          VSB_CUDA(cudaGetLastError());
-        }, 1, "unet.upborder." + std::to_string(Cout) + "@" + std::to_string(ho)});
+        pl.steps.push_back(Step{[=](cudaStream_t st) { launch_up_border_fix(x0, x1, Ci, B, IH, wk, lw, lb, u, nsm, st); }, 1,
+                                "unet.upborder." + std::to_string(Cout) + "@" + std::to_string(ho)});
       } else {
         // channel mixing first, at low resolution: y[b,i,j, tap*Cout + co] = sum_c W[co,c,tap] * [x | skip/sqrt2][b,i,j,c]
         const long Mi = (long)B * hs * hs;
@@ -979,36 +752,16 @@ class Model {
         op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.out16 = ytap; op.p.ld_out16 = 9 * Cout;
         add_conv(pl, op, up_conv[j], "unet.uptap1x1." + std::to_string(2 * Cin) + "-" + std::to_string(9 * Cout) + "@" + std::to_string(hs));
         // then bilinear x2 + reflect pad + 3x3 tap sum + LayerNorm + ReLU (CUDA cores, memory-bound)
-        const int IH = hs, Cc = Cout;
-        float *lw = up_lnw[j], *lb = up_lnb[j];
-        const int vpt = Cc <= 256 ? 1 : 2;            // 16-byte channel vectors per thread (chunkyseal's first up-conv: 512 channels)
-        const int gthreads = Cc / (8 * vpt);          // threads per output pixel
-        VSB_CHECK(Cc % (8 * vpt) == 0 && gthreads <= 32 && (gthreads & (gthreads - 1)) == 0, "up conv: C_out must be 8 * 2^k <= 512");
-        const size_t tsmem = (size_t)100 * 9 * Cc * sizeof(__half);
-        if (IH % 8 == 0 && tsmem <= 160 * 1024) {
-          // low-resolution taps of a 16 x 16 output tile staged in shared memory (ups_gather_ln_tiled_kernel)
-          pl.steps.push_back(Step{[=](cudaStream_t st) {
-            const unsigned blocks = (unsigned)((long)B * (IH / 8) * (IH / 8));
-            if (vpt == 1) {
-              static bool attr = false;
-              if (!attr) { VSB_CUDA(cudaFuncSetAttribute(ups_gather_ln_tiled_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); attr = true; }
-              ups_gather_ln_tiled_kernel<1><<<blocks, 256, tsmem, st>>>(ytap, B, IH, IH, Cc, lw, lb, 1e-6f, u, Cc);
-            } else {
-              static bool attr = false;
-              if (!attr) { VSB_CUDA(cudaFuncSetAttribute(ups_gather_ln_tiled_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); attr = true; }
-              ups_gather_ln_tiled_kernel<2><<<blocks, 256, tsmem, st>>>(ytap, B, IH, IH, Cc, lw, lb, 1e-6f, u, Cc);
-            }
-            VSB_CUDA(cudaGetLastError());
-          }, 1, "unet.upgather." + std::to_string(Cout) + "@" + std::to_string(ho)});
-        } else
-        pl.steps.push_back(Step{[=](cudaStream_t st) {
-          const int ppb = 256 / gthreads;
-          const long blocks = (Mo + ppb - 1) / ppb;
-          const unsigned grid = (unsigned)std::min<long>(blocks, (long)num_sms * 32);
-          if (vpt == 1) ups_gather_ln_kernel<1><<<grid, 256, 0, st>>>(ytap, B, IH, IH, Cc, lw, lb, 1e-6f, u, Cc);
-          else ups_gather_ln_kernel<2><<<grid, 256, 0, st>>>(ytap, B, IH, IH, Cc, lw, lb, 1e-6f, u, Cc);
-          VSB_CUDA(cudaGetLastError());
-        }, 1, "unet.upgather." + std::to_string(Cout) + "@" + std::to_string(ho)});
+        const int vpt = Cout <= 256 ? 1 : 2;            // 16-byte channel vectors per thread (chunkyseal's first up-conv: 512 channels)
+        const int gthreads = Cout / (8 * vpt);          // threads per output pixel
+        VSB_CHECK(Cout % (8 * vpt) == 0 && gthreads <= 32 && (gthreads & (gthreads - 1)) == 0, "up conv: C_out must be 8 * 2^k <= 512");
+        UpsGather g;
+        g.y = ytap; g.B = B; g.IH = hs; g.C = Cout; g.lnw = up_lnw[j]; g.lnb = up_lnb[j]; g.out = u; g.ld_out = Cout; g.num_sms = num_sms;
+        // low-resolution taps of a 16 x 16 output tile staged in shared memory (ups_gather_ln_tiled_kernel) when they fit in 160 KB
+        g.optin = 160 * 1024;
+        g.smem = hs % 8 == 0 && ups_tile_smem(2, Cout) <= g.optin ? ups_tile_smem(2, Cout) : 0;
+        pl.steps.push_back(Step{[g, vpt](cudaStream_t st) { launch_unet_upgather(g, vpt, st); }, 1,
+                                "unet.upgather." + std::to_string(Cout) + "@" + std::to_string(ho)});
       }
       dbg(pl, "up" + std::to_string(j) + "_conv", u, 1, B, ho, ho, Cout, Cout);
       const bool last = (ii == 0);
@@ -1016,18 +769,9 @@ class Model {
       ldx = Cout; hs = ho;
     }
     dbg(pl, "delta", pl.delta, 0, B, d.unet_out_ch, S, S, S);
-    Plan* ret = up.get();
-    ret->last_use = ++plan_clock;
-    embed_plans[B] = std::move(up);
-    evict_plans(embed_plans, ret);
-    return ret;
   }
 
-  Plan* get_detect_plan(int B) {
-    auto it = detect_plans.find(B);
-    if (it != detect_plans.end()) { it->second->last_use = ++plan_clock; return it->second.get(); }
-    std::unique_ptr<Plan> up(new Plan());
-    Plan& pl = *up;
+  void build_detect_plan(Plan& pl, int B) {
     Plan* plp = &pl;
     const int S = d.img_size;
     pl.x_res = pl.pool.alloc_n<float>((size_t)B * 3 * S * S);
@@ -1044,27 +788,19 @@ class Model {
     float* x = pl.pool.alloc_n<float>((size_t)B * hs * hs * Cp);
     if (stem_wk != nullptr) {
       // widths > 256: CUDA-core stem conv + LayerNorm (one warp per output pixel); the fused-LN GEMM epilogue needs N <= 256
-      const int OH = hs, Cc = C, ldo = Cp;
-      float *wk = stem_wk, *sb = stem_b, *lw = stem_lnw, *lb = stem_lnb;
-      pl.steps.push_back(Step{[=](cudaStream_t st) {
-        const long npix = (long)B * OH * OH;
-        const int grid = (int)std::min<long>((npix + 7) / 8, (long)num_sms * 16);
-        stem_ln_kernel<<<grid, 256, (size_t)8 * (48 + Cc) * sizeof(float), st>>>(plp->in_imgs, B, S, S, OH, OH, st_, wk, sb, lw, lb, Cc, x, ldo);
-        VSB_CUDA(cudaGetLastError());
-      }, 1, "cnx.stem_ln." + std::to_string(C) + "@" + std::to_string(hs)});
+      const int OH = hs, Cc = C, ldo = Cp, nsm = num_sms;
+      const float *wk = stem_wk, *sb = stem_b, *lw = stem_lnw, *lb = stem_lnb;
+      pl.steps.push_back(Step{[=](cudaStream_t st) { launch_stem_ln(plp->in_imgs, B, S, OH, st_, wk, sb, lw, lb, Cc, x, ldo, nsm, st); }, 1,
+                              "cnx.stem_ln." + std::to_string(C) + "@" + std::to_string(hs)});
       dbg(pl, "ds0", x, 0, B, hs, hs, C, Cp);
     } else {
       // stem (convnext.py:108-111): im2col of the k4 patches (x = 2*img-1 folded) -> tensor-core GEMM [M,64]x[64,C0] with the
       // conv bias and the channels-first LayerNorm fused into the epilogue, fp32 NHWC output (the residual stream)
-      const int OH = hs;
+      const int OH = hs, nsm = num_sms;
       const long M = (long)B * OH * OH;
       __half* patches = pl.pool.alloc_n<__half>(M * 64);
-      pl.steps.push_back(Step{[=](cudaStream_t st) {
-        const long total = M * 4;
-        const int grid = (int)std::min<long>((total + 255) / 256, (long)num_sms * 32);
-        stem_im2col_kernel<<<grid, 256, 0, st>>>(plp->in_imgs, B, S, S, OH, OH, st_, patches);
-        VSB_CUDA(cudaGetLastError());
-      }, 1, "cnx.stem_im2col"});
+      pl.steps.push_back(Step{[=](cudaStream_t st) { launch_stem_im2col(plp->in_imgs, B, S, OH, st_, patches, nsm, st); }, 1,
+                              "cnx.stem_im2col"});
       ConvGemmOp op; setup_tma_gemm(op, patches, M, 64, 64);
       op.p.epi = EPI_LN; op.p.act = ACT_NONE; op.p.bias = stem_b; op.p.ln_w = stem_lnw; op.p.ln_b = stem_lnb; op.p.ln_eps = 1e-6f;
       op.p.out32 = x; op.p.ld_out32 = Cp;
@@ -1106,19 +842,12 @@ class Model {
       if (s > 0) {
         const int Cv = d.ext_dims[s - 1], Cvp = Cp, Cn = d.ext_dims[s], Cnp = pitch(Cn);
         const long Mp = (long)B * hs * hs;
-        __half* xn = pl.pool.alloc_n<__half>(Mp * Cvp);
-        if (Cvp != Cv) {   // pad channels stay zero: ln_rows writes [0, Cv)
-          VSB_CUDA(cudaMemset(xn, 0, (size_t)Mp * Cvp * sizeof(__half)));
-          VSB_CUDA(cudaDeviceSynchronize());   // the plan runs on the caller's stream, which need not be ordered after stream 0
-        }
+        // pad channels stay zero: ln_rows writes [0, Cv)
+        __half* xn = Cvp != Cv ? pl.pool.alloc_zeroed<__half>(Mp * Cvp) : pl.pool.alloc_n<__half>(Mp * Cvp);
         {
-          float *lw = ds[s - 1].lnw, *lb = ds[s - 1].lnb;
-          const float* xin = x;
-          pl.steps.push_back(Step{[=](cudaStream_t st) {
-            const int grid = (int)std::min<long>((Mp + 7) / 8, (long)num_sms * 16);
-            ln_rows_kernel<<<grid, 256, 0, st>>>(xin, Mp, Cv, Cvp, lw, lb, 1e-6f, xn, Cvp);
-            VSB_CUDA(cudaGetLastError());
-          }, 1, "cnx.ln_rows"});
+          const float *lw = ds[s - 1].lnw, *lb = ds[s - 1].lnb, *xin = x;
+          const int nsm = num_sms;
+          pl.steps.push_back(Step{[=](cudaStream_t st) { launch_ln_rows(xin, Mp, Cv, Cvp, lw, lb, xn, Cvp, nsm, st); }, 1, "cnx.ln_rows"});
         }
         const int ho = (hs - 2) / 2 + 1;   // odd maps (127, 63, 31): the last row / column is dropped, like nn.Conv2d k2 s2
         float* xo = pl.pool.alloc_n<float>((size_t)B * ho * ho * Cnp);
@@ -1141,51 +870,8 @@ class Model {
       for (int jb = 0; jb < d.ext_depths[s]; ++jb) {
         const CnBlockW& w = cn[s][jb];
         {
-          const int H = hs, Cc = C, ldc = Cp;
-          const float* xin = x;
-          float *dww = w.dww, *dwb = w.dwb, *lw = w.lnw, *lb = w.lnb;
-          if (dw_ring_ok(Cc, H, ldc)) {
-            // TMA-ring register-rolling kernel (dwconv_ring.cuh) for the 96 / 192-channel stages of the tiny trunk
-            DwRingOp rop;
-            setup_dw_ring(rop, xin, B, H, Cc);
-            rop.dww = dww; rop.dwb = dwb; rop.lnw = lw; rop.lnb = lb; rop.out = a;
-            pl.steps.push_back(Step{[rop](cudaStream_t st) { launch_dw_ring(rop, st); }, 1,
-                                    "cnx.dwconv7_ln." + std::to_string(C) + "@" + std::to_string(hs)});
-          } else
-          pl.steps.push_back(Step{[=](cudaStream_t st) {
-            if (!(Cc == 96 || Cc == 192 || Cc == 384 || Cc == 768)) {
-              // any even width / odd map size (chunkyseal's proportional trunk): threads loop over the channel pairs
-              const long nstrips = (long)B * H * ((H + kDwStrip - 1) / kDwStrip);
-              const int threads = std::min(512, (Cc / 2 + 31) / 32 * 32);
-              const size_t smem_w = (size_t)kDwStrip * Cc * sizeof(float);
-              static bool attr = false;
-              if (!attr) { VSB_CUDA(cudaFuncSetAttribute(dwconv7_ln_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr = true; }
-              if (smem_w > 200 * 1024) throw Error("dwconv7: more than 6400 channels is not implemented", kErrUnsupported);
-              dwconv7_ln_wide_kernel<<<(unsigned)nstrips, threads, smem_w, st>>>(xin, B, H, H, Cc, ldc, dww, dwb, lw, lb, a, ldc);
-              VSB_CUDA(cudaGetLastError());
-              return;
-            }
-            const int strips = (H + kDwStrip - 1) / kDwStrip;
-            const long nstrips = (long)B * H * strips;
-            const int C2 = Cc / 2;
-            int spb = 1;
-            for (int s2 = 1; s2 <= 4; s2 *= 2) if ((s2 * C2) % 32 == 0 && s2 * C2 <= 512) { spb = s2; break; }
-            if (spb * C2 > 512) throw Error("dwconv7: C/2 > 512 threads is not implemented (unsupported chunky extractor width)", kErrUnsupported);
-#define VSB_DWC(CC, ST, FR, SPB, NGR) dwconv7_ln_c_kernel<CC, ST, FR><<<(unsigned)(((NGR) + (SPB) - 1) / (SPB)), (SPB) * (CC) / 2, \
-    (size_t)(SPB) * (ST) * (CC) * sizeof(float), st>>>(xin, B, H, H, dww, dwb, lw, lb, a, Cc, SPB, (int)(NGR))
-            {
-              // narrow maps: one strip = the whole row, so no column is ever out of the image
-              const long nrows = (long)B * H;
-              if (Cc == 384 && H == 16) VSB_DWC(384, 16, true, 1, nrows);
-              else if (Cc == 768 && H == 8) VSB_DWC(768, 8, true, 1, nrows);
-              else if (Cc == 96) VSB_DWC(96, 8, false, spb, nstrips);
-              else if (Cc == 192) VSB_DWC(192, 8, false, spb, nstrips);
-              else if (Cc == 384) VSB_DWC(384, 8, false, spb, nstrips);
-              else VSB_DWC(768, 8, false, spb, nstrips);
-            }
-#undef VSB_DWC
-            VSB_CUDA(cudaGetLastError());
-          }, 1, "cnx.dwconv7_ln." + std::to_string(C) + "@" + std::to_string(hs)});
+          const DwConvOp op = setup_dwconv(x, B, hs, C, Cp, w.dww, w.dwb, w.lnw, w.lnb, a);
+          pl.steps.push_back(Step{[op](cudaStream_t st) { launch_dwconv(op, st); }, 1, "cnx.dwconv7_ln." + std::to_string(C) + "@" + std::to_string(hs)});
         }
         {
           ConvGemmOp op; setup_tma_gemm(op, a, M, C, Cp);
@@ -1196,32 +882,15 @@ class Model {
           add_conv(pl, op, w.pw1, "cnx.pwconv1." + std::to_string(C) + "@" + std::to_string(hs));
         }
         {
-          const int K4 = 4 * C;
-          float* gamma = w.gamma;
+          const int K4 = 4 * C, Cc = C, part_rows = all_part ? rows_per_sample / 32 : 0, nsm = num_sms;
+          const float* gamma = w.gamma;
           float* stats = all_part ? part_buf : stats_pp[(blk_counter - 1) & 1];
           float* stats_next = all_part ? nullptr : stats_pp[blk_counter & 1];
-          const int part_rows = all_part ? rows_per_sample / 32 : 0;
-          if (wscale) {
-            // GRN multiplier folded into per-sample copies of W2 (pointwise.cuh K2e): no pass over g at all
-            const __half* w2 = w.pw2.w;
-            __half* w2s_ = w2s;
-            const int Nn = C;
-            pl.steps.push_back(Step{[=](cudaStream_t st) {
-              static bool attr = false;
-              if (!attr) { VSB_CUDA(cudaFuncSetAttribute(grn_scale_weights_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr = true; }
-              grn_scale_weights_kernel<<<dim3(B, 4), 256, 2 * K4 * sizeof(float), st>>>(stats, stats_next, gamma, w2, w2s_, Nn, K4, part_rows);
-              VSB_CUDA(cudaGetLastError());
-            }, 1, "cnx.grn_wscale." + std::to_string(C) + "@" + std::to_string(hs)});
-          } else {
+          // GRN multiplier folded into per-sample copies of W2 (pointwise.cuh K2e: no pass over g at all), or applied to g in place
+          const __half* w2 = w.pw2.w;
           pl.steps.push_back(Step{[=](cudaStream_t st) {
-            // enough row-slabs per sample to fill the GPU (~8 blocks per SM)
-            static bool attr = false;
-            if (!attr) { VSB_CUDA(cudaFuncSetAttribute(grn_apply_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr = true; }
-            int slabs = std::max(1, std::min(rows_per_sample, (num_sms * 8 + B - 1) / B));
-            grn_apply_kernel<<<B * slabs, 256, 2 * K4 * sizeof(float), st>>>(g, rows_per_sample, K4, K4, stats, stats_next, gamma, slabs, part_rows);
-            VSB_CUDA(cudaGetLastError());
-          }, 1, "cnx.grn_apply." + std::to_string(C) + "@" + std::to_string(hs)});
-          }
+            launch_grn(stats, stats_next, gamma, K4, part_rows, B, w2, w2s, Cc, g, rows_per_sample, nsm, st);
+          }, 1, (wscale ? "cnx.grn_wscale." : "cnx.grn_apply.") + std::to_string(C) + "@" + std::to_string(hs)});
         }
         {
           ConvGemmOp op; setup_tma_gemm(op, g, M, 4 * C, 4 * C);
@@ -1229,11 +898,8 @@ class Model {
           op.p.out32 = x; op.p.ld_out32 = Cp;  // in place: each element is read and written by the same thread
           if (wscale) { op.w_samples = B; op.p.rows_per_sample = rows_per_sample; }
           if (s == 3 && jb == d.ext_depths[s] - 1) {
-            x16 = pl.pool.alloc_n<__half>(M * Cp);
-            if (Cp != C) {   // the head conv's gather reads the pad channels
-              VSB_CUDA(cudaMemset(x16, 0, (size_t)M * Cp * sizeof(__half)));
-              VSB_CUDA(cudaDeviceSynchronize());
-            }
+            // the head conv's gather reads the pad channels
+            x16 = Cp != C ? pl.pool.alloc_zeroed<__half>(M * Cp) : pl.pool.alloc_n<__half>(M * Cp);
             op.p.out16 = x16; op.p.ld_out16 = Cp;
           }
           add_conv(pl, op, w.pw2, "cnx.pwconv2." + std::to_string(C) + "@" + std::to_string(hs), 0, wscale ? w2s : nullptr);
@@ -1255,22 +921,11 @@ class Model {
       dbg(pl, "head_conv", y, 0, B, hs, hs, C, Cp);
       float* pooled = pl.pool.alloc_n<float>((size_t)B * C);
       const int P = hs * hs, Cc = C, ldy = Cp, NO = 1 + d.nbits;
-      float *lw = head_lnw, *lb = head_lnb, *hw = head_lw, *hb = head_lb;
+      const float *lw = head_lnw, *lb = head_lnb, *hw = head_lw, *hb = head_lb;
       float* logits = pl.logits;
-      pl.steps.push_back(Step{[=](cudaStream_t st) {
-        static bool attr = false;
-        if (!attr) { VSB_CUDA(cudaFuncSetAttribute(head_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); attr = true; }
-        head_pool_kernel<<<B, 256, (size_t)8 * Cc * sizeof(float), st>>>(y, P, Cc, ldy, lw, lb, pooled);
-        const int grid = (int)(((long)B * NO + 7) / 8);
-        head_linear_kernel<<<grid, 256, 0, st>>>(pooled, hw, hb, B, Cc, NO, logits);
-        VSB_CUDA(cudaGetLastError());
-      }, 2, "cnx.head_tail"});
+      pl.steps.push_back(Step{[=](cudaStream_t st) { launch_head(y, B, P, Cc, ldy, lw, lb, pooled, hw, hb, NO, logits, st); }, 2,
+                              "cnx.head_tail"});
     }
-    Plan* ret = up.get();
-    ret->last_use = ++plan_clock;
-    detect_plans[B] = std::move(up);
-    evict_plans(detect_plans, ret);
-    return ret;
   }
 
   // Pixel-wise decoder stages.  Each stage is one tensor-core GEMM at the LOW resolution, Y[p, tap*C_out + co] (the tap trick of the
@@ -1290,29 +945,26 @@ class Model {
       ConvGemmOp op; setup_tma_gemm(op, x, Mi, s.kin, ldx);
       op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.out16 = ytap; op.p.ld_out16 = 9 * Co;
       add_conv(pl, op, s.taps, "pd.uptap1x1." + std::to_string(s.cin) + "-" + std::to_string(9 * Co) + "@" + std::to_string(h));
-      const float *lw = s.lnw, *lb = s.lnb;
-      const size_t tsmem = (size_t)(T + 2) * (T + 2) * 9 * Co * sizeof(__half);
+      UpsGather g;
+      g.y = ytap; g.B = B; g.IH = IH; g.C = Co; g.lnw = s.lnw; g.lnb = s.lnb; g.num_sms = nsm; g.optin = kPdMaxSmem;
+      const size_t tsmem = ups_tile_smem(F, Co);
       const std::string tag = std::to_string(Co) + "x" + std::to_string(F) + "@" + std::to_string(ho);
       if (last) {
-        const size_t smem = tsmem + (size_t)NO * (Co + 1) * sizeof(float);
-        if (IH % T != 0 || smem > kPdMaxSmem)
+        g.smem = tsmem + (size_t)NO * (Co + 1) * sizeof(float);
+        if (IH % T != 0 || g.smem > kPdMaxSmem)
           throw Error("pixel-wise head: a " + std::to_string(IH) + "-pixel map with " + std::to_string(NO) + " outputs is not implemented", kErrUnsupported);
-        const float *hw = pd_hw, *hb = pd_hb;
-        pl.steps.push_back(Step{[=](cudaStream_t st) {
-          launch_pd_head(F, Co / 8, smem, ytap, B, IH, Co, lw, lb, hw, hb, NO, plp->out_maps, st);
-        }, 1, "pd.gather_head." + tag});
+        g.hw = pd_hw; g.hb = pd_hb; g.NO = NO;
+        pl.steps.push_back(Step{[g, F, plp](cudaStream_t st) mutable { g.maps = plp->out_maps; launch_pd_gather(g, F, g.C / 8, st); }, 1,
+                                "pd.gather_head." + tag});
       } else {
         const int ldo = pd_gemm_k(Co);
-        __half* u = pl.pool.alloc_n<__half>((long)B * ho * ho * ldo);
-        if (ldo != Co) {   // pad channels stay zero: the gather writes [0, Co)
-          VSB_CUDA(cudaMemset(u, 0, (size_t)B * ho * ho * ldo * sizeof(__half)));
-          VSB_CUDA(cudaDeviceSynchronize());
-        }
-        const bool tiled = IH % T == 0 && tsmem <= kPdMaxSmem;
+        // pad channels stay zero: the gather writes [0, Co)
+        __half* u = ldo != Co ? pl.pool.alloc_zeroed<__half>((size_t)B * ho * ho * ldo) : pl.pool.alloc_n<__half>((size_t)B * ho * ho * ldo);
+        g.out = u; g.ld_out = ldo;
+        g.smem = IH % T == 0 && tsmem <= kPdMaxSmem ? tsmem : 0;
         const int vpt = pd_vpt(Co);
-        pl.steps.push_back(Step{[=](cudaStream_t st) {
-          launch_pd_stage(F, vpt, tiled, tiled ? tsmem : 0, ytap, B, IH, Co, lw, lb, u, ldo, nsm, st);
-        }, 1, std::string(tiled ? "pd.upgather." : "pd.upgather_untiled.") + tag});
+        pl.steps.push_back(Step{[g, F, vpt](cudaStream_t st) { launch_pd_gather(g, F, vpt, st); }, 1,
+                                std::string(g.smem ? "pd.upgather." : "pd.upgather_untiled.") + tag});
         dbg(pl, "pd" + std::to_string(i), u, 1, B, ho, ho, Co, ldo);
         x = u; ldx = ldo;
       }
@@ -1330,44 +982,16 @@ class Model {
     return ret;
   }
 
-  // per-call CUDA-event scope for the launches outside the plans (bench.py roofline leg: vsb_profile_enable)
-  template <class Fn> static void prof_scope(const std::string& name, cudaStream_t st, int launches, Fn&& fn) {
-    if (!g_profile.enabled) { fn(); g_launches += launches; return; }
-    cudaEvent_t a, b;
-    cudaEventCreate(&a); cudaEventCreate(&b);
-    cudaEventRecord(a, st);
-    fn();
-    cudaEventRecord(b, st);
-    g_launches += launches;
-    g_profile.pending.push_back({name, {a, b}});
-  }
-
   // resample `n` frames that are `frame_stride` floats apart to S x S (one launch, also for strided key frames)
   void resize_frames(const float* src, long frame_stride, int n, int H, int W, float* dst, bool aa, cudaStream_t st) {
     const int S = d.img_size;
-    ResampleDev* r = get_resampler(H, W, S, S, aa);
-    // (checked here, not when the table is built: the blend only reads the delta up-sampler's table, whatever its width)
-    if (r->smem > 200 * 1024) throw Error("resize: image too wide for the shared-memory resample kernel (not implemented)", kErrUnsupported);
-    const int vec = (W % 4 == 0) && (reinterpret_cast<uintptr_t>(src) % 16 == 0) && (frame_stride % 4 == 0);
-    if (n > 16384) {   // gridDim.y limit: split very long frame ranges
-      for (int i = 0; i < n; i += 16384)
-        resize_frames(src + (long)i * frame_stride, frame_stride, std::min(16384, n - i), H, W, dst + (size_t)i * 3 * S * S, aa, st);
-      return;
+    const ResampleDev* r = get_resampler(H, W, S, S, aa);
+    for (int i = 0; i < n; i += 16384) {   // gridDim.y limit: split very long frame ranges
+      const int m = std::min(16384, n - i);
+      prof_scope("pw.resize." + std::to_string(H) + "x" + std::to_string(W) + "@" + std::to_string(m), st, 1, [&] {
+        launch_resize(*r, src + (long)i * frame_stride, frame_stride, m, H, W, S, dst + (size_t)i * 3 * S * S, last_resize, st);
+      });
     }
-    const dim3 grid((S + r->toy - 1) / r->toy, n * 3);
-    const int mt = r->tab.maxt_x <= 2 ? 2 : (r->tab.maxt_x <= 8 ? 8 : 0);
-    const int32_t rec[5] = {mt, r->gstage, vec, r->toy, S};
-    std::copy(rec, rec + 5, last_resize);
-    prof_scope("pw.resize." + std::to_string(H) + "x" + std::to_string(W) + "@" + std::to_string(n), st, 1, [&] {
-#define VSB_RS(MT, GS) do { static bool attr_ = false; \
-        if (!attr_) { VSB_CUDA(cudaFuncSetAttribute(resize_sep_kernel<MT, GS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr_ = true; } \
-        resize_sep_kernel<MT, GS><<<grid, 256, r->smem, st>>>(src, frame_stride, dst, H, W, S, S, r->tab, r->toy, r->rin_max, vec); } while (0)
-      if (r->gstage == 4) { if (mt == 2) VSB_RS(2, 4); else if (mt == 8) VSB_RS(8, 4); else VSB_RS(0, 4); }
-      else if (r->gstage == 2) { if (mt == 2) VSB_RS(2, 2); else if (mt == 8) VSB_RS(8, 2); else VSB_RS(0, 2); }
-      else { if (mt == 2) VSB_RS(2, 1); else if (mt == 8) VSB_RS(8, 1); else VSB_RS(0, 1); }
-#undef VSB_RS
-    });
-    VSB_CUDA(cudaGetLastError());
   }
 
   void check_ready() const { if (!finalized) throw Error("model not finalized", kErrState); }
@@ -1375,14 +999,28 @@ class Model {
   // ---- streaming host path: embed + detect of HOST frames with the PCIe copies overlapped with compute
   cudaStream_t s_in = nullptr, s_cmp = nullptr, s_out = nullptr;
   std::vector<cudaEvent_t> ev_in, ev_cmp;
-  void embed_detect_host(const float* imgs_h, const uint8_t* msgs_h, int n_msgs, float* imgs_w_h, float* logits_h, int F, int H, int W,
-                         int step, int video_mode, int chunk_keys, float scaling_i, float scaling_w, int flags) {
-    check_ready();
+  // creates the three streams once and at least n (input, compute) event pairs
+  void stream_setup(size_t n) {
     if (!s_in) {
       VSB_CUDA(cudaStreamCreateWithFlags(&s_in, cudaStreamNonBlocking));
       VSB_CUDA(cudaStreamCreateWithFlags(&s_cmp, cudaStreamNonBlocking));
       VSB_CUDA(cudaStreamCreateWithFlags(&s_out, cudaStreamNonBlocking));
     }
+    while (ev_in.size() < n) {
+      cudaEvent_t a, b;
+      VSB_CUDA(cudaEventCreateWithFlags(&a, cudaEventDisableTiming));
+      VSB_CUDA(cudaEventCreateWithFlags(&b, cudaEventDisableTiming));
+      ev_in.push_back(a); ev_cmp.push_back(b);
+    }
+  }
+  // frames that must stay in one batch: a key frame and its step - 1 followers, or in 'interpolate' mode, where neighbouring keys
+  // of one reference chunk are mixed, whole chunks
+  static int key_unit(int step, int video_mode, int chunk_keys) {
+    return (video_mode == VSB_VIDEO_INTERPOLATE && step > 1) ? step * std::max(1, chunk_keys) : step;
+  }
+  void embed_detect_host(const float* imgs_h, const uint8_t* msgs_h, int n_msgs, float* imgs_w_h, float* logits_h, int F, int H, int W,
+                         int step, int video_mode, int chunk_keys, float scaling_i, float scaling_w, int flags) {
+    check_ready();
     const size_t fpx = (size_t)3 * H * W;
     const int NO = 1 + d.nbits;
     float* imgs = (float*)stage(0, (size_t)F * fpx * sizeof(float));
@@ -1396,7 +1034,7 @@ class Model {
     // Exposed copies: the first slice in and the last group's logits out.
     // Slice sizes: the FIRST slice's copy is the exposed one, so it is shorter than the rest.  Measured at 64 x 3x256x256 (results
     // bit-identical for every setting): first/rest 32/32 7 165 f/s, 24/40 7 207, 16/48 7 317, 8/56 7 310, 16/24 7 020 -> 16 / 48.
-    const int unit = (video_mode == VSB_VIDEO_INTERPOLATE && step > 1) ? step * std::max(1, chunk_keys) : step;
+    const int unit = key_unit(step, video_mode, chunk_keys);
     const int sl0 = (16 + unit - 1) / unit * unit, sl1 = (48 + unit - 1) / unit * unit;
     std::vector<std::pair<int, int>> slices;   // (first frame, frames)
     for (int f0 = 0; f0 < F;) {
@@ -1405,12 +1043,7 @@ class Model {
       f0 += n;
     }
     const int nsl = (int)slices.size();
-    while ((int)ev_in.size() < nsl + 1) {
-      cudaEvent_t a, b;
-      VSB_CUDA(cudaEventCreateWithFlags(&a, cudaEventDisableTiming));
-      VSB_CUDA(cudaEventCreateWithFlags(&b, cudaEventDisableTiming));
-      ev_in.push_back(a); ev_cmp.push_back(b);
-    }
+    stream_setup(nsl + 1);
     VSB_CUDA(cudaMemcpyAsync(msgs, msgs_h, (size_t)n_msgs * d.nbits, cudaMemcpyHostToDevice, s_in));
     for (int k = 0; k < nsl; ++k) {       // all input copies are queued up front: s_in runs ahead of the compute
       const int f0 = slices[k].first, n = slices[k].second;
@@ -1445,11 +1078,6 @@ class Model {
   void frames_host_u8(const uint8_t* in_h, const uint8_t* msgs_h, int n_msgs, uint8_t* out_h, float* logits_h, int F, int H, int W,
                       int step, int video_mode, int chunk_keys, float scaling_i, float scaling_w, int flags) {
     check_ready();
-    if (!s_in) {
-      VSB_CUDA(cudaStreamCreateWithFlags(&s_in, cudaStreamNonBlocking));
-      VSB_CUDA(cudaStreamCreateWithFlags(&s_cmp, cudaStreamNonBlocking));
-      VSB_CUDA(cudaStreamCreateWithFlags(&s_out, cudaStreamNonBlocking));
-    }
     const bool do_embed = out_h != nullptr, do_detect = logits_h != nullptr;
     VSB_CHECK(do_embed || do_detect, "nothing to do");
     const size_t fpx = (size_t)3 * H * W;
@@ -1462,15 +1090,10 @@ class Model {
     uint8_t* in8 = (uint8_t*)stage(4, (size_t)F * fpx);
     uint8_t* out8 = do_embed ? (uint8_t*)stage(5, (size_t)F * fpx) : nullptr;
     int ch = kMaxBatch;   // one-byte samples: the exposed first/last copies are short, so full 64-frame batches win
-    const int unit = (video_mode == VSB_VIDEO_INTERPOLATE && step > 1) ? step * std::max(1, chunk_keys) : step;
+    const int unit = key_unit(step, video_mode, chunk_keys);
     if (ch % unit) ch = ((ch + unit - 1) / unit) * unit;
     const int nch = (F + ch - 1) / ch;
-    while ((int)ev_in.size() < nch) {
-      cudaEvent_t a, b;
-      VSB_CUDA(cudaEventCreateWithFlags(&a, cudaEventDisableTiming));
-      VSB_CUDA(cudaEventCreateWithFlags(&b, cudaEventDisableTiming));
-      ev_in.push_back(a); ev_cmp.push_back(b);
-    }
+    stream_setup(nch);
     if (do_embed) VSB_CUDA(cudaMemcpyAsync(msgs, msgs_h, (size_t)n_msgs * d.nbits, cudaMemcpyHostToDevice, s_in));
     for (int k = 0; k < nch; ++k) {
       const int f0 = k * ch, n = std::min(ch, F - f0);
@@ -1478,16 +1101,15 @@ class Model {
       VSB_CUDA(cudaEventRecord(ev_in[k], s_in));
       VSB_CUDA(cudaStreamWaitEvent(s_cmp, ev_in[k], 0));
       const long npx = (long)n * plane;
-      const unsigned blocks = (unsigned)std::min<long>((npx + 255) / 256, (long)num_sms * 16);
-      u8hwc_to_f32chw_kernel<<<blocks, 256, 0, s_cmp>>>(in8 + (size_t)f0 * fpx, imgs + (size_t)f0 * fpx, npx, plane);
+      launch_u8_to_f32(in8 + (size_t)f0 * fpx, imgs + (size_t)f0 * fpx, npx, plane, num_sms, s_cmp);
       g_launches += 1;
       const float* det_in = imgs + (size_t)f0 * fpx;
       if (do_embed) {
         const uint8_t* mk = msgs + (n_msgs == 1 ? 0 : (size_t)f0 * d.nbits);
         embed(imgs + (size_t)f0 * fpx, mk, n_msgs == 1 ? 1 : n, out + (size_t)f0 * fpx, nullptr, n, H, W, step, video_mode, chunk_keys,
               scaling_i, scaling_w, flags, s_cmp);
-        f32chw_to_u8hwc_kernel<<<blocks, 256, 0, s_cmp>>>(out + (size_t)f0 * fpx, out8 + (size_t)f0 * fpx,
-                                                          do_detect ? out + (size_t)f0 * fpx : nullptr, npx, plane);
+        launch_f32_to_u8(out + (size_t)f0 * fpx, out8 + (size_t)f0 * fpx, do_detect ? out + (size_t)f0 * fpx : nullptr, npx, plane, num_sms,
+                         s_cmp);
         g_launches += 1;
         det_in = out + (size_t)f0 * fpx;
       }
@@ -1589,82 +1211,24 @@ class Model {
         // per-frame attenuated delta at processing size: out[f] = hmap(frames_res[f]) * delta(keys of f); then a plain blend
         float* lowres_buf = (float*)stage(7, (size_t)nf * PC * S * S * sizeof(float));
         VSB_CHECK(nf <= 65535, "too many frames per key-frame batch");
-        dim3 grid((S + kBlendTW - 1) / kBlendTW, (S + kBlendTH - 1) / kBlendTH, nf);
-        const int CD = d.unet_out_ch;
-        prof_scope("pw.jnd_lowres@" + std::to_string(nf), st, 1,
-                   [&] { jnd_lowres_kernel<<<grid, 256, 0, st>>>(frames_res, delta, lowres_buf, S, S, CD, step, balt, bint, bp.jnd_in, bp.jnd_out); });
-        VSB_CUDA(cudaGetLastError());
+        prof_scope("pw.jnd_lowres@" + std::to_string(nf), st, 1, [&] {
+          launch_jnd_lowres(frames_res, delta, lowres_buf, nf, S, S, d.unet_out_ch, step, balt, bint, bp.jnd_in, bp.jnd_out, st);
+        });
         bp.delta = lowres_buf; bp.step = 1; bp.alternate = 0; bp.interp_chunk = 0; bp.use_jnd = 0; bp.CD = PC;
       } else {
         bp.delta = delta; bp.step = step; bp.alternate = balt; bp.interp_chunk = bint; bp.use_jnd = use_jnd ? 1 : 0;
       }
-      launch_blend(bp, st);
+      prof_scope(std::string(bp.use_jnd ? "pw.jnd_blend." : "pw.blend.") + std::to_string(bp.H) + "x" + std::to_string(bp.W) + "@" +
+                     std::to_string(bp.F) + (bp.preds_w ? "+preds" : ""), st, 1, [&] { launch_blend(bp, last_blend, st); });
     }
-  }
-
-  void launch_blend(const BlendParams& bp, cudaStream_t st) {
-    VSB_CHECK(bp.F <= 65535, "too many frames per blend launch");
-    dim3 grid((bp.W + kB2TW - 1) / kB2TW, (bp.H + kB2TH - 1) / kB2TH, bp.F);
-    const bool vec = (bp.W % 4 == 0) && ((reinterpret_cast<uintptr_t>(bp.imgs) | reinterpret_cast<uintptr_t>(bp.imgs_w) |
-                                          reinterpret_cast<uintptr_t>(bp.preds_w)) % 16 == 0);
-    // delta read in place, or through <= 2 taps per axis (plain bilinear up-scale: every input at least as large as the processing size)
-    const bool fastup = bp.identity_resample || (bp.tab.maxt_x <= 2 && bp.tab.maxt_y <= 2 && bp.H >= bp.PH && bp.W >= bp.PW);
-    VSB_CHECK(bp.CD == 1 || bp.CD == 3, "delta must have 1 or 3 channels");
-    // TMA-fed kernel (jnd_blend3_kernel): vector layout, delta in place or <= 2 taps per axis; the delta tile needs a TMA-legal row pitch
-    const bool delta_tma = bp.identity_resample || (bp.PW % 4 == 0 && reinterpret_cast<uintptr_t>(bp.delta) % 16 == 0);
-    // (boxes never exceed the tensor they are cut from: tiny frames / processing sizes take the load-then-compute kernel)
-    const bool tma = vec && fastup && delta_tma && bp.W >= kB2LP && bp.H >= kB2TH + 4 &&
-                     (bp.identity_resample || (bp.PW >= kB3DW && bp.PH >= kB2DH)) &&
-                     (!bp.identity_resample || (bp.PW % 4 == 0 && reinterpret_cast<uintptr_t>(bp.delta) % 16 == 0));
-    CUtensorMap tmI, tmD;
-    if (tma) {
-      const uint64_t idims[3] = {(uint64_t)bp.W, (uint64_t)bp.H, (uint64_t)bp.F * 3};
-      const uint64_t istr[2] = {(uint64_t)bp.W * 4, (uint64_t)bp.H * bp.W * 4};
-      const uint32_t ibox[3] = {(uint32_t)kB2LP, (uint32_t)(kB2TH + 4), 3};
-      encode_map(&tmI, bp.imgs, 3, idims, istr, ibox, 0, true, /*f32=*/true);
-      tmD = tmI;
-      if (!bp.identity_resample) {
-        const int nkeys = (bp.F + bp.step - 1) / bp.step;
-        const uint64_t ddims[3] = {(uint64_t)bp.PW, (uint64_t)bp.PH, (uint64_t)nkeys * bp.CD};
-        const uint64_t dstr[2] = {(uint64_t)bp.PW * 4, (uint64_t)bp.PH * bp.PW * 4};
-        const uint32_t dbox[3] = {(uint32_t)kB3DW, (uint32_t)kB2DH, 1};
-        encode_map(&tmD, bp.delta, 3, ddims, dstr, dbox, 0, true, /*f32=*/true);
-      }
-    }
-    const int32_t rec[5] = {tma ? 3 : 2, vec ? 4 : 1, fastup ? 1 : 0, bp.CD, (bp.use_jnd && bp.jnd_in == 3) ? 3 : 1};
-    std::copy(rec, rec + 5, last_blend);
-    prof_scope(std::string(bp.use_jnd ? "pw.jnd_blend." : "pw.blend.") + std::to_string(bp.H) + "x" + std::to_string(bp.W) + "@" + std::to_string(bp.F) +
-                   (bp.preds_w ? "+preds" : ""), st, 1, [&] {
-#define VSB_BL(V, FU, CDV, JI) do { static bool attr_ = false; \
-        if (!attr_) { VSB_CUDA(cudaFuncSetAttribute(jnd_blend2_kernel<V, FU, CDV, JI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b2_smem(JI))); attr_ = true; } \
-        jnd_blend2_kernel<V, FU, CDV, JI><<<grid, 256, b2_smem(JI), st>>>(bp); } while (0)
-#define VSB_BL2(CDV, JI) do { \
-        if (vec) { if (fastup) VSB_BL(4, 1, CDV, JI); else VSB_BL(4, 0, CDV, JI); } else { if (fastup) VSB_BL(1, 1, CDV, JI); else VSB_BL(1, 0, CDV, JI); } } while (0)
-#define VSB_BL3(CDV, JI) do { static bool attr_ = false; \
-        if (!attr_) { VSB_CUDA(cudaFuncSetAttribute(jnd_blend3_kernel<CDV, JI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b3_smem(JI))); attr_ = true; } \
-        jnd_blend3_kernel<CDV, JI><<<grid3, 256, b3_smem(JI), st>>>(bp, tmI, tmD); } while (0)
-      const dim3 grid3(grid.x, (bp.H + kB2TH * kB3NT - 1) / (kB2TH * kB3NT), bp.F);
-      const bool j3 = bp.use_jnd && bp.jnd_in == 3;      // one heat-map per RGB channel (jnd_3_1 / jnd_3_3): rarely used, own instantiation
-      if (tma) {
-        if (bp.CD == 1) { if (j3) VSB_BL3(1, 3); else VSB_BL3(1, 1); }
-        else            { if (j3) VSB_BL3(3, 3); else VSB_BL3(3, 1); }
-      } else if (bp.CD == 1) { if (j3) VSB_BL2(1, 3); else VSB_BL2(1, 1); }
-      else                   { if (j3) VSB_BL2(3, 3); else VSB_BL2(3, 1); }
-#undef VSB_BL3
-#undef VSB_BL2
-#undef VSB_BL
-    });
-    VSB_CUDA(cudaGetLastError());
   }
 
   void jnd_heatmaps(const float* imgs, float* hmaps, int F, int H, int W, cudaStream_t st) {
     // heat-map only (operator seam, modules/jnd.py:80-108): jnd_lowres_kernel with delta == nullptr writes hmap * 1; hmaps [F, jnd_out, H, W]
     VSB_CHECK(F <= 65535, "too many frames");
     VSB_CHECK(d.jnd_in_ch != 0, "the card has no JND attenuation");
-    dim3 grid((W + kBlendTW - 1) / kBlendTW, (H + kBlendTH - 1) / kBlendTH, F);
-    jnd_lowres_kernel<<<grid, 256, 0, st>>>(imgs, nullptr, hmaps, H, W, 1, 1, 0, 0, d.jnd_in_ch, d.jnd_out_ch);
+    launch_jnd_lowres(imgs, nullptr, hmaps, F, H, W, 1, 1, 0, 0, d.jnd_in_ch, d.jnd_out_ch, st);
     g_launches += 1;
-    VSB_CUDA(cudaGetLastError());
   }
 
   void detect(const float* imgs, float* logits, int F, int H, int W, int flags, cudaStream_t st) {

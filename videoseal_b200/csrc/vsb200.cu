@@ -21,15 +21,17 @@ static_assert((int)kErrInvalid == (int)VSB_ERR_INVALID && (int)kErrUnsupported =
               "status codes of include/vsb200.h");
 
 // Every C entry point that touches the GPU runs on the model's device and restores the caller's current device afterwards (the
-// library must not change process-wide state under PyTorch), and holds the model's mutex: plans, scratch buffers, staging areas
-// and the launch / profile counters belong to the handle, so calls on ONE handle are serialised (use one handle per thread or
-// stream for concurrency; include/vsb200.h "Threading").
+// library must not change process-wide state under PyTorch), and holds the model's mutex: plans, scratch buffers and staging
+// areas belong to the handle, so calls on ONE handle are serialised (use one handle per thread or stream for concurrency;
+// include/vsb200.h "Threading").  The launch and profile counters (g_launches, g_profile) are process-wide, as the handle-less
+// vsb_launch_count and vsb_profile_* entry points need.  The guard also records the device for smem_optin (t_device).
 struct DeviceGuard {
-  int prev = -1;
+  int prev = -1, prev_t = t_device;
   explicit DeviceGuard(int dev) {
     if (dev >= 0 && cudaGetDevice(&prev) == cudaSuccess && prev != dev) { VSB_CUDA(cudaSetDevice(dev)); } else { prev = -1; }
+    if (dev >= 0) t_device = dev;
   }
-  ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
+  ~DeviceGuard() { t_device = prev_t; if (prev >= 0) cudaSetDevice(prev); }
 };
 #define VSB_MODEL_SCOPE(m) std::lock_guard<std::recursive_mutex> _lk((m)->impl.mu); DeviceGuard _dg((m)->impl.device)
 
@@ -275,9 +277,7 @@ int vsb_debug_conv(const vsb_conv_test* t, void* stream) {
       VSB_CUDA(cudaMemcpy(hw.data(), t->weights, hw.size() * sizeof(__half), cudaMemcpyDeviceToHost));
       std::vector<float> w(hw.size());
       for (size_t i = 0; i < hw.size(); ++i) w[i] = __half2float(hw[i]);
-      const std::vector<float> v = s2 ? s2d_weights(w, t->N, t->C0) : direct8_weights(w, t->N, t->R);
-      std::vector<__half> vh(v.size());
-      for (size_t i = 0; i < v.size(); ++i) vh[i] = __float2half_rn(v[i]);
+      const std::vector<__half> vh = Model::to_half(s2 ? s2d_weights(w, t->N, t->C0) : direct8_weights(w, t->N, t->R));
       VSB_CUDA(cudaMemcpy(wtmp, vh.data(), vh.size() * sizeof(__half), cudaMemcpyHostToDevice));
       pack_direct_weights(wtmp, t->N, s2 ? 4 * t->C0 : 16, wpk, (cudaStream_t)stream, s2 ? 9 : t->R * ((t->R + 1) / 2));
     } else {
