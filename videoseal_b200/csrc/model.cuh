@@ -620,6 +620,8 @@ class Model {
     add_unet_conv(pl, w.res, 1, x, B, H, W, Cin, ldx, false, nullptr, r, Cout);
     add_unet_conv(pl, w.c1, 3, x, B, H, W, Cin, ldx, true, nullptr, h, Cout);
     add_unet_conv(pl, w.c2, 3, h, B, H, W, Cout, Cout, true, r, out, ld_out, fuse_outc);
+    dbg(pl, name + ".h", h, 1, B, H, W, Cout, Cout);
+    dbg(pl, name + ".r", r, 1, B, H, W, Cout, Cout);
     if (out) dbg(pl, name, out, 1, B, H, W, Cout, ld_out);
     return out;
   }
@@ -667,6 +669,8 @@ class Model {
       pl.steps.push_back(Step{[=](cudaStream_t st) { launch_unet_first(plp->in_imgs, B, S, Z, cin, w1, b1, wr, br, h1, r0, yuv, st); }, 1,
                               "unet.first"});
     }
+    dbg(pl, "first_h", h1, 1, B, S, S, z[0], z[0]);
+    dbg(pl, "first_r", r0, 1, B, S, S, z[0], z[0]);
     std::vector<__half*> skips;  // outputs of inc, downs[0..]
     std::vector<int> skip_ld;
     __half* x = pl.pool.alloc_n<__half>(M0 * z[0]);
@@ -693,6 +697,7 @@ class Model {
         op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.bias = down_conv[i].bias; op.p.out16 = dn; op.p.ld_out16 = z[i + 1];
         add_conv(pl, op, down_conv[i], "unet.down3x3s2." + std::to_string(z[i]) + "-" + std::to_string(z[i + 1]) + "@" + std::to_string(ho));
       }
+      dbg(pl, "down" + std::to_string(i) + "_conv", dn, 1, B, ho, ho, z[i + 1], z[i + 1]);
       __half* out = nullptr; int ld_out = 0;
       if (i == L - 2) {  // last level writes straight into the message-concat buffer (channels [0, z))
         cat = pl.pool.alloc_n<__half>(Mo * zb);
@@ -751,6 +756,7 @@ class Model {
           setup_tma_gemm2(op, x, Cin, ldx, skip, Cin, ld_skip, Mi);
         op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.out16 = ytap; op.p.ld_out16 = 9 * Cout;
         add_conv(pl, op, up_conv[j], "unet.uptap1x1." + std::to_string(2 * Cin) + "-" + std::to_string(9 * Cout) + "@" + std::to_string(hs));
+        dbg(pl, "up" + std::to_string(j) + "_taps", ytap, 1, B, hs, hs, 9 * Cout, 9 * Cout);
         // then bilinear x2 + reflect pad + 3x3 tap sum + LayerNorm + ReLU (CUDA cores, memory-bound)
         const int vpt = Cout <= 256 ? 1 : 2;            // 16-byte channel vectors per thread (chunkyseal's first up-conv: 512 channels)
         const int gthreads = Cout / (8 * vpt);          // threads per output pixel
