@@ -57,8 +57,8 @@ typedef struct vsb_model_desc {
   int32_t unet_levels;       /* len(z_channels_mults), <= 6 */
   int32_t unet_z[6];         /* z_channels * mult */
   int32_t unet_num_blocks;
-  int32_t unet_act;          /* 0 relu (the only value the GPU path implements; 1 = silu is rejected by vsb_model_finalize) */
-  int32_t unet_norm;         /* 0 batch (the only value the GPU path implements; 1 = rms is rejected by vsb_model_finalize) */
+  int32_t unet_act;          /* 0 relu (the only value the GPU path implements; 1 = silu is rejected by vsb_model_create) */
+  int32_t unet_norm;         /* 0 batch (the only value the GPU path implements; 1 = rms is rejected by vsb_model_create) */
   int32_t unet_last_tanh;
   int32_t ext_depths[4];
   int32_t ext_dims[4];       /* after proportional_dim scaling, extractor.py:193-198 */
@@ -69,6 +69,11 @@ typedef struct vsb_model_desc {
 const char* vsb_last_error(void);
 int vsb_version(void);
 
+/* Checks every rule on the descriptor and chooses each U-Net layer's kernel, with no CUDA call (a load-time dry run needs no GPU).
+ * VSB_ERR_UNSUPPORTED unless: BatchNorm+ReLU; U-Net widths 16, 32, multiples of 64, or 8 in leading levels but not the last; up
+ * blocks of 8 * 2^k <= 512 channels; img_size >> (levels - 1) >= 16; img_size <= 768 with 8 channels, whose layers must fit their
+ * rings; JND channels 1 or 3.  VSB_ERR_INVALID unless: 2..6 levels, unet_in_ch 1 (yuv) or 3, unet_out_ch 1..3, img_size a multiple
+ * of 128, hidden a multiple of 8, ConvNeXt widths even and not shrinking. */
 int vsb_model_create(const vsb_model_desc* desc, vsb_model** out);
 /* one state_dict entry, fp32, host memory, contiguous; `name` is the reference state_dict key */
 int vsb_model_set_tensor(vsb_model* m, const char* name, const float* data, const int64_t* shape, int32_t ndim);
@@ -76,7 +81,11 @@ int vsb_model_set_tensor(vsb_model* m, const char* name, const float* data, cons
  * this call the model has the pooled head (one [1+nbits] logit vector per frame).  pixelwise = 1 needs 1..8 stage factors, each 2
  * or 4, and a ConvNeXt trunk with ext_stem_stride 4; stage i maps C -> C / factors[i] channels (bilinear up-sampling, reflect-padded
  * 3x3 conv, LayerNorm, GELU), then a 1x1 conv gives 1+nbits maps.  pixelwise = 0 accepts only n_stages = 1, factors = {1} (the
- * pooled head).  VSB_ERR_STATE after finalize; VSB_ERR_INVALID / VSB_ERR_UNSUPPORTED for other values. */
+ * pooled head).  Like vsb_model_create it makes no CUDA call, and it returns VSB_ERR_UNSUPPORTED unless: the trunk width
+ * ext_dims[3] is 16, 32 or >= 64; every stage width C / f is a whole multiple of 8, of the form 8 * {1, 3} * 2^k (k <= 5) for a
+ * middle stage and at most 32 for the last; the last stage's input map is a multiple of 16 / f pixels, and its staged taps,
+ * (16 / f + 2)^2 * 9 * C fp16, plus its head weights, (1 + nbits) * (C + 1) fp32, fit in 227 KB.  VSB_ERR_STATE after finalize;
+ * VSB_ERR_INVALID / VSB_ERR_UNSUPPORTED for other values. */
 int vsb_model_set_pixel_decoder(vsb_model* m, int32_t n_stages, const int32_t* factors, int32_t pixelwise);
 /* fold BN, pack to fp16 KRSC, upload to `device`, build nothing else (plans are built lazily per batch shape) */
 int vsb_model_finalize(vsb_model* m, int32_t device);

@@ -28,7 +28,7 @@ def test_desc_struct_layout_matches_header():
 
 
 @pytest.mark.parametrize("card", ["videoseal_1.0", "pixelseal", "chunkyseal"])
-def test_card_parsing_matches_oracle_spec(card):
+def test_card_parsing_matches_oracle_spec(built_lib, card):
     from tests.util import load_card
     from oracle import restate
     from videoseal_b200 import cfg

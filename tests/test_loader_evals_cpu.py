@@ -30,7 +30,7 @@ def _training_ckpt(card_name, emb_model, ext_model, as_namespace=False):
 @pytest.mark.parametrize("card_name,emb,ext", [("videoseal_1.0", "unet_small2_yuv_quant", "convnext_tiny"),
                                                ("pixelseal", "unet_base_yuv_quant", "convnext_tiny"),
                                                ("chunkyseal", "unet_sweep_3", "convnext_sweep_3_prop_stride2")])
-def test_training_checkpoint_resolves_to_the_cards_architecture(card_name, emb, ext):
+def test_training_checkpoint_resolves_to_the_cards_architecture(built_lib, card_name, emb, ext):
     path, card = _training_ckpt(card_name, emb, ext)
     got = vcfg.spec_from_card(vcfg.get_config_from_checkpoint(path))
     want = vcfg.spec_from_card(card)
@@ -39,7 +39,7 @@ def test_training_checkpoint_resolves_to_the_cards_architecture(card_name, emb, 
     assert model.spec == want and "embedder.unet.outc.bias" in model.state_dict()
 
 
-def test_training_checkpoint_args_as_namespace_and_card_name_passthrough():
+def test_training_checkpoint_args_as_namespace_and_card_name_passthrough(built_lib):
     path, card = _training_ckpt("videoseal_1.0", "unet_small2_yuv_quant", "convnext_tiny", as_namespace=True)
     assert vcfg.spec_from_card(vcfg.get_config_from_checkpoint(path)) == vcfg.spec_from_card(card)
     with pytest.raises(NotImplementedError):
@@ -277,7 +277,7 @@ def test_embed_stream_surfaces_a_dead_writer_instead_of_deadlocking():
     assert isinstance(done.get("err"), BrokenPipeError)
 
 
-def test_baked_in_attributes_are_live_properties():
+def test_baked_in_attributes_are_live_properties(built_lib):
     """ADVICE round 1 (low): img_size / embedder.yuv / attenuation are baked into the native handle; assigning them must
     rebuild it (or raise), never be a silent no-op (wam.py:147-149,196 mutate them freely in the reference)"""
     import videoseal_b200

@@ -46,7 +46,7 @@ def test_oracle_reproduces_reference_fixture(preset):
 
 @pytest.mark.parametrize("preset,dims,widths", [("convnext_tiny_pw", [96, 192, 384, 768], [768, 192, 48, 24]),
                                                 ("convnext_base_pw", [128, 256, 512, 1024], [1024, 256, 64, 32])])
-def test_training_checkpoint_naming_preset_resolves(tmp_path, preset, dims, widths):
+def test_training_checkpoint_naming_preset_resolves(built_lib, tmp_path, preset, dims, widths):
     from videoseal_b200 import cfg
     card = load_card("videoseal_1.0")
     args = argparse.Namespace(**card["args"], embedder_model="unet_small2_yuv_quant", extractor_model=preset)
@@ -85,13 +85,13 @@ def _pd_card(**pd):
     {"upscale_stages": [2, 2, 2]},                       # last stage 96 channels: more than 32
     {"upscale_stages": [4, 4, 4, 2]},                    # 768 -> 192 -> 48 -> 12: not a multiple of 8
 ])
-def test_rejected_pixel_decoders_raise_at_load(change):
+def test_rejected_pixel_decoders_raise_at_load(built_lib, change):
     from videoseal_b200 import cfg
     with pytest.raises(NotImplementedError):
         cfg.spec_from_card(_pd_card(**change))
 
 
-def test_pixel_decoder_width_and_size_rules_at_load():
+def test_pixel_decoder_width_and_size_rules_at_load(built_lib):
     from videoseal_b200 import cfg
     card = _pd_card(upscale_type="bilinear")
     assert cfg.spec_from_card(card)["pixel_decoder"]["upscale_stages"] == [4, 4, 2]
@@ -120,18 +120,21 @@ def test_pixelwise_on_chunkyseal_trunk_raises_at_load():
         cfg.spec_from_card(card)
 
 
-def test_existing_cards_keep_pooled_decoder():
+def test_existing_cards_keep_pooled_decoder(built_lib):
     from videoseal_b200 import cfg
     for name in ("videoseal_1.0", "pixelseal", "chunkyseal"):
         assert cfg.spec_from_card(load_card(name))["pixel_decoder"] == {"pixelwise": False, "upscale_stages": [1]}
 
 
-def test_set_pixel_decoder_error_codes(built_lib):
-    from videoseal_b200 import _lib
+def test_set_pixel_decoder_error_codes_on_a_valid_descriptor(built_lib):
+    from videoseal_b200 import _lib, cfg
+    from videoseal_b200.model import native_desc
     L = _lib.lib()
-    d = _lib.ModelDesc()
-    d.nbits, d.img_size, d.ext_stem_stride = 256, 256, 4
     h = C.c_void_p()
+    z = _lib.ModelDesc()                          # a mostly zero descriptor (no U-Net levels, no trunk) is no model
+    z.nbits, z.img_size, z.ext_stem_stride = 256, 256, 4
+    assert L.vsb_model_create(C.byref(z), C.byref(h)) == -1 and h.value is None
+    d = native_desc(cfg.spec_from_card(load_card("videoseal_1.0")))   # 256 bits, S = 256, a 768-wide trunk with stem stride 4
     assert L.vsb_model_create(C.byref(d), C.byref(h)) == 0
 
     def call(factors, pixelwise, n=None):

@@ -14,7 +14,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = torch.load(os.path.join(ROOT, "tests", "golden", "unet_tiny.pt"), weights_only=False)
 
 
-def test_training_checkpoint_naming_the_preset_resolves():
+def test_training_checkpoint_naming_the_preset_resolves(built_lib):
     card = ut.tiny_card()
     spec = restate.spec_from_card(card)
     path = ut.training_checkpoint(card, restate.synth_state_dict(spec, ut.SEED), "cpu_resolve")
@@ -43,7 +43,7 @@ def test_oracle_matches_reference_fixture(case):
 
 @pytest.mark.parametrize("mults,what", [([1, 1, 3, 4, 8], "width 24"), ([1, 2, 4, 8, 1], "width 8"), ([2, 1, 2, 4, 8], "width 8"),
                                         ([1, 1, 1, 1, 1], "width 8")])
-def test_unimplemented_widths_are_rejected_at_load(mults, what):
+def test_unimplemented_widths_are_rejected_at_load(built_lib, mults, what):
     card = ut.tiny_card()
     card["embedder"]["params"]["unet"]["z_channels_mults"] = mults
     with pytest.raises(NotImplementedError, match=what):
@@ -51,12 +51,12 @@ def test_unimplemented_widths_are_rejected_at_load(mults, what):
 
 
 @pytest.mark.parametrize("size", [128, 896, 1024])
-def test_unimplemented_processing_sizes_are_rejected_at_load(size):
+def test_unimplemented_processing_sizes_are_rejected_at_load(built_lib, size):
     with pytest.raises(NotImplementedError, match=f"img_size={size}"):
         cfg.spec_from_card(ut.tiny_card(img_size=size))
 
 
-def test_img_size_setter_applies_the_same_rules():
+def test_img_size_setter_applies_the_same_rules(built_lib):
     from videoseal_b200.model import Videoseal
     m = Videoseal(cfg.spec_from_card(ut.tiny_card()))
     for bad in (128, 1024):
@@ -67,7 +67,7 @@ def test_img_size_setter_applies_the_same_rules():
     assert m.img_size == 512
 
 
-def test_four_level_cards_keep_their_sizes():
+def test_four_level_cards_keep_their_sizes(built_lib):
     """the bottleneck rule leaves the 4-level cards at S >= 128 as they were"""
     from tests.util import load_card
     for name in ("videoseal_1.0", "pixelseal", "chunkyseal"):

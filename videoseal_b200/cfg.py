@@ -101,15 +101,12 @@ def spec_from_card(card: dict) -> dict:
         dims = [int(x * mult) for x in dims]
     if enc.get("temporal_convs", False) or enc.get("temporal_attention", False):
         raise NotImplementedError("temporal ConvNeXt variants are out of scope")
-    if pixelwise:
-        check_pixel_decoder(dims[-1], stages, int(img_size), nbits)
-    check_unet([int(u["z_channels"]) * int(m) for m in u["z_channels_mults"]], int(img_size))
     att = str(a.get("attenuation", "None"))
     jnd = (0, 0)
     if att.lower().startswith("jnd"):
         att_cfg = yaml.safe_load(open(resolve_config_path(a.get("attenuation_config", "configs/attenuation.yaml"))))
         jnd = (int(att_cfg[att]["in_channels"]), int(att_cfg[att]["out_channels"]))
-    return {
+    spec = {
         "nbits": nbits, "hidden": int(nbits * hsm), "img_size": int(img_size), "yuv": "yuv" in emb_name,
         "scaling_w": float(a["scaling_w"]), "scaling_i": float(a["scaling_i"]),
         "chunk_size": int(a.get("videoseal_chunk_size", a.get("videowam_chunk_size", 8))),
@@ -124,52 +121,10 @@ def spec_from_card(card: dict) -> dict:
         "pixel_decoder": {"pixelwise": pixelwise, "upscale_stages": stages},
         "jnd": jnd, "attenuation": att,
     }
-
-
-def check_pixel_decoder(c: int, stages: list, img_size: int, nbits: int) -> None:
-    """Widths and sizes the native pixel-wise decoder implements (model.cuh:add_pixel_decoder), checked at load time.  Stage i maps
-    c -> c // f_i channels (pixel_decoder.py:44-50).  The stage GEMM takes c in {16, 32} or >= 64 as its first input; every output
-    width is a multiple of 8, of the form 8 * {1, 3} * 2^k (k <= 5) for a middle stage, and at most 32 for the last one, whose
-    kernel holds one pixel's channels in registers.  The last stage's map must tile by 16 / f pixels, and its shared memory (the
-    staged taps plus the fp32 head weights) must fit in one H100 block."""
-    if not (c in (16, 32) or c >= 64):
-        raise NotImplementedError(f"pixel decoder: a trunk width of {c} is not implemented (16, 32 or >= 64)")
-    h = (img_size - 4) // 4 + 1
-    for _ in range(3):
-        h = (h - 2) // 2 + 1
-    for i, f in enumerate(stages):
-        co, last = c // f, i == len(stages) - 1
-        if c % f or co % 8:
-            raise NotImplementedError(f"pixel decoder: stage {i} maps {c} -> {c / f:g} channels; widths must be multiples of 8")
-        if last:
-            if co > 32:
-                raise NotImplementedError(f"pixel decoder: the last stage has {co} channels; at most 32 are implemented")
-            t = 16 // f
-            smem = (t + 2) ** 2 * 9 * co * 2 + (1 + nbits) * (co + 1) * 4
-            if h % t or smem > 227 * 1024:
-                raise NotImplementedError(f"pixel decoder: a last stage on a {h}-pixel map with {co} channels and {nbits} bits is not "
-                                          "implemented (the map must be a multiple of 16 / f; head weights must fit in shared memory)")
-        elif not any(co % (8 * v) == 0 and co // (8 * v) <= 32 and (co // (8 * v)) & (co // (8 * v) - 1) == 0 for v in (1, 3)):
-            raise NotImplementedError(f"pixel decoder: stage {i} has {co} channels; middle stages take 8 * {{1, 3}} * 2^k, k <= 5")
-        c, h = co, h * f
-
-
-def check_unet(z: list, img_size: int) -> None:
-    """U-Net widths and sizes the native embedder implements (model.cuh: Model::finalize), checked at load time.  A level is 16, 32
-    or a multiple of 64 channels wide, or 8 in a leading run of levels that stops before the last one (the 8-channel direct-conv
-    kernels; unet_tiny_*).  The bottleneck map, img_size / 2^(levels - 1), is at least 16 pixels: the tensor-core convs tile
-    maps by 128 pixels.  An 8-channel U-Net runs at processing sizes up to 768, where its 8-channel rings still fit in shared
-    memory."""
-    L = len(z)
-    for i, c in enumerate(z):
-        if not ((c == 8 and i < L - 1 and (i == 0 or z[i - 1] == 8)) or c in (16, 32) or (c > 0 and c % 64 == 0)):
-            raise NotImplementedError(f"U-Net width {c} at level {i} is not implemented (8 in the leading levels, 16, 32 or a "
-                                      "multiple of 64)")
-    if img_size >> (L - 1) < 16:
-        raise NotImplementedError(f"img_size={img_size}: the U-Net's {L} levels leave a {img_size >> (L - 1)}-pixel bottleneck map; "
-                                  "at least 16 is implemented")
-    if z[0] == 8 and img_size > 768:
-        raise NotImplementedError(f"img_size={img_size}: an 8-channel U-Net runs at processing sizes up to 768")
+    # the geometry rules of the kernels (widths, sizes, pixel-decoder stages) live in the native library: a dry run, no GPU needed
+    from .model import check_native
+    check_native(spec)
+    return spec
 
 
 def setup_model(card: dict, ckpt_path):

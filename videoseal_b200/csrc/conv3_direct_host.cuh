@@ -45,15 +45,12 @@ inline int conv3_direct_min_rows(int W, int R = 3, int C = 16) {
   const int rw = conv3_direct_pitch(W, R, C);
   return (kD3EpiSets * 128 + R - 1 + rw - 1) / rw + R + 2;
 }
-// W = 0: channel-count check only (weight packing time)
-inline bool conv3_direct_ok(int C, int N, int ld_in, int W = 0, int R = 3) {
-  if (ld_in != C) return false;
-  if (W == 0) return conv3_direct_ring_rows(C, N, 64, R) > 0;
+// R x R conv C -> N over a dense W-wide map: a kernel instantiation exists and its ring fits
+inline bool conv3_direct_ok(int C, int N, int W, int R = 3) {
   return W % 8 == 0 && conv3_direct_ring_rows(C, N, W, R) >= conv3_direct_min_rows(W, R, C);
 }
-// stride-2 conv Cin -> N through the space-to-depth ring (setup_down_s2d_direct) on an output map W wide (0 = channels only)
-inline bool conv3_direct_s2d_ok(int Cin, int N, int W = 0) {
-  if (W == 0) return conv3_direct_ring_rows(4 * Cin, N, 64, 3, true) > 0;
+// stride-2 conv Cin -> N through the space-to-depth ring (setup_down_s2d_direct) on an output map W wide
+inline bool conv3_direct_s2d_ok(int Cin, int N, int W) {
   return W % 8 == 0 && conv3_direct_ring_rows(4 * Cin, N, W, 3, true) >= conv3_direct_min_rows(W, 3, 4 * Cin);
 }
 

@@ -91,8 +91,9 @@ struct Plan {
   }
 };
 
-// tiling cap of the pixel decoder's gather kernels: the opt-in shared memory of one H100 block
+// tiling caps of the gather kernels: the pixel decoder's is the opt-in shared memory of one H100 block, the U-Net up-convs' 160 KB
 constexpr size_t kPdMaxSmem = 227 * 1024;
+constexpr size_t kUpGatherSmem = 160 * 1024;
 
 class Model {
  public:
@@ -126,11 +127,11 @@ class Model {
   std::vector<std::vector<CnBlockW>> cn;
   ConvW head_conv;
   float *head_lnw = nullptr, *head_lnb = nullptr, *head_lw = nullptr, *head_lb = nullptr;
-  // pixel-wise decoder (vsb_model_set_pixel_decoder; pixel_decoder.py:44-83): stage i = bilinear x pd_factors[i], reflect-padded 3x3
+  // pixel-wise decoder (vsb_model_set_pixel_decoder; pixel_decoder.py:44-83): stage i = bilinear x pd[i].f, reflect-padded 3x3
   // conv C -> C / f, LayerNorm, GELU; then the 1x1 conv head C_last -> 1 + nbits per pixel
   bool pixelwise = false;
-  std::vector<int> pd_factors;
-  struct PdStageW { ConvW taps; float* lnw; float* lnb; int cin, cout, kin; };
+  // geometry and gather kernel (16-byte vectors per thread; tiled when smem > 0) from set_pixel_decoder, weights from finalize
+  struct PdStageW { ConvW taps; float* lnw; float* lnb; int f, cin, cout, kin, vpt; size_t smem; };
   std::vector<PdStageW> pd;
   float *pd_hw = nullptr, *pd_hb = nullptr;   // fp32 [1+nbits][C_last], [1+nbits]
 
@@ -162,8 +163,91 @@ class Model {
   int32_t last_resize[5] = {-1, -1, -1, -1, -1};
   int32_t last_blend[5] = {-1, -1, -1, -1, -1};
 
-  explicit Model(const vsb_model_desc& desc) : d(desc) {}
+  explicit Model(const vsb_model_desc& desc) : d(desc) { check_desc(); }
 
+  // ---- the kernel of every U-Net layer at the map width it runs at, chosen once by check_desc.  finalize packs only the weights
+  // that kernel reads, and plan building follows them: ConvW::wd (direct ring conv) or ::w (tensor-core GEMM), down_conv[i].wd
+  // (space-to-depth ring conv) or .w (gather GEMM), up_phase_w[j] (phase-folded ring conv + border fix) or up_conv[j] (tap GEMM +
+  // gather with `vpt` 16-byte channel vectors per thread, tiled when smem > 0).
+  struct ResBlockK { bool res, c1, c2; };   // true: the direct ring conv
+  struct UpK { bool phase; int vpt; size_t smem; };
+  bool inc_k = false;
+  std::vector<bool> down_k;
+  std::vector<ResBlockK> down_rb_k, up_rb_k;
+  ResBlockK bott_rb_k{};
+  std::vector<UpK> up_k;
+
+  // vsb_model_create: every rule that depends only on the descriptor, and the U-Net's kernels (no CUDA calls)
+  void check_desc() {
+    if (d.unet_act != 0 || d.unet_norm != 0) throw Error("unsupported card: only BatchNorm+ReLU U-Nets are implemented on the GPU path", kErrUnsupported);
+    VSB_CHECK(d.unet_levels >= 2 && d.unet_levels <= 6, "unet levels");
+    VSB_CHECK(d.unet_in_ch == 1 || d.unet_in_ch == 3, "unet in_channels must be 1 or 3");
+    VSB_CHECK(d.unet_out_ch >= 1 && d.unet_out_ch <= 3, "unet out_channels must be <= 3");
+    VSB_CHECK((d.yuv != 0) == (d.unet_in_ch == 1), "yuv cards use 1 input channel");
+    const int S = d.img_size, L = d.unet_levels, zb = d.unet_z[L - 1] + d.hidden;
+    const int* z = d.unet_z;
+    for (int i = 0; i < L; ++i) {
+      // widths the kernels implement: 8 (a leading run of levels, not the last: the direct conv's 8-channel instantiations),
+      // 16, 32 and multiples of 64
+      const bool ok8 = z[i] == 8 && i < L - 1 && (i == 0 || z[i - 1] == 8);
+      if (!(ok8 || z[i] == 16 || z[i] == 32 || (z[i] > 0 && z[i] % 64 == 0)))
+        throw Error("U-Net width " + std::to_string(z[i]) + " at level " + std::to_string(i) + " is not implemented (8 in the "
+                    "leading levels, 16, 32 or a multiple of 64)", kErrUnsupported);
+    }
+    // the tensor-core convs tile maps by 128 pixels
+    if ((S >> (L - 1)) < 16)
+      throw Error("img_size=" + std::to_string(S) + ": the U-Net's " + std::to_string(L) + " levels leave a " +
+                  std::to_string(S >> (L - 1)) + "-pixel bottleneck map; at least 16 is implemented", kErrUnsupported);
+    // policy, also where the 8-channel rings would still fit: unet_tiny_yuv_quant's first ring to overflow is at 896
+    if (z[0] == 8 && S > 768)
+      throw Error("img_size=" + std::to_string(S) + ": an 8-channel U-Net runs at processing sizes up to 768", kErrUnsupported);
+    VSB_CHECK(S % 128 == 0, "processing size must be a multiple of 128");
+    VSB_CHECK(d.hidden % 8 == 0, "hidden must be a multiple of 8");
+    if (d.jnd_in_ch != 0 && !((d.jnd_in_ch == 1 || d.jnd_in_ch == 3) && (d.jnd_out_ch == 1 || d.jnd_out_ch == 3)))
+      throw Error("JND attenuation: in_channels / out_channels must be 1 or 3 (configs/attenuation.yaml)", kErrUnsupported);
+    for (int s = 0; s < 4; ++s) {
+      VSB_CHECK(d.ext_dims[s] % 2 == 0, "extractor widths must be even (channel pairs in the depthwise kernel)");
+      VSB_CHECK(s == 0 || d.ext_dims[s] >= d.ext_dims[s - 1], "extractor widths must not shrink along the trunk");
+    }
+    // 8-channel layers have no GEMM path: where their ring does not fit, the model is not implemented
+    auto ring8 = [](bool ring, int C, int W) {
+      if (C == 8 && !ring)
+        throw Error("8-channel layer on a " + std::to_string(W) + "-wide map: the direct conv's ring does not fit (processing size "
+                    "too large for an 8-channel U-Net)", kErrUnsupported);
+      return ring;
+    };
+    // ResnetBlock of C channels on a W-wide map; dense_out: its output has pitch C (the last down level writes the concat buffer)
+    auto resblock = [&](int C, int W, bool dense_out) {
+      return ResBlockK{ring8(conv3_direct_ok(C, C, W, 1), C, W), ring8(conv3_direct_ok(C, C, W), C, W),
+                       ring8(dense_out && conv3_direct_ok(C, C, W), C, W)};
+    };
+    inc_k = ring8(conv3_direct_ok(z[0], z[0], S), z[0], S);
+    for (int i = 0; i < L - 1; ++i) {
+      down_k.push_back(ring8(conv3_direct_s2d_ok(z[i], z[i + 1], S >> (i + 1)), z[i + 1], S >> (i + 1)));
+      down_rb_k.push_back(resblock(z[i + 1], S >> (i + 1), i < L - 2));
+    }
+    bott_rb_k = resblock(zb, S >> (L - 1), true);
+    for (int ii = L - 2; ii >= 0; --ii) {
+      const int hs = S >> (ii + 1), Cin = ii == L - 2 ? zb : z[ii + 1], Cout = z[ii];
+      UpK k{Cout == 16 && 2 * Cin == 64 && conv3_direct_ok(64, 64, hs), 0, 0};
+      if (!k.phase) {
+        // Cout / (8 * vpt) threads per output pixel, a power of two <= 32: VPT 2 only above 256 channels, which no shipped card has
+        // (chunkyseal's widest up block outputs 256)
+        k.vpt = Cout <= 256 ? 1 : 2;
+        const int g = Cout / (8 * k.vpt);
+        if (Cout % (8 * k.vpt) != 0 || g > 32 || (g & (g - 1)) != 0)
+          throw Error("U-Net up-conv to " + std::to_string(Cout) + " channels is not implemented (8 * 2^k, at most 512)", kErrUnsupported);
+        // low-resolution taps of a 16 x 16 output tile staged in shared memory (ups_gather_ln_tiled_kernel) when they fit
+        k.smem = hs % 8 == 0 && ups_tile_smem(2, Cout) <= kUpGatherSmem ? ups_tile_smem(2, Cout) : 0;
+      }
+      up_k.push_back(k);
+      up_rb_k.push_back(resblock(Cout, 2 * hs, true));
+    }
+  }
+
+  // vsb_model_set_pixel_decoder: the stage rules (include/vsb200.h) and each stage's gather kernel, no CUDA calls.  Stage i maps
+  // c -> c / f_i channels on an h-pixel map; the last stage's kernel holds one pixel's channels in registers and the head's weights
+  // beside its staged taps.
   void set_pixel_decoder(int n, const int32_t* f, int pw) {
     if (finalized) throw Error("model already finalized", kErrState);
     VSB_CHECK(pw == 0 || pw == 1, "pixelwise must be 0 or 1");
@@ -172,14 +256,38 @@ class Model {
     if (!pw) {
       if (n != 1 || f[0] != 1) throw Error("pooled pixel decoder: only upscale_stages [1] is implemented", kErrUnsupported);
       pixelwise = false;
-      pd_factors.clear();
+      pd.clear();
       return;
     }
     for (int i = 0; i < n; ++i)
       if (f[i] != 2 && f[i] != 4) throw Error("pixel-wise decoder: upscale factors must be 2 or 4", kErrUnsupported);
     if (d.ext_stem_stride != 4) throw Error("pixel-wise decoder: needs a ConvNeXt trunk with stem stride 4", kErrUnsupported);
+    std::vector<PdStageW> stages;
+    int c = d.ext_dims[3], h = trunk_map();
+    for (int i = 0; i < n; ++i) {
+      const int F = f[i], co = c / F, T = 16 / F;
+      const bool last = i + 1 == n;
+      if (c % F != 0 || co % 8 != 0 || (last ? co > 32 : pd_vpt(co) == 0) || (i == 0 && pd_gemm_k(c) != c))
+        throw Error("pixel decoder: stage " + std::to_string(i) + " (" + std::to_string(c) + " channels / " + std::to_string(F) +
+                    ") is not implemented (a trunk width of 16, 32 or >= 64; stage widths multiples of 8 of the form 8 * {1,3} * 2^k, "
+                    "the last one at most 32)", kErrUnsupported);
+      PdStageW s{};
+      s.f = F; s.cin = c; s.cout = co; s.kin = pd_gemm_k(c);
+      const size_t tsmem = ups_tile_smem(F, co);
+      if (last) {
+        s.vpt = co / 8;
+        s.smem = tsmem + (size_t)(1 + d.nbits) * (co + 1) * sizeof(float);
+        if (h % T != 0 || s.smem > kPdMaxSmem)
+          throw Error("pixel-wise head: a " + std::to_string(h) + "-pixel map with " + std::to_string(1 + d.nbits) + " outputs is not implemented", kErrUnsupported);
+      } else {
+        s.vpt = pd_vpt(co);
+        s.smem = h % T == 0 && tsmem <= kPdMaxSmem ? tsmem : 0;
+      }
+      stages.push_back(s);
+      c = co; h *= F;
+    }
     pixelwise = true;
-    pd_factors.assign(f, f + n);
+    pd = std::move(stages);
   }
   // side of the trunk's last feature map: stem k4 / stride st, then three k2 s2 downsampling layers
   int trunk_map() const {
@@ -190,7 +298,7 @@ class Model {
   // floats vsb_detect writes per frame: 1+nbits logits, or 1+nbits maps of P x P for a pixel-wise model
   size_t detect_out_per_frame() const {
     size_t P = (size_t)trunk_map();
-    for (int f : pd_factors) P *= f;
+    for (const PdStageW& s : pd) P *= s.f;
     return pixelwise ? (size_t)(1 + d.nbits) * P * P : (size_t)(1 + d.nbits);
   }
   void check_pooled_head(const std::string& what) const {
@@ -351,16 +459,17 @@ class Model {
     return pack_direct_taps(s2d_weights(conv_taps(w, nullptr), N, Ci), N, 4 * Ci);
   }
   static bool use_halo(int C) { return C <= 16; }
-  ConvW pack_conv3(const std::string& wkey, const std::vector<float>* out_scale, const std::vector<float>& bias) {
-    const int C = (int)get(wkey).shape[1], N = (int)get(wkey).shape[0];
+  // U-Net conv (3x3 or 1x1, stride 1) in the layout its kernel reads: the direct ring conv's, or the GEMM's (for 3x3 convs up to 16
+  // input channels, the halo loader's)
+  ConvW pack_unet_conv(const std::string& wkey, const std::vector<float>* out_scale, const std::vector<float>& bias, bool direct) {
+    const HostTensor& w = get(wkey);
+    const int C = (int)w.shape[1];
+    if (!direct)
+      return w.shape.size() == 4 && w.shape[2] == 3 && use_halo(C) ? pack_conv_halo(wkey, out_scale, bias, C, 0) : pack_conv(wkey, out_scale, bias);
     ConvW cw;
-    if (C == 8) {   // no GEMM path
-      cw.N = N; cw.K = 9 * C;
-      cw.bias = wpool.upload(bias);
-    } else {
-      cw = use_halo(C) ? pack_conv_halo(wkey, out_scale, bias, C, 0) : pack_conv(wkey, out_scale, bias);
-    }
-    if (C == 8 || conv3_direct_ok(C, N, C)) cw.wd = pack_direct(wkey, out_scale);
+    cw.N = (int)w.shape[0];
+    cw.wd = pack_direct(wkey, out_scale);
+    cw.bias = wpool.upload(bias);
     return cw;
   }
   // eval-mode BatchNorm2d folded into the preceding bias-free conv: w' = w*g/sqrt(var+eps), b' = beta - mean*g/sqrt(var+eps)
@@ -374,16 +483,14 @@ class Model {
       bias[i] = b.data[i] - mu.data[i] * s;
     }
   }
-  ResBlockW pack_resblock(const std::string& key) {
+  ResBlockW pack_resblock(const std::string& key, const ResBlockK& k) {
     ResBlockW rb;
     std::vector<float> s, b;
     bn_fold(key + ".double_conv.1", s, b);
-    rb.c1 = pack_conv3(key + ".double_conv.0.weight", &s, b);
+    rb.c1 = pack_unet_conv(key + ".double_conv.0.weight", &s, b, k.c1);
     bn_fold(key + ".double_conv.4", s, b);
-    rb.c2 = pack_conv3(key + ".double_conv.3.weight", &s, b);
-    rb.res = pack_conv(key + ".res_conv.weight", nullptr, get(key + ".res_conv.bias").data);
-    if (rb.res.K == 8 || conv3_direct_ok(rb.res.K, rb.res.N, rb.res.K, 0, 1))   // narrow 1x1: same ring kernel with a single tap
-      rb.res.wd = pack_direct(key + ".res_conv.weight", nullptr);
+    rb.c2 = pack_unet_conv(key + ".double_conv.3.weight", &s, b, k.c2);
+    rb.res = pack_unet_conv(key + ".res_conv.weight", nullptr, get(key + ".res_conv.bias").data, k.res);
     return rb;
   }
 
@@ -397,12 +504,6 @@ class Model {
     if (prop.major != 9 || prop.minor != 0) throw Error("libvsb200 is built for sm_90a only (found sm_" + std::to_string(prop.major) + std::to_string(prop.minor) + ")", kErrUnsupported);
     device = dev;
     num_sms = prop.multiProcessorCount;
-    if (d.unet_act != 0 || d.unet_norm != 0) throw Error("unsupported card: only BatchNorm+ReLU U-Nets are implemented on the GPU path", kErrUnsupported);
-    VSB_CHECK(d.unet_levels >= 2 && d.unet_levels <= 6, "unet levels");
-    VSB_CHECK(d.unet_in_ch == 1 || d.unet_in_ch == 3, "unet in_channels must be 1 or 3");
-    VSB_CHECK(d.unet_out_ch >= 1 && d.unet_out_ch <= 3, "unet out_channels must be <= 3");
-    VSB_CHECK((d.yuv != 0) == (d.unet_in_ch == 1), "yuv cards use 1 input channel");
-    VSB_CHECK(d.img_size % 128 == 0, "processing size must be a multiple of 128");
     const std::string P = "embedder.unet.";
     const int L = d.unet_levels;
     std::vector<int> z(d.unet_z, d.unet_z + L);
@@ -412,17 +513,6 @@ class Model {
       bn_fold(P + "inc.double_conv.1", s, b);
       const HostTensor& w = get(P + "inc.double_conv.0.weight");
       VSB_CHECK((int)w.shape[0] == z[0] && (int)w.shape[1] == d.unet_in_ch, "inc conv shape");
-      for (int i = 0; i < L; ++i) {
-        // widths the kernels implement: 8 (a leading run of levels, not the last: the direct conv's 8-channel instantiations),
-        // 16, 32 and multiples of 64 (cfg.check_unet has the same rule)
-        const bool ok8 = z[i] == 8 && i < L - 1 && (i == 0 || z[i - 1] == 8);
-        if (!(ok8 || z[i] == 16 || z[i] == 32 || (z[i] > 0 && z[i] % 64 == 0)))
-          throw Error("U-Net width " + std::to_string(z[i]) + " at level " + std::to_string(i) + " is not implemented (8 in the "
-                      "leading levels, 16, 32 or a multiple of 64)", kErrUnsupported);
-      }
-      if ((d.img_size >> (L - 1)) < 16)
-        throw Error("U-Net bottleneck map " + std::to_string(d.img_size >> (L - 1)) + "^2 is below 16^2 (processing size " +
-                    std::to_string(d.img_size) + ", " + std::to_string(L) + " levels): not implemented", kErrUnsupported);
       std::vector<float> w1(w.data);
       const size_t per = (size_t)d.unet_in_ch * 9;
       for (int n = 0; n < z[0]; ++n) for (size_t k = 0; k < per; ++k) w1[n * per + k] *= s[n];
@@ -430,15 +520,18 @@ class Model {
       first_wr = wpool.upload(get(P + "inc.res_conv.weight").data);
       first_br = wpool.upload(get(P + "inc.res_conv.bias").data);
       bn_fold(P + "inc.double_conv.4", s, b);
-      inc_c2 = pack_conv3(P + "inc.double_conv.3.weight", &s, b);
+      inc_c2 = pack_unet_conv(P + "inc.double_conv.3.weight", &s, b, inc_k);
     }
     for (int i = 0; i < L - 1; ++i) {
-      down_conv.push_back(pack_conv(P + "downs." + std::to_string(i) + ".down.weight", nullptr, get(P + "downs." + std::to_string(i) + ".down.bias").data));
-      if (conv3_direct_s2d_ok(z[i], z[i + 1]))
-        down_conv.back().wd = pack_down_s2d(P + "downs." + std::to_string(i) + ".down.weight");
-      down_rb.push_back(pack_resblock(P + "downs." + std::to_string(i) + ".conv"));
+      const std::string D = P + "downs." + std::to_string(i);
+      const std::vector<float>& bias = get(D + ".down.bias").data;
+      ConvW dc;
+      if (down_k[i]) { dc.wd = pack_down_s2d(D + ".down.weight"); dc.bias = wpool.upload(bias); }
+      else dc = pack_conv(D + ".down.weight", nullptr, bias);
+      down_conv.push_back(dc);
+      down_rb.push_back(pack_resblock(D + ".conv", down_rb_k[i]));
     }
-    for (int i = 0; i < d.unet_num_blocks; ++i) bott_rb.push_back(pack_resblock(P + "bottleneck.model." + std::to_string(i)));
+    for (int i = 0; i < d.unet_num_blocks; ++i) bott_rb.push_back(pack_resblock(P + "bottleneck.model." + std::to_string(i), bott_rb_k));
     {
       std::vector<int> zz(z);
       zz[L - 1] += d.hidden;
@@ -449,14 +542,13 @@ class Model {
         std::vector<float> in_scale(2 * zz[ii + 1], 1.0f);
         for (int c = zz[ii + 1]; c < 2 * zz[ii + 1]; ++c) in_scale[c] = 0.70710678118654752440f;
         // 8-channel sources go through the gather loader, whose K block is 64: pad K to one block
-        up_conv.push_back(pack_upconv_taps(U + ".up.upsample_block.2.weight", in_scale, zz[ii + 1] == 8 ? 64 : 0));
+        up_conv.push_back(up_k[j].phase ? ConvW{} : pack_upconv_taps(U + ".up.upsample_block.2.weight", in_scale, zz[ii + 1] == 8 ? 64 : 0));
         __half* pw = nullptr; float* bw = nullptr;
-        if (zz[ii] == 16 && 2 * zz[ii + 1] == 64 && conv3_direct_ok(64, 64, 64, 0, 3))
-          pack_upconv_phase(U + ".up.upsample_block.2.weight", in_scale, &pw, &bw);
+        if (up_k[j].phase) pack_upconv_phase(U + ".up.upsample_block.2.weight", in_scale, &pw, &bw);
         up_phase_w.push_back(pw); up_border_w.push_back(bw);
         up_lnw.push_back(wpool.upload(get(U + ".up.upsample_block.3.weight").data));
         up_lnb.push_back(wpool.upload(get(U + ".up.upsample_block.3.bias").data));
-        up_rb.push_back(pack_resblock(U + ".conv"));
+        up_rb.push_back(pack_resblock(U + ".conv", up_rb_k[j]));
       }
     }
     outc_w = wpool.upload(get(P + "outc.weight").data);  // [n_out][z0][1][1]
@@ -464,7 +556,6 @@ class Model {
     {
       const HostTensor& t = get(P + "msg_processor.msg_embeddings.weight");
       VSB_CHECK((int)t.shape[0] == 2 * d.nbits && (int)t.shape[1] == d.hidden, "message table shape");
-      VSB_CHECK(d.hidden % 8 == 0, "hidden must be a multiple of 8");
       msg_table = wpool.upload(t.data);
     }
     // ---- extractor (ConvNeXt-V2)
@@ -497,7 +588,6 @@ class Model {
     cn.resize(4);
     for (int s = 0; s < 4; ++s) {
       const int C = d.ext_dims[s];
-      VSB_CHECK(C % 2 == 0, "extractor widths must be even (channel pairs in the depthwise kernel)");
       for (int j = 0; j < d.ext_depths[s]; ++j) {
         const std::string B = Q + "stages." + std::to_string(s) + "." + std::to_string(j) + ".";
         CnBlockW w;
@@ -524,27 +614,18 @@ class Model {
     }
     if (pixelwise) {
       const std::string D = "detector.pixel_decoder.";
-      int c = d.ext_dims[3];
-      for (size_t i = 0; i < pd_factors.size(); ++i) {
+      for (size_t i = 0; i < pd.size(); ++i) {
         const std::string K = D + "output_upscaling." + std::to_string(i) + ".upsample_block.";
-        const int f = pd_factors[i], co = c / f;
-        const bool last = i + 1 == pd_factors.size();
+        PdStageW& sw = pd[i];
         const HostTensor& w = get(K + "2.weight");
-        VSB_CHECK(w.shape.size() == 4 && (int)w.shape[0] == co && (int)w.shape[1] == c && w.shape[2] == 3 && w.shape[3] == 3,
+        VSB_CHECK(w.shape.size() == 4 && (int)w.shape[0] == sw.cout && (int)w.shape[1] == sw.cin && w.shape[2] == 3 && w.shape[3] == 3,
                   "pixel decoder stage " + std::to_string(i) + ": weight must be [C/f, C, 3, 3]");
-        if (co % 8 != 0 || (last ? co > 32 : pd_vpt(co) == 0) || (i == 0 && pd_gemm_k(c) != c))
-          throw Error("pixel decoder: stage width " + std::to_string(c) + " -> " + std::to_string(co) + " is not implemented (widths must be "
-                      "multiples of 8 of the form 8 * {1,3} * 2^k, the last one at most 32)", kErrUnsupported);
-        PdStageW sw;
-        sw.cin = c; sw.cout = co; sw.kin = pd_gemm_k(c);
-        sw.taps = pack_upconv_taps(K + "2.weight", std::vector<float>(c, 1.f), sw.kin);
+        sw.taps = pack_upconv_taps(K + "2.weight", std::vector<float>(sw.cin, 1.f), sw.kin);
         sw.lnw = wpool.upload(get(K + "3.weight").data);
         sw.lnb = wpool.upload(get(K + "3.bias").data);
-        pd.push_back(sw);
-        c = co;
       }
       const HostTensor& lw = get(D + "linear.weight");
-      VSB_CHECK(lw.shape.size() == 4 && (int)lw.shape[0] == 1 + d.nbits && (int)lw.shape[1] == c && lw.shape[2] == 1 && lw.shape[3] == 1,
+      VSB_CHECK(lw.shape.size() == 4 && (int)lw.shape[0] == 1 + d.nbits && (int)lw.shape[1] == pd.back().cout && lw.shape[2] == 1 && lw.shape[3] == 1,
                 "pixel-wise head: linear.weight must be [1+nbits, C, 1, 1]");
       pd_hw = wpool.upload(lw.data);
       pd_hb = wpool.upload(get(D + "linear.bias").data);
@@ -572,12 +653,13 @@ class Model {
   }
 
   // One U-Net conv step, R x R (3: stride 1, zero pad 1; or 1) over x [B,H,W,Cin] (pitch ldx): the direct ring conv when its
-  // weights were packed and the map allows it, else the tensor-core GEMM.  Epilogue: bias, ReLU (relu), + the fp16 residual
+  // weights were packed for it (choose_unet), else the tensor-core GEMM.  Epilogue: bias, ReLU (relu), + the fp16 residual
   // `resid` (pitch w.N), output `out` (pitch ld_out; nullptr: not written) and, fuse_outc, the 1x1 outc + tanh into pl.delta.
   void add_unet_conv(Plan& pl, const ConvW& w, int R, const __half* x, int B, int H, int W, int Cin, int ldx, bool relu,
                      const __half* resid, __half* out, int ld_out, bool fuse_outc = false) {
     const int N = w.N;
-    const bool direct = w.wd && conv3_direct_ok(Cin, N, ldx, W, R) && (out == nullptr || ld_out == N);
+    const bool direct = w.wd != nullptr;
+    VSB_CHECK(!direct || (ldx == Cin && (out == nullptr || ld_out == N)), "direct conv: dense input and output");
     const std::string name = std::string("unet.conv") + (R == 3 ? "3x3" : "1x1") + (direct ? "d" : "") + (fuse_outc ? "+outc." : ".") +
                              std::to_string(Cin) + "-" + std::to_string(N) + "@" + std::to_string(H);
     if (direct) {
@@ -590,7 +672,7 @@ class Model {
       return;
     }
     // 3x3 up to 16 input channels: on-chip im2col from a shared-memory halo tile (input crosses L2->SM once), one TMA load per tap
-    // above; the weight layout was chosen by the same rule at pack time (pack_conv3)
+    // above; the weight layout follows the same rule (pack_unet_conv)
     ConvGemmOp op;
     if (R == 3 && use_halo(Cin)) setup_halo_conv3(op, x, B, H, W, Cin, ldx);
     else setup_tma_conv(op, x, B, H, W, Cin, ldx, R, R, R / 2);
@@ -614,9 +696,6 @@ class Model {
     __half* r = pl.pool.alloc_n<__half>(M * Cout);
     __half* h = pl.pool.alloc_n<__half>(M * Cout);
     if (!out && !fuse_outc) { out = pl.pool.alloc_n<__half>(M * Cout); ld_out = Cout; }
-    if (Cout == 8 && !(conv3_direct_ok(8, 8, ldx, W) && conv3_direct_ok(8, 8, ldx, W, 1) && (out == nullptr || ld_out == 8)))
-      throw Error("8-channel ResnetBlock on a " + std::to_string(W) + "-wide map: the direct conv's ring does not fit (processing "
-                  "size too large for an 8-channel U-Net)", kErrUnsupported);
     add_unet_conv(pl, w.res, 1, x, B, H, W, Cin, ldx, false, nullptr, r, Cout);
     add_unet_conv(pl, w.c1, 3, x, B, H, W, Cin, ldx, true, nullptr, h, Cout);
     add_unet_conv(pl, w.c2, 3, h, B, H, W, Cout, Cout, true, r, out, ld_out, fuse_outc);
@@ -674,8 +753,6 @@ class Model {
     std::vector<__half*> skips;  // outputs of inc, downs[0..]
     std::vector<int> skip_ld;
     __half* x = pl.pool.alloc_n<__half>(M0 * z[0]);
-    if (z[0] == 8 && !conv3_direct_ok(8, 8, 8, S))
-      throw Error("8-channel inc block on a " + std::to_string(S) + "-wide map: the direct conv's ring does not fit", kErrUnsupported);
     add_unet_conv(pl, inc_c2, 3, h1, B, S, S, z[0], z[0], true, r0, x, z[0]);
     dbg(pl, "inc", x, 1, B, S, S, z[0], z[0]);
     int ldx = z[0], hs = S;
@@ -685,13 +762,12 @@ class Model {
       const int ho = hs / 2;
       const long Mo = (long)B * ho * ho;
       __half* dn = pl.pool.alloc_n<__half>(Mo * z[i + 1]);
-      if (down_conv[i].wd && ldx == z[i] && hs % 2 == 0 && conv3_direct_s2d_ok(z[i], z[i + 1], ho)) {
+      if (down_conv[i].wd) {
         Conv3DirectOp op;
         setup_down_s2d_direct(op, x, z[i], B, ho, ho, z[i + 1], down_conv[i].wd, down_conv[i].bias, dn, num_sms);
         pl.steps.push_back(Step{[op](cudaStream_t st) { launch_direct(op, st); }, 1,
                                 "unet.down3x3s2d." + std::to_string(z[i]) + "-" + std::to_string(z[i + 1]) + "@" + std::to_string(ho)});
       } else {
-        if (z[i + 1] == 8) throw Error("8-channel stride-2 conv on a " + std::to_string(ho) + "-wide map: the direct conv's ring does not fit", kErrUnsupported);
         ConvGemmOp op;
         setup_gather_conv(op, LD_GATHER_CONV, x, z[i], ldx, nullptr, 0, 0, B, hs, hs, ho, ho, 3, 3, 2, 1, 0);
         op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.bias = down_conv[i].bias; op.p.out16 = dn; op.p.ld_out16 = z[i + 1];
@@ -734,7 +810,7 @@ class Model {
       const int ho = hs * 2;
       const long Mo = (long)B * ho * ho;
       __half* u = pl.pool.alloc_n<__half>(Mo * Cout);
-      if (up_phase_w[j] && ldx == Cin && ld_skip == Cin && conv3_direct_ok(64, 64, 64, hs, 3)) {
+      if (up_phase_w[j]) {
         // one tensor-core conv on the low-resolution grid (bilinear weights folded per output phase) + exact border pixels
         Conv3DirectOp op;
         setup_up_phase_direct(op, x, Cin, skip, Cin, B, hs, hs, up_phase_w[j], up_lnw[j], up_lnb[j], 1e-6f, u, num_sms);
@@ -758,14 +834,11 @@ class Model {
         add_conv(pl, op, up_conv[j], "unet.uptap1x1." + std::to_string(2 * Cin) + "-" + std::to_string(9 * Cout) + "@" + std::to_string(hs));
         dbg(pl, "up" + std::to_string(j) + "_taps", ytap, 1, B, hs, hs, 9 * Cout, 9 * Cout);
         // then bilinear x2 + reflect pad + 3x3 tap sum + LayerNorm + ReLU (CUDA cores, memory-bound)
-        const int vpt = Cout <= 256 ? 1 : 2;            // 16-byte channel vectors per thread (chunkyseal's first up-conv: 512 channels)
-        const int gthreads = Cout / (8 * vpt);          // threads per output pixel
-        VSB_CHECK(Cout % (8 * vpt) == 0 && gthreads <= 32 && (gthreads & (gthreads - 1)) == 0, "up conv: C_out must be 8 * 2^k <= 512");
+        const int vpt = up_k[j].vpt;
         UpsGather g;
         g.y = ytap; g.B = B; g.IH = hs; g.C = Cout; g.lnw = up_lnw[j]; g.lnb = up_lnb[j]; g.out = u; g.ld_out = Cout; g.num_sms = num_sms;
-        // low-resolution taps of a 16 x 16 output tile staged in shared memory (ups_gather_ln_tiled_kernel) when they fit in 160 KB
-        g.optin = 160 * 1024;
-        g.smem = hs % 8 == 0 && ups_tile_smem(2, Cout) <= g.optin ? ups_tile_smem(2, Cout) : 0;
+        g.optin = kUpGatherSmem;
+        g.smem = up_k[j].smem;
         pl.steps.push_back(Step{[g, vpt](cudaStream_t st) { launch_unet_upgather(g, vpt, st); }, 1,
                                 "unet.upgather." + std::to_string(Cout) + "@" + std::to_string(ho)});
       }
@@ -816,7 +889,6 @@ class Model {
     }
     int maxK4 = 0;
     for (int s = 0; s < 4; ++s) maxK4 = std::max(maxK4, 4 * d.ext_dims[s]);
-    for (int s = 1; s < 4; ++s) VSB_CHECK(d.ext_dims[s] >= d.ext_dims[s - 1], "extractor widths must not shrink along the trunk");
     // GRN statistics ping-pong: block j's pwconv1 accumulates into stats_pp[j&1]; its apply pass clears stats_pp[(j+1)&1] over
     // B*K_j floats, which covers what block j-1 left there because the widths never shrink along the trunk.  Both buffers are
     // zeroed at the start of every run (the last block of the previous run leaves its statistics behind).
@@ -944,7 +1016,7 @@ class Model {
     const int NO = 1 + d.nbits, nsm = num_sms;
     for (size_t i = 0; i < pd.size(); ++i) {
       const PdStageW& s = pd[i];
-      const int F = pd_factors[i], ho = F * h, Co = s.cout, IH = h, T = 16 / F;
+      const int F = s.f, ho = F * h, Co = s.cout, IH = h;
       const bool last = i + 1 == pd.size();
       const long Mi = (long)B * h * h;
       __half* ytap = pl.pool.alloc_n<__half>(Mi * 9 * Co);
@@ -953,22 +1025,18 @@ class Model {
       add_conv(pl, op, s.taps, "pd.uptap1x1." + std::to_string(s.cin) + "-" + std::to_string(9 * Co) + "@" + std::to_string(h));
       UpsGather g;
       g.y = ytap; g.B = B; g.IH = IH; g.C = Co; g.lnw = s.lnw; g.lnb = s.lnb; g.num_sms = nsm; g.optin = kPdMaxSmem;
-      const size_t tsmem = ups_tile_smem(F, Co);
+      g.smem = s.smem;
+      const int vpt = s.vpt;
       const std::string tag = std::to_string(Co) + "x" + std::to_string(F) + "@" + std::to_string(ho);
       if (last) {
-        g.smem = tsmem + (size_t)NO * (Co + 1) * sizeof(float);
-        if (IH % T != 0 || g.smem > kPdMaxSmem)
-          throw Error("pixel-wise head: a " + std::to_string(IH) + "-pixel map with " + std::to_string(NO) + " outputs is not implemented", kErrUnsupported);
         g.hw = pd_hw; g.hb = pd_hb; g.NO = NO;
-        pl.steps.push_back(Step{[g, F, plp](cudaStream_t st) mutable { g.maps = plp->out_maps; launch_pd_gather(g, F, g.C / 8, st); }, 1,
+        pl.steps.push_back(Step{[g, F, vpt, plp](cudaStream_t st) mutable { g.maps = plp->out_maps; launch_pd_gather(g, F, vpt, st); }, 1,
                                 "pd.gather_head." + tag});
       } else {
         const int ldo = pd_gemm_k(Co);
         // pad channels stay zero: the gather writes [0, Co)
         __half* u = ldo != Co ? pl.pool.alloc_zeroed<__half>((size_t)B * ho * ho * ldo) : pl.pool.alloc_n<__half>((size_t)B * ho * ho * ldo);
         g.out = u; g.ld_out = ldo;
-        g.smem = IH % T == 0 && tsmem <= kPdMaxSmem ? tsmem : 0;
-        const int vpt = pd_vpt(Co);
         pl.steps.push_back(Step{[g, F, vpt](cudaStream_t st) { launch_pd_gather(g, F, vpt, st); }, 1,
                                 std::string(g.smem ? "pd.upgather." : "pd.upgather_untiled.") + tag});
         dbg(pl, "pd" + std::to_string(i), u, 1, B, ho, ho, Co, ldo);
@@ -1168,8 +1236,6 @@ class Model {
     const bool same = (H == S && W == S);
     const bool aa = !(flags & VSB_FLAG_RESIZE_NO_AA);
     const bool use_jnd = !(flags & VSB_FLAG_NO_ATTENUATION) && d.jnd_in_ch != 0;
-    if (use_jnd && !((d.jnd_in_ch == 1 || d.jnd_in_ch == 3) && (d.jnd_out_ch == 1 || d.jnd_out_ch == 3)))
-      throw Error("JND attenuation: in_channels / out_channels must be 1 or 3 (configs/attenuation.yaml)", kErrUnsupported);
     // channels of hmaps * preds_w (broadcast): what `preds_w` holds and what the low-resolution path hands to the blend
     const int PC = use_jnd ? std::max(d.unet_out_ch, d.jnd_out_ch) : d.unet_out_ch;
     const bool lowres = use_jnd && (flags & VSB_FLAG_LOWRES_ATTN);

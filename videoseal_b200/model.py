@@ -19,6 +19,49 @@ from . import _lib
 _DEF_INTERP = {"mode": "bilinear", "align_corners": False, "antialias": True}
 
 
+def native_desc(spec: dict) -> _lib.ModelDesc:
+    """vsb_model_desc of `spec` (cfg.spec_from_card)"""
+    d = _lib.ModelDesc()
+    d.nbits, d.hidden, d.img_size, d.yuv = spec["nbits"], spec["hidden"], spec["img_size"], int(spec["yuv"])
+    u = spec["unet"]
+    d.unet_in_ch, d.unet_out_ch, d.unet_levels = u["in_channels"], u["out_channels"], len(u["z"])
+    for i, z in enumerate(u["z"]):
+        d.unet_z[i] = z
+    d.unet_num_blocks = u["num_blocks"]
+    acts, norms = {"relu": 0, "silu": 1}, {"batch": 0, "rms": 1}
+    if u["activation"] not in acts or not any(u["normalization"].startswith(k) for k in norms):
+        raise NotImplementedError(f"U-Net activation/normalization {u['activation']}/{u['normalization']} not implemented")
+    d.unet_act = acts[u["activation"]]
+    d.unet_norm = 0 if u["normalization"].startswith("batch") else 1
+    d.unet_last_tanh = int(u["last_tanh"])
+    cn = spec["convnext"]
+    for i in range(4):
+        d.ext_depths[i], d.ext_dims[i] = cn["depths"][i], cn["dims"][i]
+    d.ext_stem_stride = cn["stem_stride"]
+    d.jnd_in_ch, d.jnd_out_ch = spec["jnd"]
+    return d
+
+
+def _create(spec: dict):
+    """Native handle of `spec` without weights or a device.  vsb_model_create and vsb_model_set_pixel_decoder check every rule the
+    kernels place on the model's geometry; a model they do not implement raises NotImplementedError."""
+    L = _lib.lib()
+    h = C.c_void_p()
+    _lib.check(L.vsb_model_create(C.byref(native_desc(spec)), C.byref(h)))
+    pd = spec.get("pixel_decoder", {"pixelwise": False})
+    f = pd["upscale_stages"] if pd["pixelwise"] else None
+    rc = L.vsb_model_set_pixel_decoder(h, len(f), (C.c_int32 * len(f))(*f), 1) if f else 0
+    if rc != 0:
+        L.vsb_model_destroy(h)
+    _lib.check(rc)
+    return h
+
+
+def check_native(spec: dict) -> None:
+    """Load-time dry run: the native library implements `spec` (no GPU needed)."""
+    _lib.lib().vsb_model_destroy(_create(spec))
+
+
 class Blender:
     """models/blender.py: only the additive method is on the hot path (all shipped cards)."""
     AVAILABLE_BLENDING_METHODS = ["additive"]
@@ -133,12 +176,7 @@ class Videoseal(nn.Module):
         if v != self.spec["img_size"]:
             if v <= 0 or v % 128 != 0:
                 raise ValueError(f"img_size={v}: the native path needs a processing size that is a positive multiple of 128")
-            from .cfg import check_unet
-            check_unet(self.spec["unet"]["z"], v)
-            if self.pixelwise:
-                from .cfg import check_pixel_decoder
-                check_pixel_decoder(self.spec["convnext"]["dims"][-1], self.spec["pixel_decoder"]["upscale_stages"], v,
-                                    self.spec["nbits"])
+            check_native({**self.spec, "img_size": v})
             self._respec(img_size=v)
 
     @property
@@ -200,32 +238,8 @@ class Videoseal(nn.Module):
             return self._native[1]
         self._release()
         L = _lib.lib()
-        s = self.spec
-        d = _lib.ModelDesc()
-        d.nbits, d.hidden, d.img_size, d.yuv = s["nbits"], s["hidden"], s["img_size"], int(s["yuv"])
-        u = s["unet"]
-        d.unet_in_ch, d.unet_out_ch, d.unet_levels = u["in_channels"], u["out_channels"], len(u["z"])
-        for i, z in enumerate(u["z"]):
-            d.unet_z[i] = z
-        d.unet_num_blocks = u["num_blocks"]
-        acts, norms = {"relu": 0, "silu": 1}, {"batch": 0, "rms": 1}
-        if u["activation"] not in acts or not any(u["normalization"].startswith(k) for k in norms):
-            raise NotImplementedError(f"U-Net activation/normalization {u['activation']}/{u['normalization']} not implemented")
-        d.unet_act = acts[u["activation"]]
-        d.unet_norm = 0 if u["normalization"].startswith("batch") else 1
-        d.unet_last_tanh = int(u["last_tanh"])
-        cn = s["convnext"]
-        for i in range(4):
-            d.ext_depths[i], d.ext_dims[i] = cn["depths"][i], cn["dims"][i]
-        d.ext_stem_stride = cn["stem_stride"]
-        d.jnd_in_ch, d.jnd_out_ch = s["jnd"]
-        h = C.c_void_p()
-        _lib.check(L.vsb_model_create(C.byref(d), C.byref(h)))
+        h = _create(self.spec)
         try:
-            pd = s.get("pixel_decoder", {"pixelwise": False})
-            if pd["pixelwise"]:
-                f = pd["upscale_stages"]
-                _lib.check(L.vsb_model_set_pixel_decoder(h, len(f), (C.c_int32 * len(f))(*f), 1))
             for k, v in self._sd.items():
                 if k.startswith(("attenuation.", "rgb2yuv.")) or v.dim() > 4:
                     continue
