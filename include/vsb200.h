@@ -13,7 +13,7 @@
  *        modules/jnd.py:80, Blender.additive_blend blender.py:61, clamp)
  *   vsb_embedder_forward                      <-  models/embedder.py:151-165 UnetEmbedder.forward (operator seam)
  *   vsb_detect                                <-  models/wam.py:206-234 Wam.detect / videoseal.py:352-388 (resize,
- *        ConvnextExtractor.forward models/extractor.py:154)
+ *        ConvnextExtractor.forward models/extractor.py:154, or SegmentationExtractor.forward models/extractor.py:55-69)
  *   vsb_jnd_heatmaps                          <-  modules/jnd.py:80-108 JND.heatmaps (operator seam)
  *   vsb_embed_host / vsb_detect_host          <-  the same calls with HOST (CPU) tensors as the reference keeps
  *        full-resolution video on the CPU (evals/full.py:117-120); H2D/D2H copies happen inside.
@@ -79,14 +79,32 @@ int vsb_model_create(const vsb_model_desc* desc, vsb_model** out);
 int vsb_model_set_tensor(vsb_model* m, const char* name, const float* data, const int64_t* shape, int32_t ndim);
 /* Pixel-wise extractor head (modules/pixel_decoder.py:44-83 with pixelwise=True), called between create and finalize.  Without
  * this call the model has the pooled head (one [1+nbits] logit vector per frame).  pixelwise = 1 needs 1..8 stage factors, each 2
- * or 4, and a ConvNeXt trunk with ext_stem_stride 4; stage i maps C -> C / factors[i] channels (bilinear up-sampling, reflect-padded
+ * or 4, and a ConvNeXt trunk with ext_stem_stride 4 or a SAM-ViT trunk; stage i maps C -> C / factors[i] channels (bilinear up-sampling, reflect-padded
  * 3x3 conv, LayerNorm, GELU), then a 1x1 conv gives 1+nbits maps.  pixelwise = 0 accepts only n_stages = 1, factors = {1} (the
- * pooled head).  Like vsb_model_create it makes no CUDA call, and it returns VSB_ERR_UNSUPPORTED unless: the trunk width
- * ext_dims[3] is 16, 32 or >= 64; every stage width C / f is a whole multiple of 8, of the form 8 * {1, 3} * 2^k (k <= 5) for a
+ * pooled head).  A SAM-ViT trunk (vsb_model_set_vit_extractor, called first) has width out_chans on an img_size / 16 map and no
+ * stem-stride rule.  Like vsb_model_create it makes no CUDA call, and it returns VSB_ERR_UNSUPPORTED unless: the trunk width
+ * (ext_dims[3] or out_chans) is 16, 32 or >= 64; every stage width C / f is a whole multiple of 8, of the form 8 * {1, 3} * 2^k (k <= 5) for a
  * middle stage and at most 32 for the last; the last stage's input map is a multiple of 16 / f pixels, and its staged taps,
  * (16 / f + 2)^2 * 9 * C fp16, plus its head weights, (1 + nbits) * (C + 1) fp32, fit in 227 KB.  VSB_ERR_STATE after finalize;
  * VSB_ERR_INVALID / VSB_ERR_UNSUPPORTED for other values. */
 int vsb_model_set_pixel_decoder(vsb_model* m, int32_t n_stages, const int32_t* factors, int32_t pixelwise);
+/* SAM-ViT extractor (models/extractor.py:41-69 SegmentationExtractor, modules/vit.py ImageEncoderViT with use_abs_pos), replacing the
+ * ConvNeXt trunk; the ext_* fields of the model descriptor are then unused (zero).  The trunk's output is out_chans channels on a
+ * grid = img_size / 16 map, which the pooled head or the pixel-wise decoder reads as it reads the ConvNeXt trunk's. */
+typedef struct vsb_vit_desc {
+  int32_t embed_dim, depth, num_heads, patch_size, window_size;
+  uint32_t global_mask;      /* bit i set: block i attends over the whole grid (global_attn_indexes), else over windows */
+  int32_t mlp_dim;           /* int(embed_dim * mlp_ratio) */
+  int32_t out_chans;         /* neck width */
+  int32_t qkv_bias, use_rel_pos;
+} vsb_vit_desc;
+/* Called after vsb_model_create and before vsb_model_set_pixel_decoder and finalize; no CUDA call.  VSB_ERR_STATE after finalize.
+ * VSB_ERR_UNSUPPORTED unless: head dim embed_dim / num_heads = 64; mlp_dim and out_chans multiples of 64; patch_size 16; depth <= 32;
+ * grid = img_size / 16 divisible by window_size (no window padding) and every window a multiple of 64 tokens (window 8 passes, 14
+ * does not); global attention over at most 1024 tokens (img_size <= 512); with use_rel_pos, windows at most 32 tokens wide (the
+ * 2n - 1 rows of a relative-position table must fit in 64).  VSB_ERR_INVALID for depth < 1, mask bits at or above
+ * depth, or flags other than 0 / 1. */
+int vsb_model_set_vit_extractor(vsb_model* m, const vsb_vit_desc* vit);
 /* fold BN, pack to fp16 KRSC, upload to `device`, build nothing else (plans are built lazily per batch shape) */
 int vsb_model_finalize(vsb_model* m, int32_t device);
 void vsb_model_destroy(vsb_model* m);

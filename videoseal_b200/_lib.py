@@ -13,7 +13,7 @@ EXPORTS = [
     "vsb_last_error", "vsb_version", "vsb_model_create", "vsb_model_set_tensor", "vsb_model_set_pixel_decoder", "vsb_model_finalize",
     "vsb_model_destroy", "vsb_embed", "vsb_embedder_forward", "vsb_detect", "vsb_jnd_heatmaps", "vsb_embed_host",
     "vsb_detect_host", "vsb_embed_detect_host", "vsb_frames_host_u8", "vsb_launch_count", "vsb_profile_enable", "vsb_profile_read", "vsb_debug_get_tensor", "vsb_debug_conv",
-    "vsb_debug_resample_table", "vsb_debug_last_dispatch", "vsb_quality_workspace_bytes", "vsb_ssim",
+    "vsb_debug_resample_table", "vsb_debug_last_dispatch", "vsb_quality_workspace_bytes", "vsb_ssim", "vsb_model_set_vit_extractor",
 ]
 
 FLAG_CLAMP, FLAG_LOWRES_ATTN, FLAG_NO_ATTENUATION, FLAG_RESIZE_NO_AA = 1, 2, 4, 8
@@ -27,6 +27,14 @@ class ModelDesc(C.Structure):
         ("unet_num_blocks", C.c_int32), ("unet_act", C.c_int32), ("unet_norm", C.c_int32), ("unet_last_tanh", C.c_int32),
         ("ext_depths", C.c_int32 * 4), ("ext_dims", C.c_int32 * 4), ("ext_stem_stride", C.c_int32),
         ("jnd_in_ch", C.c_int32), ("jnd_out_ch", C.c_int32),
+    ]
+
+
+class VitDesc(C.Structure):
+    _fields_ = [
+        ("embed_dim", C.c_int32), ("depth", C.c_int32), ("num_heads", C.c_int32), ("patch_size", C.c_int32),
+        ("window_size", C.c_int32), ("global_mask", C.c_uint32), ("mlp_dim", C.c_int32), ("out_chans", C.c_int32),
+        ("qkv_bias", C.c_int32), ("use_rel_pos", C.c_int32),
     ]
 
 
@@ -62,6 +70,7 @@ def lib():
     L.vsb_model_create.argtypes = [C.POINTER(ModelDesc), C.POINTER(C.c_void_p)]
     L.vsb_model_set_tensor.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.POINTER(C.c_int64), C.c_int32]
     L.vsb_model_set_pixel_decoder.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_int32]
+    L.vsb_model_set_vit_extractor.argtypes = [C.c_void_p, C.POINTER(VitDesc)]
     L.vsb_model_finalize.argtypes = [C.c_void_p, C.c_int32]
     L.vsb_model_destroy.argtypes = [C.c_void_p]
     L.vsb_model_destroy.restype = None

@@ -71,8 +71,9 @@ def spec_from_card(card: dict) -> dict:
     ext_name = str(card["extractor"]["model"])
     if not emb_name.startswith("unet"):
         raise NotImplementedError(f"embedder '{emb_name}': only the unet* family is on the CUDA hot path")
-    if not ext_name.startswith("convnext"):
-        raise NotImplementedError(f"extractor '{ext_name}': only the convnext* family is on the CUDA hot path")
+    is_vit = ext_name.startswith("sam")
+    if not (ext_name.startswith("convnext") or is_vit):
+        raise NotImplementedError(f"extractor '{ext_name}': only the convnext* and sam* families are on the CUDA hot path")
     u = card["embedder"]["params"]["unet"]
     mp = card["embedder"]["params"].get("msg_processor", {})
     if mp.get("msg_processor_type", "binary+concat") != "binary+concat":
@@ -93,14 +94,7 @@ def spec_from_card(card: dict) -> dict:
     if pixelwise and str(pd.get("upscale_type", "bilinear")) != "bilinear":
         raise NotImplementedError(f"pixel decoder: upscale_type '{pd.get('upscale_type')}' is not implemented (only 'bilinear')")
     enc = ep["encoder"]
-    if pixelwise and (ep.get("proportional_dim", False) or int(enc.get("stem_stride", 4)) != 4):
-        raise NotImplementedError("pixel decoder: pixel-wise maps need a non-proportional ConvNeXt trunk with stem_stride 4")
-    dims = [int(x) for x in enc["dims"]]
-    if ep.get("proportional_dim", False):
-        mult = math.sqrt(nbits / 128)
-        dims = [int(x * mult) for x in dims]
-    if enc.get("temporal_convs", False) or enc.get("temporal_attention", False):
-        raise NotImplementedError("temporal ConvNeXt variants are out of scope")
+    trunk = _vit_trunk(enc) if is_vit else _convnext_trunk(ep, enc, nbits, pixelwise)
     att = str(a.get("attenuation", "None"))
     jnd = (0, 0)
     if att.lower().startswith("jnd"):
@@ -117,7 +111,7 @@ def spec_from_card(card: dict) -> dict:
             "activation": str(u["activation"]), "normalization": str(u["normalization"]),
             "last_tanh": bool(u.get("last_tanh", True)),
         },
-        "convnext": {"depths": [int(x) for x in enc["depths"]], "dims": dims, "stem_stride": int(enc.get("stem_stride", 4))},
+        **trunk,
         "pixel_decoder": {"pixelwise": pixelwise, "upscale_stages": stages},
         "jnd": jnd, "attenuation": att,
     }
@@ -125,6 +119,46 @@ def spec_from_card(card: dict) -> dict:
     from .model import check_native
     check_native(spec)
     return spec
+
+
+def _convnext_trunk(ep: dict, enc: dict, nbits: int, pixelwise: bool) -> dict:
+    """spec['convnext'] of a convnext* extractor (extractor.py:188-213)"""
+    if pixelwise and (ep.get("proportional_dim", False) or int(enc.get("stem_stride", 4)) != 4):
+        raise NotImplementedError("pixel decoder: pixel-wise maps need a non-proportional ConvNeXt trunk with stem_stride 4")
+    dims = [int(x) for x in enc["dims"]]
+    if ep.get("proportional_dim", False):
+        mult = math.sqrt(nbits / 128)
+        dims = [int(x * mult) for x in dims]
+    if enc.get("temporal_convs", False) or enc.get("temporal_attention", False):
+        raise NotImplementedError("temporal ConvNeXt variants are out of scope")
+    return {"convnext": {"depths": [int(x) for x in enc["depths"]], "dims": dims, "stem_stride": int(enc.get("stem_stride", 4))}}
+
+
+_VIT_KEYS = ("embed_dim", "depth", "num_heads", "patch_size", "window_size", "global_attn_indexes", "mlp_ratio", "out_chans")
+_CONVNEXT_KEYS = ("depths", "dims", "stem_stride", "drop_path_rate", "layer_scale_init_value", "head_init_scale")
+
+
+def _vit_trunk(enc: dict) -> dict:
+    """spec['vit'] of a sam* extractor (extractor.py:170-176, ImageEncoderViT vit.py:14-110); the processing size is the ViT's
+    img_size (build_extractor overrides the card's)"""
+    missing = [k for k in _VIT_KEYS if k not in enc]
+    foreign = [k for k in _CONVNEXT_KEYS if k in enc]
+    if missing or foreign:
+        raise NotImplementedError(f"SAM-ViT extractor: the encoder block lacks {missing} / carries ConvNeXt keys {foreign}")
+    if not enc.get("use_abs_pos", True):
+        raise NotImplementedError("SAM-ViT extractor: use_abs_pos=False is not implemented")
+    if enc.get("temporal_attention", False):
+        raise NotImplementedError("SAM-ViT extractor: temporal_attention is out of scope")
+    E, depth, ws = int(enc["embed_dim"]), int(enc["depth"]), int(enc["window_size"])
+    glob = sorted({int(i) for i in enc["global_attn_indexes"]})
+    if ws == 0:          # vit.py:79: window_size 0 makes every block global
+        glob = list(range(depth))
+    return {"vit": {
+        "embed_dim": E, "depth": depth, "num_heads": int(enc["num_heads"]), "patch_size": int(enc["patch_size"]),
+        "window_size": ws, "global_attn_indexes": [i for i in glob if 0 <= i < depth],
+        "mlp_dim": int(E * float(enc["mlp_ratio"])), "out_chans": int(enc["out_chans"]),
+        "qkv_bias": bool(enc.get("qkv_bias", True)), "use_rel_pos": bool(enc.get("use_rel_pos", False)),
+    }}
 
 
 def setup_model(card: dict, ckpt_path):

@@ -10,6 +10,7 @@
 #include <vector>
 
 #include "../../include/vsb200.h"
+#include "attention_host.cuh"
 #include "conv_gemm_host.cuh"
 #include "conv3_direct_host.cuh"
 #include "pointwise_host.cuh"
@@ -134,6 +135,15 @@ class Model {
   struct PdStageW { ConvW taps; float* lnw; float* lnb; int f, cin, cout, kin, vpt; size_t smem; };
   std::vector<PdStageW> pd;
   float *pd_hw = nullptr, *pd_hb = nullptr;   // fp32 [1+nbits][C_last], [1+nbits]
+  // SAM-ViT extractor (vsb_model_set_vit_extractor; modules/vit.py ImageEncoderViT): replaces the ConvNeXt trunk when `vit`
+  bool vit = false;
+  vsb_vit_desc vd{};
+  ConvW vit_patch;                      // [E][768] fp16, x*2-1 folded: W' = 2W (K order c, r, s); no bias (it is in vit_pos)
+  float* vit_pos = nullptr;             // fp32 [grid^2][E]: pos_embed + b - sum(W)
+  struct VitBlockW { float *n1w, *n1b, *n2w, *n2b; ConvW qkv, proj, lin1, lin2; __half *rel_h, *rel_w; };
+  std::vector<VitBlockW> vit_blk;
+  ConvW vit_neck1, vit_neck3;
+  float *vit_nln1w = nullptr, *vit_nln1b = nullptr, *vit_nln2w = nullptr, *vit_nln2b = nullptr;
 
   // grow-only device staging for the host-buffer entry points (no cudaMalloc on the steady-state path)
   struct Staging { void* p = nullptr; size_t cap = 0; };
@@ -261,9 +271,9 @@ class Model {
     }
     for (int i = 0; i < n; ++i)
       if (f[i] != 2 && f[i] != 4) throw Error("pixel-wise decoder: upscale factors must be 2 or 4", kErrUnsupported);
-    if (d.ext_stem_stride != 4) throw Error("pixel-wise decoder: needs a ConvNeXt trunk with stem stride 4", kErrUnsupported);
+    if (!vit && d.ext_stem_stride != 4) throw Error("pixel-wise decoder: needs a ConvNeXt trunk with stem stride 4", kErrUnsupported);
     std::vector<PdStageW> stages;
-    int c = d.ext_dims[3], h = trunk_map();
+    int c = trunk_width(), h = trunk_map();
     for (int i = 0; i < n; ++i) {
       const int F = f[i], co = c / F, T = 16 / F;
       const bool last = i + 1 == n;
@@ -289,8 +299,41 @@ class Model {
     pixelwise = true;
     pd = std::move(stages);
   }
-  // side of the trunk's last feature map: stem k4 / stride st, then three k2 s2 downsampling layers
+  // vsb_model_set_vit_extractor: the ViT rules (include/vsb200.h), no CUDA calls
+  void set_vit_extractor(const vsb_vit_desc& v) {
+    if (finalized) throw Error("model already finalized", kErrState);
+    if (pixelwise) throw Error("vsb_model_set_vit_extractor must come before vsb_model_set_pixel_decoder", kErrState);
+    VSB_CHECK(v.depth >= 1 && v.num_heads >= 1 && v.embed_dim >= 1 && v.window_size >= 0, "ViT: depth, num_heads and embed_dim must be positive");
+    VSB_CHECK(v.depth >= 32 || (v.global_mask >> v.depth) == 0, "ViT: global_mask has bits at or above depth");
+    VSB_CHECK((v.qkv_bias == 0 || v.qkv_bias == 1) && (v.use_rel_pos == 0 || v.use_rel_pos == 1), "ViT: qkv_bias / use_rel_pos must be 0 or 1");
+    auto unsup = [](const std::string& m) { throw Error("SAM-ViT extractor: " + m, kErrUnsupported); };
+    if (v.embed_dim % v.num_heads != 0 || v.embed_dim / v.num_heads != kAttnHd)
+      unsup("head dim " + std::to_string(v.embed_dim) + " / " + std::to_string(v.num_heads) + " is not implemented (64 only)");
+    if (v.mlp_dim <= 0 || v.mlp_dim % 64 != 0) unsup("mlp_dim " + std::to_string(v.mlp_dim) + " is not a multiple of 64");
+    if (v.out_chans <= 0 || v.out_chans % 64 != 0) unsup("out_chans " + std::to_string(v.out_chans) + " is not a multiple of 64");
+    if (v.patch_size != kVitPatch) unsup("patch_size " + std::to_string(v.patch_size) + " is not implemented (16 only)");
+    if (v.depth > 32) unsup("depth " + std::to_string(v.depth) + " above 32 is not implemented");
+    const int G = d.img_size / kVitPatch;
+    const uint32_t all = v.depth == 32 ? ~0u : (1u << v.depth) - 1u;
+    if (v.global_mask != all) {   // some block attends over windows
+      if (v.window_size <= 0 || G % v.window_size != 0)
+        unsup("a " + std::to_string(G) + "-token grid is not divisible by window_size " + std::to_string(v.window_size) + " (window padding is not implemented)");
+      if (v.window_size * v.window_size % kAttnTile != 0)
+        unsup("window_size " + std::to_string(v.window_size) + " holds " + std::to_string(v.window_size * v.window_size) + " tokens, not a multiple of 64");
+    }
+    if (v.global_mask != 0 && G * G > 1024)
+      unsup("global attention over " + std::to_string(G * G) + " tokens (img_size " + std::to_string(d.img_size) + ") is not implemented (at most 1024, img_size <= 512)");
+    // the kernel stages the 2n - 1 rows of each relative-position table in 64 rows: region sides n <= 32 (global blocks: the cap above)
+    if (v.use_rel_pos && v.global_mask != all && v.window_size > kAttnMaxRelSide)
+      unsup("relative positions over " + std::to_string(v.window_size) + "-token-wide windows are not implemented (at most " +
+            std::to_string(kAttnMaxRelSide) + ")");
+    vd = v;
+    vit = true;
+  }
+  int trunk_width() const { return vit ? vd.out_chans : d.ext_dims[3]; }
+  // side of the trunk's last feature map: stem k4 / stride st, then three k2 s2 downsampling layers; the ViT's token grid
   int trunk_map() const {
+    if (vit) return d.img_size / kVitPatch;
     int h = (d.img_size - 4) / d.ext_stem_stride + 1;
     for (int s = 1; s < 4; ++s) h = (h - 2) / 2 + 1;
     return h;
@@ -558,7 +601,87 @@ class Model {
       VSB_CHECK((int)t.shape[0] == 2 * d.nbits && (int)t.shape[1] == d.hidden, "message table shape");
       msg_table = wpool.upload(t.data);
     }
-    // ---- extractor (ConvNeXt-V2)
+    if (vit) finalize_vit();
+    else finalize_convnext();
+    finalize_head();
+    sd.clear();  // host copies no longer needed
+    finalized = true;
+  }
+
+  // ---- SAM-ViT extractor (modules/vit.py:14-143, :146-210, :302-353, :494-525)
+  void finalize_vit() {
+    const std::string Q = "detector.image_encoder.";
+    const int E = vd.embed_dim, G = d.img_size / kVitPatch;
+    auto shape_is = [](const HostTensor& t, std::vector<int64_t> s) { return t.shape == s; };
+    auto vec = [&](const std::string& k, int n) {
+      const HostTensor& t = get(k);
+      VSB_CHECK(t.numel() == n, k + ": expected " + std::to_string(n) + " values");
+      return wpool.upload(t.data);
+    };
+    {
+      const HostTensor& w = get(Q + "patch_embed.proj.weight");
+      VSB_CHECK(shape_is(w, {E, 3, kVitPatch, kVitPatch}), Q + "patch_embed.proj.weight: expected [embed_dim, 3, 16, 16]");
+      const HostTensor& b = get(Q + "patch_embed.proj.bias");
+      const HostTensor& pos = get(Q + "pos_embed");
+      if (!shape_is(pos, {1, G, G, E}))
+        throw Error(Q + "pos_embed: a " + std::to_string(G) + " x " + std::to_string(G) + " grid of " + std::to_string(E) +
+                    " is needed at img_size " + std::to_string(d.img_size), kErrInvalid);
+      // x*2-1 folded (extractor.py:64): W (2x - 1) + b = (2W) x + (b - sum W)
+      std::vector<float> wp(w.data.size()), table((size_t)G * G * E);
+      std::vector<double> bias(E);
+      for (int e = 0; e < E; ++e) {
+        double s = 0.0;
+        for (int k = 0; k < 768; ++k) { s += w.data[(size_t)e * 768 + k]; wp[(size_t)e * 768 + k] = 2.f * w.data[(size_t)e * 768 + k]; }
+        bias[e] = (double)b.data[e] - s;
+      }
+      for (int pidx = 0; pidx < G * G; ++pidx)
+        for (int e = 0; e < E; ++e) table[(size_t)pidx * E + e] = (float)((double)pos.data[(size_t)pidx * E + e] + bias[e]);
+      vit_patch.N = E; vit_patch.K = 768;
+      vit_patch.w = wpool.upload(to_half(wp));
+      vit_pos = wpool.upload(table);
+    }
+    for (int i = 0; i < vd.depth; ++i) {
+      const std::string B = Q + "blocks." + std::to_string(i) + ".";
+      VitBlockW w{};
+      w.n1w = vec(B + "norm1.weight", E); w.n1b = vec(B + "norm1.bias", E);
+      w.n2w = vec(B + "norm2.weight", E); w.n2b = vec(B + "norm2.bias", E);
+      auto lin = [&](const std::string& k, int N, int K, bool bias) {
+        VSB_CHECK(shape_is(get(k + ".weight"), {N, K}), k + ".weight: expected [" + std::to_string(N) + ", " + std::to_string(K) + "]");
+        return pack_conv(k + ".weight", nullptr, bias ? get(k + ".bias").data : std::vector<float>{});
+      };
+      w.qkv = lin(B + "attn.qkv", 3 * E, E, vd.qkv_bias != 0);
+      w.proj = lin(B + "attn.proj", E, E, true);
+      w.lin1 = lin(B + "mlp.lin1", vd.mlp_dim, E, true);
+      w.lin2 = lin(B + "mlp.lin2", E, vd.mlp_dim, true);
+      if (vd.use_rel_pos) {
+        const int n = (vd.global_mask >> i) & 1u ? G : vd.window_size;
+        auto rel = [&](const std::string& k) {
+          const HostTensor& t = get(k);
+          // the reference interpolates a table of another length (vit.py:398-428, for checkpoints of another size): not here
+          if (!shape_is(t, {2 * n - 1, kAttnHd}))
+            throw Error(k + ": expected [" + std::to_string(2 * n - 1) + ", 64] (2 * " + std::to_string(n) + " - 1 relative positions); "
+                        "tables of another length are not interpolated", kErrInvalid);
+          VSB_CHECK(n <= kAttnMaxRelSide, k + ": more than 63 relative positions (set_vit_extractor's rule)");
+          std::vector<float> p((size_t)kAttnTile * kAttnHd, 0.f);   // zero rows past 2n-1: the kernel reads whole 8-row tiles
+          std::copy(t.data.begin(), t.data.end(), p.begin());
+          return wpool.upload(to_half(p));
+        };
+        w.rel_h = rel(B + "attn.rel_pos_h");
+        w.rel_w = rel(B + "attn.rel_pos_w");
+      }
+      vit_blk.push_back(w);
+    }
+    const int oc = vd.out_chans;
+    VSB_CHECK(shape_is(get(Q + "neck.0.weight"), {oc, E, 1, 1}), Q + "neck.0.weight: expected [out_chans, embed_dim, 1, 1]");
+    VSB_CHECK(shape_is(get(Q + "neck.2.weight"), {oc, oc, 3, 3}), Q + "neck.2.weight: expected [out_chans, out_chans, 3, 3]");
+    vit_neck1 = pack_conv(Q + "neck.0.weight", nullptr, {});
+    vit_neck3 = pack_conv(Q + "neck.2.weight", nullptr, {}, nullptr, /*pad_taps=*/true);
+    vit_nln1w = vec(Q + "neck.1.weight", oc); vit_nln1b = vec(Q + "neck.1.bias", oc);
+    vit_nln2w = vec(Q + "neck.3.weight", oc); vit_nln2b = vec(Q + "neck.3.bias", oc);
+  }
+
+  // ---- extractor (ConvNeXt-V2)
+  void finalize_convnext() {
     const std::string Q = "detector.convnext.";
     {
       const HostTensor& w = get(Q + "downsample_layers.0.0.weight");  // [C0][3][4][4]
@@ -612,6 +735,10 @@ class Model {
         cn[s].push_back(w);
       }
     }
+  }
+
+  // ---- pixel decoder (pixel_decoder.py:44-83): pooled head or pixel-wise stages
+  void finalize_head() {
     if (pixelwise) {
       const std::string D = "detector.pixel_decoder.";
       for (size_t i = 0; i < pd.size(); ++i) {
@@ -639,8 +766,6 @@ class Model {
       head_lw = wpool.upload(lw.data);
       head_lb = wpool.upload(get(D + "linear.bias").data);
     }
-    sd.clear();  // host copies no longer needed
-    finalized = true;
   }
 
   // ---------------------------------------------------------------- plan building helpers
@@ -856,6 +981,10 @@ class Model {
     pl.x_res = pl.pool.alloc_n<float>((size_t)B * 3 * S * S);
     dbg(pl, "x_res", pl.x_res, 0, B, 3, S, S, S);
     pl.logits = pl.pool.alloc_n<float>((size_t)B * (1 + d.nbits));
+    if (vit) {
+      build_vit_trunk(pl, B);
+      return;
+    }
     const int st_ = d.ext_stem_stride;
     int hs = (S - 4) / st_ + 1;
     int C = d.ext_dims[0];
@@ -925,7 +1054,7 @@ class Model {
         {
           const float *lw = ds[s - 1].lnw, *lb = ds[s - 1].lnb, *xin = x;
           const int nsm = num_sms;
-          pl.steps.push_back(Step{[=](cudaStream_t st) { launch_ln_rows(xin, Mp, Cv, Cvp, lw, lb, xn, Cvp, nsm, st); }, 1, "cnx.ln_rows"});
+          pl.steps.push_back(Step{[=](cudaStream_t st) { launch_ln_rows(xin, Mp, Cv, Cvp, lw, lb, 1e-6f, xn, Cvp, nsm, st); }, 1, "cnx.ln_rows"});
         }
         const int ho = (hs - 2) / 2 + 1;   // odd maps (127, 63, 31): the last row / column is dropped, like nn.Conv2d k2 s2
         float* xo = pl.pool.alloc_n<float>((size_t)B * ho * ho * Cnp);
@@ -986,24 +1115,128 @@ class Model {
       }
       dbg(pl, "stage" + std::to_string(s), x, 0, B, hs, hs, C, Cp);
     }
-    // ---- head (pixel_decoder.py:61-83)
+    add_head(pl, x16, B, hs, C, Cp, "cnx.");
+  }
+
+  // ---- head (pixel_decoder.py:61-83) on the trunk's fp16 NHWC output x16 [B, hs, hs, C] (pixel pitch Cp)
+  void add_head(Plan& pl, const __half* x16, int B, int hs, int C, int Cp, const std::string& prefix) {
     if (pixelwise) {
       add_pixel_decoder(pl, x16, B, hs, Cp);
-    } else {
-      const long M = (long)B * hs * hs;
-      float* y = pl.pool.alloc_n<float>(M * Cp);
-      ConvGemmOp op;
-      setup_gather_conv(op, LD_GATHER_CONV, x16, Cp, Cp, nullptr, 0, 0, B, hs, hs, hs, hs, 3, 3, 1, 1, 1);
-      op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.out32 = y; op.p.ld_out32 = Cp;
-      add_conv(pl, op, head_conv, "cnx.head3x3." + std::to_string(C) + "@" + std::to_string(hs));
-      dbg(pl, "head_conv", y, 0, B, hs, hs, C, Cp);
-      float* pooled = pl.pool.alloc_n<float>((size_t)B * C);
-      const int P = hs * hs, Cc = C, ldy = Cp, NO = 1 + d.nbits;
-      const float *lw = head_lnw, *lb = head_lnb, *hw = head_lw, *hb = head_lb;
-      float* logits = pl.logits;
-      pl.steps.push_back(Step{[=](cudaStream_t st) { launch_head(y, B, P, Cc, ldy, lw, lb, pooled, hw, hb, NO, logits, st); }, 2,
-                              "cnx.head_tail"});
+      return;
     }
+    const long M = (long)B * hs * hs;
+    float* y = pl.pool.alloc_n<float>(M * Cp);
+    ConvGemmOp op;
+    setup_gather_conv(op, LD_GATHER_CONV, x16, Cp, Cp, nullptr, 0, 0, B, hs, hs, hs, hs, 3, 3, 1, 1, 1);
+    op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.out32 = y; op.p.ld_out32 = Cp;
+    add_conv(pl, op, head_conv, prefix + "head3x3." + std::to_string(C) + "@" + std::to_string(hs));
+    dbg(pl, "head_conv", y, 0, B, hs, hs, C, Cp);
+    float* pooled = pl.pool.alloc_n<float>((size_t)B * C);
+    const int P = hs * hs, Cc = C, ldy = Cp, NO = 1 + d.nbits;
+    const float *lw = head_lnw, *lb = head_lnb, *hw = head_lw, *hb = head_lb;
+    float* logits = pl.logits;
+    pl.steps.push_back(Step{[=](cudaStream_t st) { launch_head(y, B, P, Cc, ldy, lw, lb, pooled, hw, hb, NO, logits, st); }, 2,
+                            prefix + "head_tail"});
+  }
+
+  // SAM-ViT trunk (modules/vit.py:111-143) on the fp32 residual stream x [B*G*G][E] (token rows in raster order), ending in the
+  // fp16 [B, G, G, out_chans] map the head reads
+  void build_vit_trunk(Plan& pl, int B) {
+    Plan* plp = &pl;
+    const int S = d.img_size, G = S / kVitPatch, E = vd.embed_dim, H3 = 3 * E, MLP = vd.mlp_dim, oc = vd.out_chans, nsm = num_sms;
+    const long M = (long)B * G * G;
+    float* x = pl.pool.alloc_n<float>(M * E);
+    float* x0 = pl.pool.alloc_n<float>(M * E);         // patch embedding + position table: block 0 reads it, its proj writes x
+    __half* xn = pl.pool.alloc_n<__half>(M * E);       // LayerNorm output, the A operand of qkv / lin1
+    __half* qkv = pl.pool.alloc_n<__half>(M * H3);
+    __half* att = pl.pool.alloc_n<__half>(M * E);
+    __half* hid = pl.pool.alloc_n<__half>(M * MLP);
+    __half* x16 = pl.pool.alloc_n<__half>(M * E);      // fp16 copy of the last block's output: the neck's A operand
+    {
+      // patch embed (vit.py:494-525): im2col of the 16 x 16 patches, GEMM into the fp32 stream, + (pos_embed + folded bias)
+      __half* patches = pl.pool.alloc_n<__half>(M * 768);
+      pl.steps.push_back(Step{[=](cudaStream_t st) { launch_vit_patch_im2col(plp->in_imgs, B, S, patches, nsm, st); }, 1, "vit.patch"});
+      ConvGemmOp op; setup_tma_gemm(op, patches, M, 768, 768);
+      op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.out32 = x0; op.p.ld_out32 = E;
+      add_conv(pl, op, vit_patch, "vit.patch");
+      const float* table = vit_pos;
+      pl.steps.push_back(Step{[=](cudaStream_t st) { launch_vit_pos_add(x0, M, G * G, E, table, nsm, st); }, 1, "vit.patch"});
+      dbg(pl, "vit.embed", x0, 0, B, G, G, E, E);
+    }
+    for (int i = 0; i < vd.depth; ++i) {
+      const VitBlockW& w = vit_blk[i];
+      const std::string bi = "vit.blk" + std::to_string(i);
+      const bool global = (vd.global_mask >> i) & 1u;
+      const float* xin = i == 0 ? x0 : x;   // the block's input stream
+      {
+        const float *lw = w.n1w, *lb = w.n1b;
+        pl.steps.push_back(Step{[=](cudaStream_t st) { launch_ln_rows(xin, M, E, E, lw, lb, 1e-5f, xn, E, nsm, st); }, 1, "vit.ln"});
+      }
+      {
+        ConvGemmOp op; setup_tma_gemm(op, xn, M, E, E);
+        op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.bias = w.qkv.bias; op.p.out16 = qkv; op.p.ld_out16 = H3;
+        add_conv(pl, op, w.qkv, "vit.qkv");
+      }
+      {
+        AttnParams ap{};
+        ap.qkv = qkv; ap.out = att; ap.rel_h = w.rel_h; ap.rel_w = w.rel_w;
+        ap.G = G; ap.n = global ? G : vd.window_size; ap.heads = vd.num_heads; ap.E = E;
+        ap.regions = (G / ap.n) * (G / ap.n); ap.scale = 1.0f / std::sqrt((float)kAttnHd);
+        pl.steps.push_back(Step{[=](cudaStream_t st) { launch_vit_attention(ap, B, st); }, 1,
+                                global ? "vit.attn_global." + std::to_string(G * G) : "vit.attn_win." + std::to_string(ap.n * ap.n)});
+      }
+      {
+        ConvGemmOp op; setup_tma_gemm(op, att, M, E, E);
+        op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.bias = w.proj.bias; op.p.resid32 = xin; op.p.ld_res32 = E;
+        op.p.out32 = x; op.p.ld_out32 = E;   // in place after block 0: each element is read and written by the same thread
+        add_conv(pl, op, w.proj, "vit.proj");
+      }
+      {
+        const float *lw = w.n2w, *lb = w.n2b;
+        pl.steps.push_back(Step{[=](cudaStream_t st) { launch_ln_rows(x, M, E, E, lw, lb, 1e-5f, xn, E, nsm, st); }, 1, "vit.ln"});
+      }
+      {
+        ConvGemmOp op; setup_tma_gemm(op, xn, M, E, E);
+        op.p.epi = EPI_AFFINE; op.p.act = ACT_GELU; op.p.bias = w.lin1.bias; op.p.out16 = hid; op.p.ld_out16 = MLP;
+        add_conv(pl, op, w.lin1, "vit.lin1");
+      }
+      {
+        ConvGemmOp op; setup_tma_gemm(op, hid, M, MLP, MLP);
+        op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.bias = w.lin2.bias; op.p.resid32 = x; op.p.ld_res32 = E;
+        op.p.out32 = x; op.p.ld_out32 = E;
+        if (i + 1 == vd.depth) { op.p.out16 = x16; op.p.ld_out16 = E; }
+        add_conv(pl, op, w.lin2, "vit.lin2");
+      }
+      // the stream, qkv and att buffers are reused by every block, so they hold the LAST block's values after a run: only its taps
+      // exist.  Per-block copies would cost ~0.9 GB per 64-frame 256^2 plan; block k - 1 of a model is compared through the model
+      // of depth k built from the same checkpoint prefix (tests/test_vit_gpu.py)
+      if (i + 1 == vd.depth) {
+        dbg(pl, bi + ".qkv", qkv, 1, B, G, G, H3, H3);
+        dbg(pl, bi + ".attn", att, 1, B, G, G, E, E);
+        dbg(pl, bi, x, 0, B, G, G, E, E);
+      }
+    }
+    // neck (vit.py:90-109): 1x1 conv, LayerNorm2d, 3x3 conv (zero padding 1), LayerNorm2d; both without bias, eps 1e-6
+    float* y = pl.pool.alloc_n<float>(M * oc);
+    __half* yn = pl.pool.alloc_n<__half>(M * oc);
+    __half* out = pl.pool.alloc_n<__half>(M * oc);
+    {
+      ConvGemmOp op; setup_tma_gemm(op, x16, M, E, E);
+      op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.out32 = y; op.p.ld_out32 = oc;
+      add_conv(pl, op, vit_neck1, "vit.neck1x1");
+      const float *lw = vit_nln1w, *lb = vit_nln1b;
+      pl.steps.push_back(Step{[=](cudaStream_t st) { launch_ln_rows(y, M, oc, oc, lw, lb, 1e-6f, yn, oc, nsm, st); }, 1, "vit.neck_ln"});
+    }
+    {
+      ConvGemmOp op;
+      setup_gather_conv(op, LD_GATHER_CONV, yn, oc, oc, nullptr, 0, 0, B, G, G, G, G, 3, 3, 1, 1, 0);
+      op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.out32 = y; op.p.ld_out32 = oc;
+      add_conv(pl, op, vit_neck3, "vit.neck3x3");
+      const float *lw = vit_nln2w, *lb = vit_nln2b;
+      pl.steps.push_back(Step{[=](cudaStream_t st) { launch_ln_rows(y, M, oc, oc, lw, lb, 1e-6f, out, oc, nsm, st); }, 1, "vit.neck_ln"});
+    }
+    dbg(pl, "vit.neck", out, 1, B, G, G, oc, oc);
+    add_head(pl, out, B, G, oc, oc, "vit.");
   }
 
   // Pixel-wise decoder stages.  Each stage is one tensor-core GEMM at the LOW resolution, Y[p, tap*C_out + co] (the tap trick of the

@@ -113,10 +113,11 @@ inline void launch_stem_im2col(const float* imgs, int B, int S, int OH, int stri
   VSB_CUDA(cudaGetLastError());
 }
 
-inline void launch_ln_rows(const float* x, long M, int C, int ldx, const float* lnw, const float* lnb, __half* out, int ld_out,
+// eps: 1e-6 for the ConvNeXt downsample layers and the SAM-ViT neck, 1e-5 for the ViT blocks' nn.LayerNorm
+inline void launch_ln_rows(const float* x, long M, int C, int ldx, const float* lnw, const float* lnb, float eps, __half* out, int ld_out,
                            int num_sms, cudaStream_t st) {
   const int grid = (int)std::min<long>((M + 7) / 8, (long)num_sms * 16);
-  ln_rows_kernel<<<grid, 256, 0, st>>>(x, M, C, ldx, lnw, lnb, 1e-6f, out, ld_out);
+  ln_rows_kernel<<<grid, 256, 0, st>>>(x, M, C, ldx, lnw, lnb, eps, out, ld_out);
   VSB_CUDA(cudaGetLastError());
 }
 

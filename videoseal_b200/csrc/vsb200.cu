@@ -77,6 +77,15 @@ int vsb_model_set_pixel_decoder(vsb_model* m, int32_t n_stages, const int32_t* f
   VSB_API_END
 }
 
+int vsb_model_set_vit_extractor(vsb_model* m, const vsb_vit_desc* vit) {
+  VSB_API_BEGIN
+  VSB_CHECK(m != nullptr && vit != nullptr, "null argument");
+  std::lock_guard<std::recursive_mutex> lk(m->impl.mu);
+  m->impl.set_vit_extractor(*vit);
+  return VSB_OK;
+  VSB_API_END
+}
+
 int vsb_model_finalize(vsb_model* m, int32_t device) {
   VSB_API_BEGIN
   VSB_CHECK(m != nullptr, "null model");

@@ -34,23 +34,43 @@ def native_desc(spec: dict) -> _lib.ModelDesc:
     d.unet_act = acts[u["activation"]]
     d.unet_norm = 0 if u["normalization"].startswith("batch") else 1
     d.unet_last_tanh = int(u["last_tanh"])
-    cn = spec["convnext"]
-    for i in range(4):
-        d.ext_depths[i], d.ext_dims[i] = cn["depths"][i], cn["dims"][i]
-    d.ext_stem_stride = cn["stem_stride"]
+    cn = spec.get("convnext")     # a SAM-ViT spec leaves the ConvNeXt fields zero
+    if cn is not None:
+        for i in range(4):
+            d.ext_depths[i], d.ext_dims[i] = cn["depths"][i], cn["dims"][i]
+        d.ext_stem_stride = cn["stem_stride"]
     d.jnd_in_ch, d.jnd_out_ch = spec["jnd"]
     return d
 
 
+def native_vit_desc(vit: dict) -> _lib.VitDesc:
+    """vsb_vit_desc of spec['vit'] (cfg.spec_from_card)"""
+    v = _lib.VitDesc()
+    v.embed_dim, v.depth, v.num_heads = vit["embed_dim"], vit["depth"], vit["num_heads"]
+    v.patch_size, v.window_size = vit["patch_size"], vit["window_size"]
+    v.global_mask = sum(1 << i for i in set(vit["global_attn_indexes"]) if 0 <= i < 32)
+    v.mlp_dim, v.out_chans = vit["mlp_dim"], vit["out_chans"]
+    v.qkv_bias, v.use_rel_pos = int(vit["qkv_bias"]), int(vit["use_rel_pos"])
+    return v
+
+
+def trunk_map(spec: dict) -> int:
+    """side of the extractor trunk's output map: img_size / 16 tokens for a SAM-ViT, img_size / 32 for the ConvNeXt trunks"""
+    return spec["img_size"] // (16 if "vit" in spec else 32)
+
+
 def _create(spec: dict):
-    """Native handle of `spec` without weights or a device.  vsb_model_create and vsb_model_set_pixel_decoder check every rule the
-    kernels place on the model's geometry; a model they do not implement raises NotImplementedError."""
+    """Native handle of `spec` without weights or a device.  vsb_model_create, vsb_model_set_vit_extractor and
+    vsb_model_set_pixel_decoder check every rule the kernels place on the model's geometry; a model they do not implement raises
+    NotImplementedError."""
     L = _lib.lib()
     h = C.c_void_p()
     _lib.check(L.vsb_model_create(C.byref(native_desc(spec)), C.byref(h)))
     pd = spec.get("pixel_decoder", {"pixelwise": False})
     f = pd["upscale_stages"] if pd["pixelwise"] else None
-    rc = L.vsb_model_set_pixel_decoder(h, len(f), (C.c_int32 * len(f))(*f), 1) if f else 0
+    rc = L.vsb_model_set_vit_extractor(h, C.byref(native_vit_desc(spec["vit"]))) if "vit" in spec else 0
+    if rc == 0 and f:
+        rc = L.vsb_model_set_pixel_decoder(h, len(f), (C.c_int32 * len(f))(*f), 1)
     if rc != 0:
         L.vsb_model_destroy(h)
     _lib.check(rc)
@@ -176,6 +196,11 @@ class Videoseal(nn.Module):
         if v != self.spec["img_size"]:
             if v <= 0 or v % 128 != 0:
                 raise ValueError(f"img_size={v}: the native path needs a processing size that is a positive multiple of 128")
+            pos = self._sd.get("detector.image_encoder.pos_embed")
+            if "vit" in self.spec and pos is not None and pos.dim() == 4 and pos.shape[1] != v // 16:
+                # the reference fails here too (a shape error adding pos_embed in ImageEncoderViT.forward, vit.py:113-115)
+                raise ValueError(f"img_size={v}: this ViT extractor's pos_embed is a {pos.shape[1]} x {pos.shape[2]} grid, "
+                                 f"img_size / 16 = {v // 16} does not match")
             check_native({**self.spec, "img_size": v})
             self._respec(img_size=v)
 
@@ -321,8 +346,8 @@ class Videoseal(nn.Module):
 
     def _detect_dev(self, x: torch.Tensor, antialias: bool) -> torch.Tensor:
         shape = (x.shape[0], 1 + self.spec["nbits"])
-        if self.pixelwise:   # trunk map (img_size / 32) x the product of the stage factors: img_size for [4, 4, 2]
-            P = self.spec["img_size"] // 32
+        if self.pixelwise:   # trunk map (img_size / 32, a ViT's img_size / 16) x the product of the stage factors
+            P = trunk_map(self.spec)
             for f in self.spec["pixel_decoder"]["upscale_stages"]:
                 P *= f
             shape += (P, P)
