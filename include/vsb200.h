@@ -207,6 +207,9 @@ typedef struct vsb_conv_test {
   int32_t ld0;               /* pixel pitch of src0 in elements (0 = C0): widths that are not multiples of 8 live in padded rows */
   int32_t ldw;               /* row pitch of the weights (0 = K) */
   int32_t ld_out;            /* row pitch of out16 / out32 / resid32 (0 = N) */
+  int32_t kernel;            /* tensor-core loaders: 0 = the kernel the library selects, 1 = force the 128-row kernel, 2 = force the
+                              * 256-row long-K kernel (an error unless the op is one it can run) */
+  int32_t* kernel_ran;       /* if not null (host memory): receives 1 or 2, the kernel this call launched */
 } vsb_conv_test;
 int vsb_debug_conv(const vsb_conv_test* t, void* stream);
 /* host-only (no GPU needed): the separable table the resize kernels use along one axis of length `in` -> `out`, i.e. the library's

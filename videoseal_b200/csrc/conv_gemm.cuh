@@ -1066,4 +1066,218 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   __syncthreads();
 }
 
+// ------------------------------------------------------------------------------------------------------------------------------
+// Long-K variant of the LD_TMA kernel: 256 x BN output tiles, the accumulators stay in registers through the epilogue.
+//
+//   warpgroup 0    : producer; gives its registers away (setmaxnreg) and one elected thread runs the TMA loop: per K block of 64
+//                    a [256 x 64] A tile (one box: tile_h x tile_w = 256 pixels of the map, or 256 GEMM rows) and a [BN x 64] B tile
+//   warpgroups 1,2 : consumers; warpgroup h owns rows [128h, 128h + 128) of the tile as two m64 wgmma chains that read the same B
+//                    tile, 2 x BN / 2 accumulators per thread, and runs the epilogue of its rows straight from the fragments:
+//                    acc + bias -> ReLU -> + fp16 residual -> clamp -> fp16, staged per warp in swizzled [16 rows] boxes that leave
+//                    through TMA stores
+//
+// Against the 128-row kernel a K block moves 48 KB instead of 2 x 32 KB from L2 for the same 4.2 MFLOP, a pipeline stage is worth
+// twice the MMA time, and no accumulator crosses shared memory.  The price: a warpgroup's epilogue does not overlap its own next
+// main loop (the producer keeps filling the ring meanwhile), so finalize_op selects this kernel for long main loops only.  The
+// K-block order, the k16 order inside a block and the epilogue arithmetic are those of conv_gemm_kernel's lean affine path: both
+// kernels produce the same bits.
+constexpr int kLongM = 256;
+constexpr int kLongThreads = 384;
+constexpr int kLongHeaderBytes = 1024;                // full / empty barriers
+constexpr uint32_t kLongOstWarpBytes = 16 * kMaxBlockN * 2;   // staging of one consumer warp: one chain's [16 rows][BN] fp16
+constexpr int kLongConsumerWarps = 8;
+
+// read-only global loads that keep their place among the barrier / wgmma statements
+__device__ __forceinline__ uint32_t ld_nc_u32(const void* g) {
+  uint32_t v;
+  asm volatile("ld.global.nc.b32 %0, [%1];" : "=r"(v) : "l"(g));
+  return v;
+}
+__device__ __forceinline__ float2 ld_nc_f32x2(const float* g) {
+  float2 v;
+  asm volatile("ld.global.nc.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(g));
+  return v;
+}
+
+template <int BN, int ACT>
+__global__ void __launch_bounds__(kLongThreads, 1)
+conv_gemm_longk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                       const __grid_constant__ CUtensorMap tmO, const __grid_constant__ ConvGemmParams p) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem);
+  uint64_t* empty_bar = full_bar + kMaxStages;
+  uint8_t* tiles = smem + kLongHeaderBytes;
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < p.stages; ++s) {
+      mbar_init(&full_bar[s], 1u);
+      mbar_init(&empty_bar[s], (uint32_t)kLongConsumerWarps);
+    }
+    fence_barrier_init();
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    tma_prefetch_desc(&tmO);
+  }
+  __syncthreads();
+  // nothing above reads or writes a tensor produced by an earlier kernel
+  pdl_launch_dependents();
+  pdl_wait();
+
+  if (warp < 4) {
+    // ===================================================================== TMA producer
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        const int m_tile = p.fd_ntiles.div(tile), brow = (tile - m_tile * p.n_tiles) * BN;
+        int cb = 0, cx = 0, cy = 0;
+        if (p.a_is_conv) {
+          cb = p.fd_tpi.div(m_tile);
+          const int rem = m_tile - cb * p.tiles_per_img;
+          const int ty = p.fd_tx.div(rem);
+          cy = ty * p.tile_h;
+          cx = (rem - ty * p.tiles_x) * p.tile_w;
+        }
+        int tap_r = 0, tap_s = 0, cblk = 0;
+        for (int kb = 0; kb < p.num_kb; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1u);
+          uint8_t* sa = tiles + (size_t)stage * p.stage_bytes;
+          mbar_arrive_expect_tx(&full_bar[stage], p.a_stage_bytes + p.b_stage_bytes);
+          if (p.a_is_conv) {
+            tma_load_4d(&tmA, &full_bar[stage], sa, cblk * 64, cx + tap_s - p.pad, cy + tap_r - p.pad, cb);
+            if (++cblk == p.c_blocks) { cblk = 0; if (++tap_s == p.S) { tap_s = 0; ++tap_r; } }
+          } else {
+            tma_load_2d(&tmA, &full_bar[stage], sa, kb * 64, m_tile * kLongM);
+          }
+          tma_load_2d(&tmB, &full_bar[stage], sa + p.a_stage_bytes, kb * 64, brow);
+          if (++stage == p.stages) { stage = 0; phase ^= 1u; }
+        }
+      }
+    }
+  } else {
+    // ===================================================================== consumers: MMA + epilogue of rows [128h, 128h + 128)
+    setmaxnreg_inc<232>();
+    const int h = (warp >> 2) - 1, wq = warp & 3;
+    const int rl = lane >> 2, q = lane & 3;
+    // staging boxes of this warp: [16 rows][kBoxCols] fp16 in the TMA swizzle of that row width; fragment row rl and rl + 8 share
+    // the XOR term, and the 4-byte stores of a warp instruction (8 rows x 4 lanes) fall into 32 different banks
+    constexpr int kBoxCols = BN % 64 == 0 ? 64 : 16;
+    constexpr uint32_t kBoxRowB = kBoxCols * 2, kBoxBytes = 16 * kBoxRowB;
+    const uint32_t swz_x = kBoxCols == 64 ? (uint32_t)rl : (uint32_t)((rl >> 2) & 1);
+    uint8_t* ost = smem + p.ostage_off + (size_t)(warp - 4) * kLongOstWarpBytes;
+    const bool has_res = p.resid16 != nullptr;
+    constexpr uint32_t kRowBytes = 128;                           // K block of 64 fp16
+    const uint32_t a_off = (uint32_t)h * 128u * kRowBytes;
+    float d[2][BN / 2];
+    // The epilogue walks the 2 x BN / 8 eight-column groups of the two chains in kGrp-sized steps; the bias pairs and residual
+    // half2 of step t + 1 are loaded while step t is converted.  Only two steps' worth sit in registers beside the 2 x BN / 2
+    // accumulators (the whole tile's would not fit), and the loads are ordered statements so that they stay where they are put.
+    constexpr int kGrp = BN % 32 == 0 ? 4 : 5, kSteps = BN / 8 / kGrp;     // steps per chain
+    static_assert(kGrp * kSteps * 8 == BN, "block_n must split into whole epilogue steps");
+    float2 gb0[kGrp], gb1[kGrp];
+    uint32_t gr0[2 * kGrp], gr1[2 * kGrp];
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+      const int m_tile = p.fd_ntiles.div(tile), n0 = (tile - m_tile * p.n_tiles) * BN;
+      const long m_warp = (long)m_tile * kLongM + h * 128 + wq * 16;     // first row of this warp's chain-0 fragment
+      int prev = -1;
+      for (int kb = 0; kb < p.num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(tiles + (size_t)stage * p.stage_bytes);
+        const uint64_t adesc0 = make_smem_desc(sa + a_off, kRowBytes);
+        const uint64_t adesc1 = make_smem_desc(sa + a_off + 64u * kRowBytes, kRowBytes);
+        const uint64_t bdesc = make_smem_desc(sa + p.a_stage_bytes, kRowBytes);
+        wgmma_fence_regs(d[0]);
+        wgmma_fence_regs(d[1]);
+        wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          // advance 16 K-elements = 32 bytes inside the swizzled row: +2 in the (addr >> 4) field
+          Wgmma<BN>::mma(d[0], adesc0 + (uint64_t)(2 * j), bdesc + (uint64_t)(2 * j), (uint32_t)((kb | j) != 0));
+          Wgmma<BN>::mma(d[1], adesc1 + (uint64_t)(2 * j), bdesc + (uint64_t)(2 * j), (uint32_t)((kb | j) != 0));
+        }
+        wgmma_commit();
+        wgmma_fence_regs(d[0]);
+        wgmma_fence_regs(d[1]);
+        if (prev >= 0) {
+          wgmma_wait<1>();   // the previous K-block's wgmma have read their slot
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        }
+        prev = stage;
+        if (++stage == p.stages) { stage = 0; phase ^= 1u; }
+      }
+      auto load_step = [&](float2 (&gb)[kGrp], uint32_t (&gr)[2 * kGrp], int t) {
+        const int c = t / kSteps, j0 = (t % kSteps) * kGrp;
+        const __half* r0 = p.resid16 + (m_warp + 64 * c + rl) * p.ld_res16 + n0 + 8 * j0 + 2 * q;
+        const __half* r1 = r0 + 8 * (long)p.ld_res16;
+#pragma unroll
+        for (int jj = 0; jj < kGrp; ++jj) {
+          gb[jj] = p.bias != nullptr ? ld_nc_f32x2(p.bias + n0 + 8 * (j0 + jj) + 2 * q) : make_float2(0.f, 0.f);
+          if (has_res) {
+            gr[2 * jj] = ld_nc_u32(r0 + 8 * jj);
+            gr[2 * jj + 1] = ld_nc_u32(r1 + 8 * jj);
+          }
+        }
+      };
+      load_step(gb0, gr0, 0);       // in flight while the last wgmma group drains
+      wgmma_wait<0>();
+      wgmma_fence_regs(d[0]);
+      wgmma_fence_regs(d[1]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+#pragma unroll
+      for (int t = 0; t < 2 * kSteps; ++t) {
+        const int c = t / kSteps, g = t % kSteps;
+        if (g == 0) {
+          if (lane == 0) bulk_wait_group_read0();     // the previous stores of this warp have finished reading the staging boxes
+          __syncwarp();
+        }
+        auto convert_step = [&](const float2 (&gb)[kGrp], const uint32_t (&gr)[2 * kGrp]) {
+#pragma unroll
+          for (int jj = 0; jj < kGrp; ++jj) {
+            const int j = g * kGrp + jj;
+            uint8_t* obox = ost + (uint32_t)((8 * j) / kBoxCols) * kBoxBytes + ((((uint32_t)((8 * j) % kBoxCols) >> 3) ^ swz_x) << 4) + 4u * q;
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+              float v0 = d[c][4 * j + 2 * hh] + gb[jj].x, v1 = d[c][4 * j + 2 * hh + 1] + gb[jj].y;
+              if (ACT == ACT_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+              if (has_res) {
+                const uint32_t rbits = gr[2 * jj + hh];
+                const float2 rf = __half22float2(*reinterpret_cast<const __half2*>(&rbits));
+                v0 += rf.x; v1 += rf.y;
+              }
+              v0 = fminf(v0, 65504.f); v1 = fminf(v1, 65504.f);
+              if (ACT == ACT_NONE || has_res) { v0 = fmaxf(v0, -65504.f); v1 = fmaxf(v1, -65504.f); }   // ReLU >= 0
+              *reinterpret_cast<__half2*>(obox + (uint32_t)(rl + 8 * hh) * kBoxRowB) = __floats2half2_rn(v0, v1);
+            }
+          }
+        };
+        if ((t & 1) == 0) {
+          if (t + 1 < 2 * kSteps) load_step(gb1, gr1, t + 1);
+          convert_step(gb0, gr0);
+        } else {
+          if (t + 1 < 2 * kSteps) load_step(gb0, gr0, t + 1);
+          convert_step(gb1, gr1);
+        }
+        if (g == kSteps - 1) {
+          fence_proxy_async_smem();     // generic-proxy writes of the staging boxes -> async proxy
+          __syncwarp();
+          if (lane == 0) {
+#pragma unroll
+            for (int b = 0; b < BN / kBoxCols; ++b) tma_store_2d(&tmO, ost + b * kBoxBytes, n0 + b * kBoxCols, (int)(m_warp + 64 * c));
+            bulk_commit_group();
+          }
+        }
+      }
+    }
+    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // all stores of this warp have landed
+  }
+}
+
 }  // namespace vsb

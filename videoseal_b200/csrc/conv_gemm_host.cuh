@@ -116,6 +116,12 @@ struct ConvGemmOp {
   int w_samples = 1;   // > 1: weights are [w_samples][N][K], sample = row / rows_per_sample (finalize_op)
   size_t smem = 0;
   const char* name = "";
+  // the A operand as setup_tma_conv / setup_tma_gemm encoded it (a_rank 4 / 2; 0: another loader or the two-source GEMM), kept so
+  // that finalize_op can encode the same tensor with the 256-row box of the long-K kernel
+  const void* a_base = nullptr;
+  int a_rank = 0;
+  uint64_t a_dims[4] = {0, 0, 0, 0}, a_strides[3] = {0, 0, 0};
+  int longk = 0;       // 1: conv_gemm_longk_kernel runs this op (finalize_op)
   ConvGemmOp() { memset(&p, 0, sizeof(p)); memset(&tmA, 0, sizeof(tmA)); memset(&tmA2, 0, sizeof(tmA2)); memset(&tmB, 0, sizeof(tmB)); memset(&tmO, 0, sizeof(tmO)); }
 };
 
@@ -128,9 +134,76 @@ inline int pick_block_n(int N, int max_bn = kMaxBlockN) {
   return max_bn / 16 * 16;
 }
 
+// ---- the long-K kernel (conv_gemm_longk_kernel): which ops may run on it, and its tiling / shared-memory plan
+enum : int { kKernelAuto = 0, kKernel128 = 1, kKernelLongK = 2 };   // kernel_sel of finalize_op (1, 2: test seam of vsb_debug_conv)
+
+// 256-pixel patch of an H x W map as one TMA box (each box dimension <= 256); false when the map does not tile by it
+inline bool longk_conv_tile(int H, int W, int& tile_w, int& tile_h) {
+  tile_w = W < kLongM ? W : kLongM;
+  tile_h = kLongM / tile_w;
+  return tile_w * tile_h == kLongM && W % tile_w == 0 && H % tile_h == 0;
+}
+
+// Everything but the tile count: a TMA-fed op with a long main loop whose epilogue is the lean affine one (bias, ReLU or none,
+// optional fp16 residual, fp16 output), in whole 256 x block_n tiles of a width the kernel is instantiated for.
+inline bool longk_eligible(const ConvGemmOp& op, int N) {
+  const ConvGemmParams& p = op.p;
+  int tw, th;
+  return op.loader == LD_TMA && op.a_rank != 0 && op.w_samples == 1 && p.kblk == 64 && p.num_kb >= 24 &&
+         p.epi == EPI_AFFINE && (p.act == ACT_NONE || p.act == ACT_RELU) &&
+         p.out16 != nullptr && p.out32 == nullptr && p.resid32 == nullptr && p.outc_w == nullptr && p.grn_stats == nullptr &&
+         (reinterpret_cast<uintptr_t>(p.out16) & 15) == 0 && p.ld_out16 % 8 == 0 && (reinterpret_cast<uintptr_t>(p.bias) & 7) == 0 &&
+         (p.resid16 == nullptr || ((reinterpret_cast<uintptr_t>(p.resid16) & 3) == 0 && p.ld_res16 % 8 == 0)) &&
+         (p.block_n == 128 || p.block_n == 80) && N % p.block_n == 0 && p.M % kLongM == 0 &&
+         (!p.a_is_conv || longk_conv_tile(p.H, p.W, tw, th));
+}
+
+inline void finalize_longk(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw, int num_sms) {
+  ConvGemmParams& p = op.p;
+  op.longk = 1;
+  p.group = 1;
+  p.m_tiles = p.M / kLongM;
+  p.num_tiles = p.m_tiles * p.n_tiles;
+  uint32_t abox[4] = {64u, (uint32_t)kLongM, 1u, 1u};
+  if (p.a_is_conv) {
+    longk_conv_tile(p.H, p.W, p.tile_w, p.tile_h);
+    p.tiles_x = p.W / p.tile_w;
+    p.tiles_per_img = p.tiles_x * (p.H / p.tile_h);
+    abox[1] = (uint32_t)p.tile_w; abox[2] = (uint32_t)p.tile_h;
+  }
+  encode_map(&op.tmA, op.a_base, op.a_rank, op.a_dims, op.a_strides, abox, 64);
+  p.fd_ntiles = make_fastdiv(p.n_tiles); p.fd_tpi = make_fastdiv(p.tiles_per_img); p.fd_tx = make_fastdiv(p.tiles_x);
+  p.a_stage_bytes = (uint32_t)(kLongM * 64 * 2);
+  p.b_stage_bytes = (uint32_t)(p.block_n * 64 * 2);
+  p.stage_bytes = p.a_stage_bytes + ((p.b_stage_bytes + 1023u) & ~1023u);
+  // shared memory: [barriers | stages x (A|B) | staging boxes of the 8 consumer warps]; 4 stages of 48 KB at block_n 128
+  const size_t ostage_total = (size_t)kLongConsumerWarps * kLongOstWarpBytes;
+  int stages = (int)((226 * 1024 - kLongHeaderBytes - ostage_total) / p.stage_bytes);
+  if (stages > kMaxStages) stages = kMaxStages;
+  VSB_CHECK(stages >= 3, "long-K tile does not fit in shared memory");
+  p.stages = stages;
+  p.ostage_off = (uint32_t)(kLongHeaderBytes + (size_t)stages * p.stage_bytes);
+  op.smem = 1024 /*align slack*/ + p.ostage_off + ostage_total;
+  {  // output map [M rows][N cols]; box = one staging box: 16 fragment rows x 64 columns (128-byte swizzle) or x 16 (32-byte swizzle)
+    const int box_cols = p.block_n % 64 == 0 ? 64 : 16;
+    uint64_t odims[2] = {(uint64_t)N, (uint64_t)p.M};
+    uint64_t ostrides[1] = {(uint64_t)p.ld_out16 * 2};
+    uint32_t obox[2] = {(uint32_t)box_cols, 16u};
+    encode_map(&op.tmO, p.out16, 2, odims, ostrides, obox, 0, /*no_swizzle=*/true, false, box_cols * 2);
+  }
+  uint64_t dims[2] = {(uint64_t)Kw, (uint64_t)N};
+  uint64_t strides[1] = {(uint64_t)ldw * 2};
+  uint32_t box[2] = {64u, (uint32_t)p.block_n};
+  encode_map(&op.tmB, W, 2, dims, strides, box, 64);
+  op.grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
+  op.threads = kLongThreads;
+  VSB_CHECK((long)p.M < (1L << 31), "M too large for 32-bit row indices");
+}
+
 // Common finalisation: weights map, tiling, stage count, smem, grid.
 // W: [N, Kw] fp16 row-major (K-major), Kw >= num_kb*kblk need not hold (TMA zero-fills out-of-bounds K).
-inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw, int num_sms, int block_n_override = 0) {
+inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw, int num_sms, int block_n_override = 0,
+                        int kernel_sel = kKernelAuto) {
   ConvGemmParams& p = op.p;
   p.N = N;
   // block_n <= 128: the two MMA warpgroups hold a 128 x block_n fp32 accumulator in registers (block_n / 2 per thread); an fp32
@@ -138,6 +211,17 @@ inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw,
   p.block_n = block_n_override ? block_n_override : pick_block_n(N, p.resid32 ? 64 : kMaxBlockN);
   VSB_CHECK(p.block_n % 16 == 0 && p.block_n >= 16 && p.block_n <= kMaxBlockN, "bad block_n");
   p.n_tiles = (N + p.block_n - 1) / p.block_n;
+  {
+    // Long main loops run on 256-row tiles when there are at least two of them per SM.  Below that the 128-row kernel fills the
+    // machine better: it has twice the tiles to spread, and the last wave of 256-row tiles would leave SMs idle for a whole
+    // 256-row main loop.  (Not measured below the threshold; the bottleneck convs at 64 frames have 5.8 tiles per SM.)
+    const bool eligible = longk_eligible(op, N);
+    VSB_CHECK(kernel_sel != kKernelLongK || eligible, "the long-K kernel cannot run this op");
+    if (eligible && kernel_sel != kKernel128 && (kernel_sel == kKernelLongK || (long)(p.M / kLongM) * p.n_tiles >= 2L * num_sms)) {
+      finalize_longk(op, W, N, Kw, ldw, num_sms);
+      return;
+    }
+  }
   // small-N layers: several consecutive M tiles share one accumulator round (columns g*block_n of the accumulator tile) so that
   // the per-tile barrier handshakes / index math are amortised
   p.group = p.block_n <= 32 ? kAccCols / p.block_n : 1;
@@ -291,6 +375,9 @@ inline void setup_tma_conv(ConvGemmOp& op, const __half* src, int B, int H, int 
   uint64_t strides[3] = {(uint64_t)ld * 2, (uint64_t)W * ld * 2, (uint64_t)H * W * ld * 2};
   uint32_t box[4] = {(uint32_t)p.kblk, (uint32_t)p.tile_w, (uint32_t)p.tile_h, 1u};
   encode_map(&op.tmA, src, 4, dims, strides, box, p.kblk);
+  op.a_base = src; op.a_rank = 4;
+  for (int i = 0; i < 4; ++i) op.a_dims[i] = dims[i];
+  for (int i = 0; i < 3; ++i) op.a_strides[i] = strides[i];
 }
 
 
@@ -349,6 +436,8 @@ inline void setup_tma_gemm(ConvGemmOp& op, const __half* A, long M, int K, int l
   uint64_t strides[1] = {(uint64_t)ld * 2};
   uint32_t box[2] = {(uint32_t)p.kblk, (uint32_t)kBlockM};
   encode_map(&op.tmA, A, 2, dims, strides, box, p.kblk);
+  op.a_base = A; op.a_rank = 2;
+  op.a_dims[0] = dims[0]; op.a_dims[1] = dims[1]; op.a_strides[0] = strides[0];
 }
 
 // A = [A0 | A1] virtual concat along K of two [M, K0] / [M, K1] fp16 matrices (row pitches ld0 / ld1)
@@ -429,9 +518,21 @@ inline void launch_one(const ConvGemmOp& op, cudaStream_t st) {
   launch_pdl(conv_gemm_kernel<LOADER, ACT>, dim3(op.grid), dim3(op.threads), op.smem, st, op.tmA, op.tmA2, op.tmB, op.tmO, op.p);
 }
 
+template <int BN, int ACT>
+inline void launch_longk(const ConvGemmOp& op, cudaStream_t st) {
+  smem_optin<conv_gemm_longk_kernel<BN, ACT>>(227 * 1024);
+  launch_pdl(conv_gemm_longk_kernel<BN, ACT>, dim3(op.grid), dim3(op.threads), op.smem, st, op.tmA, op.tmB, op.tmO, op.p);
+}
+
 // instantiated (loader, activation) pairs: only what the networks need, to bound compile time
 inline void launch(const ConvGemmOp& op, cudaStream_t st) {
   const int a = op.p.act;
+  if (op.longk) {   // block_n 128 / 80 and ReLU / none: longk_eligible
+    if (op.p.block_n == 128) { if (a == ACT_RELU) launch_longk<128, ACT_RELU>(op, st); else launch_longk<128, ACT_NONE>(op, st); }
+    else { if (a == ACT_RELU) launch_longk<80, ACT_RELU>(op, st); else launch_longk<80, ACT_NONE>(op, st); }
+    VSB_CUDA(cudaGetLastError());
+    return;
+  }
   switch (op.loader) {
     case LD_TMA:
       if (a == ACT_NONE) launch_one<LD_TMA, ACT_NONE>(op, st);

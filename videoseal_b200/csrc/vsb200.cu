@@ -333,7 +333,9 @@ int vsb_debug_conv(const vsb_conv_test* t, void* stream) {
   p.outc_w = t->outc_w; p.outc_b = t->outc_b; p.n_out = t->n_out; p.delta = t->delta; p.hw = OH * OW; p.outc_tanh = 1;
   p.grn_stats = t->grn_stats;
   if (t->rows_per_sample) p.rows_per_sample = t->rows_per_sample;
-  finalize_op(op, (const __half*)t->weights, t->N, K, t->ldw ? t->ldw : K, num_sms, t->block_n);
+  VSB_CHECK(t->kernel >= kKernelAuto && t->kernel <= kKernelLongK, "bad kernel selector");
+  finalize_op(op, (const __half*)t->weights, t->N, K, t->ldw ? t->ldw : K, num_sms, t->block_n, t->kernel);
+  if (t->kernel_ran) *t->kernel_ran = op.longk ? kKernelLongK : kKernel128;
   launch(op, (cudaStream_t)stream);
   g_launches += 1;
   return VSB_OK;
