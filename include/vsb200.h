@@ -183,6 +183,18 @@ int vsb_ssim(const float* x_dev, const float* y_dev, int32_t B, int32_t C, int32
 /* copy a named intermediate activation of the most recent embed/detect sub-batch to the host as fp32.
  * shape4 receives [B, H, W, C] (NHWC) or [M, C, 1, 1]-style dims; returns the element count or <0. */
 int64_t vsb_debug_get_tensor(vsb_model* m, const char* name, float* host_out, int64_t capacity, int64_t* shape4);
+/* ConvNeXt detect plans: on != 0 adds device-to-device copies of the fp32 residual stream where the blocks read it, so that each
+ * kernel can be checked on its own inputs.  The stream is updated in place by every block's pwconv2, so without them the input
+ * of a block is kept nowhere.  Taps while on (s = 0..3):
+ *   s{s}_ds   the stream right after the stem (s = 0) or the down conv of stage s
+ *   s{s}_in   the stream right before the stage's last block (the same copy as s{s}_ds at depth 1)
+ * The copies only read the stream: the logits are bit-identical with the seam on and off.  Setting it drops the cached detect
+ * plans; off (the default), the plans are built exactly as without the seam.  Taps in every ConvNeXt detect plan:
+ *   s{s}_ln (s >= 1) the fp16 LayerNorm'd rows the down conv reads;  s{s}_a / s{s}_g  the last block's dwconv + LN output and
+ *   its pwconv1 + GELU output (after the in-place GRN on stages that apply it);  s{s}_w2s  [B, C, 1, 4C] the per-sample GRN-scaled
+ *   W2 of stages that fold GRN into the weights;  stage{s}  the stream after stage s;  stage3_16  its fp16 copy the head conv
+ *   reads;  head_conv;  head_pooled  [B, 1, 1, C] the LayerNorm + GELU + mean the linear head reads. */
+int vsb_debug_keep_inputs(vsb_model* m, int32_t on);
 /* which compiled variant the most recent launch of each full-resolution kernel used (host state, no synchronisation):
  *   out[0..4]  resize_sep_kernel:  MT (x taps in registers: 2, 8, or 0 = any count), GST (input rows per staging round: 4, 2, 1),
  *              vec (1 = bulk copies, 0 = 4-byte cp.async), toy (output rows per block), OW (output width = img_size)

@@ -76,19 +76,9 @@ def net_walk(card):
     taps = {}
     ref_logits = orc.detector(ref["imgs_w"], taps)
     got_logits = model.detect(ref["imgs_w"].cuda(), is_video=False)["preds"].cpu()
+    # per-block kernels are judged on their own inputs by tests/test_cnx_kernels_gpu.py
     for s in range(4):
-        cmp(f"ds{s}", taps[f"ds{s}"])
         cmp(f"stage{s}", taps[f"stage{s}"])
-    # first block of every stage, its LayerNorm'd dwconv output and its GELU output (oracle recomputed from the stage input)
-    import torch.nn.functional as F
-    for s in range(4):
-        key = f"detector.convnext.stages.{s}.0."
-        xin = taps[f"ds{s}"]
-        C = xin.shape[1]
-        a = F.conv2d(xin, orc.sd[key + "dwconv.weight"], orc.sd[key + "dwconv.bias"], padding=3, groups=C).permute(0, 2, 3, 1)
-        a = F.layer_norm(a, (C,), orc.sd[key + "norm.weight"], orc.sd[key + "norm.bias"], 1e-6)
-        cmp(f"s{s}b0_a", a.permute(0, 3, 1, 2))
-        cmp(f"s{s}b0_g", F.gelu(F.linear(a, orc.sd[key + "pwconv1.weight"], orc.sd[key + "pwconv1.bias"])).permute(0, 3, 1, 2))
     err = (got_logits - ref_logits).abs()
     rows.append({"tensor": "logits", "maxerr": err.max().item(), "ref_absmax": ref_logits.abs().max().item(),
                  "bit_mismatch": int(((got_logits[:, 1:] > 0) != (ref_logits[:, 1:] > 0)).sum())})

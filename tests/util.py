@@ -59,6 +59,9 @@ def apply_overrides(card: dict, o: dict) -> dict:
         card["embedder"]["params"]["unet"]["num_blocks"] = o["num_blocks"]
     if "attenuation" in o:
         card["args"]["attenuation"] = o["attenuation"]
+    if "extractor" in o:   # a preset of configs/extractor.yaml in place of the card's extractor
+        ext = yaml.safe_load(open(Path(ROOT) / "videoseal_b200" / "configs" / "extractor.yaml"))
+        card["extractor"] = {"model": o["extractor"], "params": copy.deepcopy(ext[o["extractor"]])}
     if "depths" in o:
         card["extractor"]["params"]["encoder"]["depths"] = o["depths"]
     return card

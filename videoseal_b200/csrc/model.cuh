@@ -172,6 +172,13 @@ class Model {
   //   resize: MT, GST, vec, toy, OW       blend: 3 (jnd_blend3_kernel) or 2 (jnd_blend2_kernel), VEC, FASTUP, CD, JIN
   int32_t last_resize[5] = {-1, -1, -1, -1, -1};
   int32_t last_blend[5] = {-1, -1, -1, -1, -1};
+  // test seam (vsb_debug_keep_inputs): detect plans copy the ConvNeXt residual stream aside where the blocks read it
+  bool keep_inputs = false;
+  void set_keep_inputs(bool on) {
+    keep_inputs = on;
+    for (auto& kv : detect_plans) if (kv.second.get() == last_plan) last_plan = nullptr;
+    detect_plans.clear();
+  }
 
   explicit Model(const vsb_model_desc& desc) : d(desc) { check_desc(); }
 
@@ -1000,7 +1007,6 @@ class Model {
       const float *wk = stem_wk, *sb = stem_b, *lw = stem_lnw, *lb = stem_lnb;
       pl.steps.push_back(Step{[=](cudaStream_t st) { launch_stem_ln(plp->in_imgs, B, S, OH, st_, wk, sb, lw, lb, Cc, x, ldo, nsm, st); }, 1,
                               "cnx.stem_ln." + std::to_string(C) + "@" + std::to_string(hs)});
-      dbg(pl, "ds0", x, 0, B, hs, hs, C, Cp);
     } else {
       // stem (convnext.py:108-111): im2col of the k4 patches (x = 2*img-1 folded) -> tensor-core GEMM [M,64]x[64,C0] with the
       // conv bias and the channels-first LayerNorm fused into the epilogue, fp32 NHWC output (the residual stream)
@@ -1014,8 +1020,17 @@ class Model {
       op.p.out32 = x; op.p.ld_out32 = Cp;
       ConvW sw; sw.w = stem_w16; sw.N = C; sw.K = 64; sw.bias = stem_b;
       add_conv(pl, op, sw, "cnx.stem_gemm." + std::to_string(C) + "@" + std::to_string(hs));
-      dbg(pl, "ds0", x, 0, B, hs, hs, C, Cp);
     }
+    // keep_inputs (vsb_debug_keep_inputs): the residual stream is updated in place by every block, so the values a stage's first
+    // and last blocks read are copied aside as they pass: s{s}_ds after the stem / down conv, s{s}_in before the last block
+    auto keep = [&](const std::string& name, const float* src, int h, int c, int cp) {
+      const size_t bytes = (size_t)B * h * h * cp * sizeof(float);
+      float* dst = pl.pool.alloc_n<float>((size_t)B * h * h * cp);
+      pl.steps.push_back(Step{[=](cudaStream_t st) { VSB_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st)); }, 0,
+                              "dbg.keep." + name});
+      dbg(pl, name, dst, 0, B, h, h, c, cp);
+      return dst;
+    };
     int maxK4 = 0;
     for (int s = 0; s < 4; ++s) maxK4 = std::max(maxK4, 4 * d.ext_dims[s]);
     // GRN statistics ping-pong: block j's pwconv1 accumulates into stats_pp[j&1]; its apply pass clears stats_pp[(j+1)&1] over
@@ -1025,10 +1040,10 @@ class Model {
     float* stats_all = pl.pool.alloc_n<float>(2 * stats_n);
     float* stats_pp[2] = {stats_all, stats_all + stats_n};
     int blk_counter = 0;
-    // Deterministic mode (every stage of the tiny trunk): rows per sample a multiple of 32 -> the pwconv1 epilogue
-    // warps STORE per-warp partial column sums ([M/32][4C]) and the GRN kernels add them in a fixed order: no atomics, no clearing,
-    // bit-reproducible logits.  Otherwise (chunkyseal's odd maps) float atomics into [B][4C] as before, cleared here and by the
-    // GRN kernels.
+    // Deterministic mode (every stage's rows per sample a multiple of 32: the tiny and base trunks at S a multiple of 256): the
+    // pwconv1 epilogue warps STORE per-warp partial column sums ([M/32][4C]) and the GRN kernels add them in a fixed order: no
+    // atomics, no clearing, bit-reproducible logits.  Otherwise (chunkyseal's odd maps; the tiny and base trunks at S = 128, 384,
+    // 640, ...) float atomics into [B][4C], cleared here and by the GRN kernels.
     bool all_part = true;
     size_t part_n = 0;
     {
@@ -1056,6 +1071,7 @@ class Model {
           const int nsm = num_sms;
           pl.steps.push_back(Step{[=](cudaStream_t st) { launch_ln_rows(xin, Mp, Cv, Cvp, lw, lb, 1e-6f, xn, Cvp, nsm, st); }, 1, "cnx.ln_rows"});
         }
+        dbg(pl, "s" + std::to_string(s) + "_ln", xn, 1, B, hs, hs, Cv, Cvp);
         const int ho = (hs - 2) / 2 + 1;   // odd maps (127, 63, 31): the last row / column is dropped, like nn.Conv2d k2 s2
         float* xo = pl.pool.alloc_n<float>((size_t)B * ho * ho * Cnp);
         ConvGemmOp op;
@@ -1064,8 +1080,9 @@ class Model {
         op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.bias = ds[s - 1].conv.bias; op.p.out32 = xo; op.p.ld_out32 = Cnp;
         add_conv(pl, op, ds[s - 1].conv, "cnx.down2x2s2." + std::to_string(Cv) + "-" + std::to_string(Cn) + "@" + std::to_string(ho));
         x = xo; hs = ho; C = Cn; Cp = Cnp;
-        dbg(pl, "ds" + std::to_string(s), x, 0, B, hs, hs, C, Cp);
       }
+      const std::string ss = "s" + std::to_string(s);
+      const float* kept_ds = keep_inputs ? keep(ss + "_ds", x, hs, C, Cp) : nullptr;
       const long M = (long)B * hs * hs;
       const int rows_per_sample = hs * hs;
       __half* a = pl.pool.alloc_n<__half>(M * Cp);
@@ -1076,9 +1093,15 @@ class Model {
       __half* w2s = wscale ? pl.pool.alloc_n<__half>((size_t)B * C * 4 * C) : nullptr;
       for (int jb = 0; jb < d.ext_depths[s]; ++jb) {
         const CnBlockW& w = cn[s][jb];
+        const bool last = jb == d.ext_depths[s] - 1;
+        if (keep_inputs && last) {
+          if (jb == 0) dbg(pl, ss + "_in", kept_ds, 0, B, hs, hs, C, Cp);
+          else keep(ss + "_in", x, hs, C, Cp);
+        }
         {
           const DwConvOp op = setup_dwconv(x, B, hs, C, Cp, w.dww, w.dwb, w.lnw, w.lnb, a);
-          pl.steps.push_back(Step{[op](cudaStream_t st) { launch_dwconv(op, st); }, 1, "cnx.dwconv7_ln." + std::to_string(C) + "@" + std::to_string(hs)});
+          pl.steps.push_back(Step{[op](cudaStream_t st) { launch_dwconv(op, st); }, 1,
+                                  std::string("cnx.dwconv7_ln.") + dw_kind_name(op.kind) + "." + std::to_string(C) + "@" + std::to_string(hs)});
         }
         {
           ConvGemmOp op; setup_tma_gemm(op, a, M, C, Cp);
@@ -1104,15 +1127,20 @@ class Model {
           op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.bias = w.pw2.bias; op.p.resid32 = x; op.p.ld_res32 = Cp;
           op.p.out32 = x; op.p.ld_out32 = Cp;  // in place: each element is read and written by the same thread
           if (wscale) { op.w_samples = B; op.p.rows_per_sample = rows_per_sample; }
-          if (s == 3 && jb == d.ext_depths[s] - 1) {
+          if (s == 3 && last) {
             // the head conv's gather reads the pad channels
             x16 = Cp != C ? pl.pool.alloc_zeroed<__half>(M * Cp) : pl.pool.alloc_n<__half>(M * Cp);
             op.p.out16 = x16; op.p.ld_out16 = Cp;
+            dbg(pl, "stage3_16", x16, 1, B, hs, hs, C, Cp);
           }
           add_conv(pl, op, w.pw2, "cnx.pwconv2." + std::to_string(C) + "@" + std::to_string(hs), 0, wscale ? w2s : nullptr);
         }
-        if (jb == 0) { dbg(pl, "s" + std::to_string(s) + "b0_a", a, 1, B, hs, hs, C, Cp); dbg(pl, "s" + std::to_string(s) + "b0_g", g, 1, B, hs, hs, 4 * C, 4 * C); }
       }
+      // a, g and w2s are reused by every block of the stage: after a run they hold the last block's values (g after the in-place
+      // GRN where it is applied)
+      dbg(pl, ss + "_a", a, 1, B, hs, hs, C, Cp);
+      dbg(pl, ss + "_g", g, 1, B, hs, hs, 4 * C, 4 * C);
+      if (wscale) dbg(pl, ss + "_w2s", w2s, 1, B, C, 1, 4 * C, 4 * C);
       dbg(pl, "stage" + std::to_string(s), x, 0, B, hs, hs, C, Cp);
     }
     add_head(pl, x16, B, hs, C, Cp, "cnx.");
@@ -1132,6 +1160,7 @@ class Model {
     add_conv(pl, op, head_conv, prefix + "head3x3." + std::to_string(C) + "@" + std::to_string(hs));
     dbg(pl, "head_conv", y, 0, B, hs, hs, C, Cp);
     float* pooled = pl.pool.alloc_n<float>((size_t)B * C);
+    dbg(pl, "head_pooled", pooled, 0, B, 1, 1, C, C);
     const int P = hs * hs, Cc = C, ldy = Cp, NO = 1 + d.nbits;
     const float *lw = head_lnw, *lb = head_lnb, *hw = head_lw, *hb = head_lb;
     float* logits = pl.logits;

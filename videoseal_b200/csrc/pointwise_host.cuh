@@ -167,9 +167,13 @@ inline void launch_f32_to_u8(const float* src, uint8_t* dst, float* requant, lon
 // (dwconv_ring.cuh, map built at plan time) takes 96 / 192 dense channels on maps that tile by 16; the strip kernel the rest of
 // 96 to 768 (at 16 x 16 maps a 384-channel ring block would run one 192-thread block per SM with a 14-step prologue per 8 rows); the
 // wide kernel any even width / odd map size (chunkyseal's proportional trunk), its threads looping over the channel pairs.
+// The variant is chosen here and named in the plan's step names: ring (TMA ring), row (strip kernel, one strip = the whole row),
+// strip (strip kernel, 8-pixel strips with predicated edge columns), wide (any even width, padded rows).
+enum DwKind : int { DW_RING, DW_ROW, DW_STRIP, DW_WIDE };
+inline const char* dw_kind_name(int k) { return k == DW_RING ? "ring" : k == DW_ROW ? "row" : k == DW_STRIP ? "strip" : "wide"; }
 struct DwConvOp {
   CUtensorMap tm;
-  bool ring = false;
+  int kind = DW_WIDE;
   const float* x = nullptr;
   int B = 0, H = 0, C = 0, ld = 0, R = 0;
   const float *dww = nullptr, *dwb = nullptr, *lnw = nullptr, *lnb = nullptr;
@@ -180,8 +184,10 @@ inline DwConvOp setup_dwconv(const float* x, int B, int H, int C, int ld, const 
   DwConvOp op;
   op.x = x; op.B = B; op.H = H; op.C = C; op.ld = ld;
   op.dww = dww; op.dwb = dwb; op.lnw = lnw; op.lnb = lnb; op.out = out;
-  op.ring = ld == C && (C == 96 || C == 192) && H % 16 == 0;
-  if (op.ring) {
+  if (ld == C && (C == 96 || C == 192) && H % 16 == 0) op.kind = DW_RING;
+  else if (!(C == 96 || C == 192 || C == 384 || C == 768)) op.kind = DW_WIDE;
+  else op.kind = (C == 384 && H == 16) || (C == 768 && H == 8) ? DW_ROW : DW_STRIP;
+  if (op.kind == DW_RING) {
     op.R = H % 32 == 0 ? 32 : 16;    // rows per block: 6 halo rows + the block prologue are amortised over R
     const int BW = (C == 96 ? 8 : 4) + 6;
     uint64_t dims[4] = {(uint64_t)C, (uint64_t)H, (uint64_t)H, (uint64_t)B};
@@ -208,10 +214,10 @@ inline void launch_dw_strip_t(const DwConvOp& op, int spb, long ngroups, cudaStr
 inline void launch_dwconv(const DwConvOp& op, cudaStream_t st) {
   const int C = op.C, H = op.H;
   const long nstrips = (long)op.B * H * ((H + kDwStrip - 1) / kDwStrip);
-  if (op.ring) {
+  if (op.kind == DW_RING) {
     if (C == 96) launch_dw_ring_t<96, 2, 4, 8>(op, st);
     else launch_dw_ring_t<192, 1, 4, 8>(op, st);
-  } else if (!(C == 96 || C == 192 || C == 384 || C == 768)) {
+  } else if (op.kind == DW_WIDE) {
     const int threads = std::min(512, (C / 2 + 31) / 32 * 32);
     const size_t smem_w = (size_t)kDwStrip * C * sizeof(float);
     smem_optin<dwconv7_ln_wide_kernel>(200 * 1024);
@@ -224,8 +230,8 @@ inline void launch_dwconv(const DwConvOp& op, cudaStream_t st) {
     if (spb * C2 > 512) throw Error("dwconv7: C/2 > 512 threads is not implemented (unsupported chunky extractor width)", kErrUnsupported);
     // narrow maps: one strip = the whole row, so no column is ever out of the image
     const long nrows = (long)op.B * H;
-    if (C == 384 && H == 16) launch_dw_strip_t<384, 16, true>(op, 1, nrows, st);
-    else if (C == 768 && H == 8) launch_dw_strip_t<768, 8, true>(op, 1, nrows, st);
+    if (op.kind == DW_ROW && C == 384) launch_dw_strip_t<384, 16, true>(op, 1, nrows, st);
+    else if (op.kind == DW_ROW) launch_dw_strip_t<768, 8, true>(op, 1, nrows, st);
     else if (C == 96) launch_dw_strip_t<96, 8, false>(op, spb, nstrips, st);
     else if (C == 192) launch_dw_strip_t<192, 8, false>(op, spb, nstrips, st);
     else if (C == 384) launch_dw_strip_t<384, 8, false>(op, spb, nstrips, st);

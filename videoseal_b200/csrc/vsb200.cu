@@ -245,6 +245,15 @@ int64_t vsb_debug_get_tensor(vsb_model* m, const char* name, float* host_out, in
   }
 }
 
+int vsb_debug_keep_inputs(vsb_model* m, int32_t on) {
+  VSB_API_BEGIN
+  VSB_CHECK(m != nullptr, "null argument");
+  VSB_MODEL_SCOPE(m);
+  m->impl.set_keep_inputs(on != 0);
+  return VSB_OK;
+  VSB_API_END
+}
+
 int32_t vsb_debug_last_dispatch(vsb_model* m, int32_t* out, int32_t capacity) {
   try {
     VSB_CHECK(m && out, "null argument");
