@@ -40,12 +40,25 @@ enum vsb_status {
 
 enum vsb_video_mode { VSB_VIDEO_REPEAT = 0, VSB_VIDEO_ALTERNATE = 1, VSB_VIDEO_INTERPOLATE = 2 };
 
+/* Resizes follow the reference's `interpolation` dict, F.interpolate(size=..., **interpolation) at both resize sites (frames to
+ * img_size, wam.py:161-164 / videoseal.py:305; the delta back to the frame size, wam.py:183-185 / videoseal.py:329).  The mode sits
+ * in bits 5-6 (VSB_FLAG_RESIZE_MODE(m)); all resize bits zero = bilinear, align_corners=False, antialias=True.  Nearest and area
+ * need VSB_FLAG_RESIZE_NO_AA and no VSB_FLAG_RESIZE_ALIGN_CORNERS (F.interpolate raises ValueError otherwise; here
+ * VSB_ERR_INVALID when a resize happens).  Outputs of bicubic resizes are not clamped (only imgs_w is, by VSB_FLAG_CLAMP). */
+enum vsb_resize_mode { VSB_RESIZE_BILINEAR = 0, VSB_RESIZE_BICUBIC = 1, VSB_RESIZE_NEAREST = 2, VSB_RESIZE_AREA = 3 };
+
 enum vsb_flags {
   VSB_FLAG_CLAMP = 1,            /* clamp imgs_w to [0,1]           (wam.py:196-197) */
   VSB_FLAG_LOWRES_ATTN = 2,      /* JND at processing resolution    (wam.py:177-180) */
   VSB_FLAG_NO_ATTENUATION = 4,   /* model.attenuation = None        */
-  VSB_FLAG_RESIZE_NO_AA = 8      /* interpolation antialias=False   (videoseal.py:394) */
+  VSB_FLAG_RESIZE_NO_AA = 8,     /* interpolation antialias=False   (videoseal.py:394) */
+  VSB_FLAG_RESIZE_ALIGN_CORNERS = 16,   /* interpolation align_corners=True */
+  VSB_FLAG_RESIZE_MODE_SHIFT = 5,       /* interpolation mode: a vsb_resize_mode in bits 5-6 */
+  VSB_FLAG_RESIZE_MODE_MASK = 0x60
 };
+#define VSB_FLAG_RESIZE_MODE(m) ((int32_t)(m) << VSB_FLAG_RESIZE_MODE_SHIFT)
+/* the bits of vsb_flags that describe a resize */
+#define VSB_FLAG_RESIZE_BITS (VSB_FLAG_RESIZE_NO_AA | VSB_FLAG_RESIZE_ALIGN_CORNERS | VSB_FLAG_RESIZE_MODE_MASK)
 
 /* Architecture hyper-parameters taken from the model card (videoseal/cards/<card>.yaml). */
 typedef struct vsb_model_desc {
@@ -199,7 +212,8 @@ int vsb_debug_keep_inputs(vsb_model* m, int32_t on);
  *   out[0..4]  resize_sep_kernel:  MT (x taps in registers: 2, 8, or 0 = any count), GST (input rows per staging round: 4, 2, 1),
  *              vec (1 = bulk copies, 0 = 4-byte cp.async), toy (output rows per block), OW (output width = img_size)
  *   out[5..9]  blend:  3 = jnd_blend3_kernel (TMA-fed) or 2 = jnd_blend2_kernel, VEC (4 or 1), FASTUP (1 = delta read in place or
- *              through <= 2 taps per axis), CD (delta channels), JIN (heat-map inputs: 1 luminance, 3 per RGB channel)
+ *              through <= 2 taps per axis, 4 = through 3 or 4 taps per axis (bicubic), 0 = generic tables), CD (delta channels),
+ *              JIN (heat-map inputs: 1 luminance, 3 per RGB channel)
  * Entries are -1 until that kernel has run on this handle.  capacity >= 10; returns 10, or < 0. */
 int32_t vsb_debug_last_dispatch(vsb_model* m, int32_t* out, int32_t capacity);
 /* standalone conv/GEMM on the wgmma kernels for unit tests: see tests/test_conv_gemm_gpu.py */
@@ -228,6 +242,11 @@ int vsb_debug_conv(const vsb_conv_test* t, void* stream);
  * restatement of ATen's bilinear (anti-aliased or plain, align_corners=False) index/weight computation behind F.interpolate
  * (wam.py:163,184,224).  start / cnt: [out]; weights: [out * maxt] row-major, capacity in floats.  Returns maxt, or < 0. */
 int vsb_debug_resample_table(int32_t in, int32_t out, int32_t antialias, int32_t* start, int32_t* cnt, float* weights, int64_t capacity);
+/* the same for any resize the flags describe: mode a vsb_resize_mode, align_corners and antialias 0 / 1 (VSB_ERR_INVALID for the
+ * combinations F.interpolate rejects).  Every table has contiguous taps inside [0, in): bicubic taps past an edge are folded into
+ * the edge tap's weight.  With mode 0 and align_corners 0 it returns what vsb_debug_resample_table returns. */
+int vsb_debug_resample_table2(int32_t in, int32_t out, int32_t mode, int32_t align_corners, int32_t antialias, int32_t* start, int32_t* cnt,
+                              float* weights, int64_t capacity);
 
 #ifdef __cplusplus
 }

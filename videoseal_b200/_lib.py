@@ -13,10 +13,13 @@ EXPORTS = [
     "vsb_last_error", "vsb_version", "vsb_model_create", "vsb_model_set_tensor", "vsb_model_set_pixel_decoder", "vsb_model_finalize",
     "vsb_model_destroy", "vsb_embed", "vsb_embedder_forward", "vsb_detect", "vsb_jnd_heatmaps", "vsb_embed_host",
     "vsb_detect_host", "vsb_embed_detect_host", "vsb_frames_host_u8", "vsb_launch_count", "vsb_profile_enable", "vsb_profile_read", "vsb_debug_get_tensor", "vsb_debug_keep_inputs", "vsb_debug_conv",
-    "vsb_debug_resample_table", "vsb_debug_last_dispatch", "vsb_quality_workspace_bytes", "vsb_ssim", "vsb_model_set_vit_extractor",
+    "vsb_debug_resample_table", "vsb_debug_resample_table2", "vsb_debug_last_dispatch", "vsb_quality_workspace_bytes", "vsb_ssim", "vsb_model_set_vit_extractor",
 ]
 
 FLAG_CLAMP, FLAG_LOWRES_ATTN, FLAG_NO_ATTENUATION, FLAG_RESIZE_NO_AA = 1, 2, 4, 8
+FLAG_RESIZE_ALIGN_CORNERS, FLAG_RESIZE_MODE_SHIFT = 16, 5
+# F.interpolate modes the resizes implement (vsb_resize_mode), in bits 5-6 of the flags
+RESIZE_MODES = {"bilinear": 0, "bicubic": 1, "nearest": 2, "area": 3}
 VIDEO_MODES = {"repeat": 0, "alternate": 1, "interpolate": 2}
 
 
@@ -97,6 +100,8 @@ def lib():
     L.vsb_debug_keep_inputs.argtypes = [C.c_void_p, C.c_int32]
     L.vsb_debug_conv.argtypes = [C.POINTER(ConvTest), C.c_void_p]
     L.vsb_debug_resample_table.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
+    L.vsb_debug_resample_table2.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_int64]
     L.vsb_debug_last_dispatch.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int32]
     L.vsb_debug_last_dispatch.restype = C.c_int32
     L.vsb_quality_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]

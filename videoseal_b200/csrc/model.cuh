@@ -7,6 +7,7 @@
 #include <memory>
 #include <mutex>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include "../../include/vsb200.h"
@@ -166,7 +167,7 @@ class Model {
   }
 
   std::map<int, std::unique_ptr<Plan>> embed_plans, detect_plans;
-  std::map<uint64_t, std::unique_ptr<ResampleDev>> resamplers;
+  std::map<std::tuple<int, int, int, int, int, bool, bool>, std::unique_ptr<ResampleDev>> resamplers;
   Plan* last_plan = nullptr;
   // test seam (vsb_debug_last_dispatch): the variant of the most recent launch of each full-resolution kernel, -1 before the first
   //   resize: MT, GST, vec, toy, OW       blend: 3 (jnd_blend3_kernel) or 2 (jnd_blend2_kernel), VEC, FASTUP, CD, JIN
@@ -1308,20 +1309,20 @@ class Model {
     }
   }
 
-  ResampleDev* get_resampler(int ih, int iw, int oh, int ow, bool aa) {
-    const uint64_t key = ((uint64_t)ih << 48) ^ ((uint64_t)iw << 32) ^ ((uint64_t)oh << 16) ^ ((uint64_t)ow << 1) ^ (aa ? 1 : 0);
+  ResampleDev* get_resampler(int ih, int iw, int oh, int ow, ResampleMode m) {
+    const auto key = std::make_tuple(ih, iw, oh, ow, m.mode, m.align_corners, m.antialias);
     auto it = resamplers.find(key);
     if (it != resamplers.end()) return it->second.get();
-    std::unique_ptr<ResampleDev> r(new ResampleDev(ih, iw, oh, ow, aa));
+    std::unique_ptr<ResampleDev> r(new ResampleDev(ih, iw, oh, ow, m));
     ResampleDev* ret = r.get();
     resamplers[key] = std::move(r);
     return ret;
   }
 
   // resample `n` frames that are `frame_stride` floats apart to S x S (one launch, also for strided key frames)
-  void resize_frames(const float* src, long frame_stride, int n, int H, int W, float* dst, bool aa, cudaStream_t st) {
+  void resize_frames(const float* src, long frame_stride, int n, int H, int W, float* dst, ResampleMode rm, cudaStream_t st) {
     const int S = d.img_size;
-    const ResampleDev* r = get_resampler(H, W, S, S, aa);
+    const ResampleDev* r = get_resampler(H, W, S, S, rm);
     for (int i = 0; i < n; i += 16384) {   // gridDim.y limit: split very long frame ranges
       const int m = std::min(16384, n - i);
       prof_scope("pw.resize." + std::to_string(H) + "x" + std::to_string(W) + "@" + std::to_string(m), st, 1, [&] {
@@ -1398,7 +1399,7 @@ class Model {
       VSB_CUDA(cudaMemcpyAsync(imgs_w_h + (size_t)f0 * fpx, out + (size_t)f0 * fpx, (size_t)n * fpx * sizeof(float), cudaMemcpyDeviceToHost, s_out));
       if (f0 + n - g0 >= kMaxBatch || k == nsl - 1) {   // a full extractor batch (or the tail) is complete: detect its frames
         const int gn = f0 + n - g0;
-        detect(out + (size_t)g0 * fpx, lg + (size_t)g0 * NO, gn, H, W, flags & VSB_FLAG_RESIZE_NO_AA, s_cmp);
+        detect(out + (size_t)g0 * fpx, lg + (size_t)g0 * NO, gn, H, W, flags & VSB_FLAG_RESIZE_BITS, s_cmp);
         VSB_CUDA(cudaEventRecord(ev_cmp[nsl], s_cmp));
         VSB_CUDA(cudaStreamWaitEvent(s_out, ev_cmp[nsl], 0));
         VSB_CUDA(cudaMemcpyAsync(logits_h + (size_t)g0 * NO, lg + (size_t)g0 * NO, (size_t)gn * NO * sizeof(float), cudaMemcpyDeviceToHost, s_out));
@@ -1449,7 +1450,7 @@ class Model {
         g_launches += 1;
         det_in = out + (size_t)f0 * fpx;
       }
-      if (do_detect) detect(det_in, lg + (size_t)f0 * NO, n, H, W, flags & VSB_FLAG_RESIZE_NO_AA, s_cmp);
+      if (do_detect) detect(det_in, lg + (size_t)f0 * NO, n, H, W, flags & VSB_FLAG_RESIZE_BITS, s_cmp);
       VSB_CUDA(cudaGetLastError());
       VSB_CUDA(cudaEventRecord(ev_cmp[k], s_cmp));
       VSB_CUDA(cudaStreamWaitEvent(s_out, ev_cmp[k], 0));
@@ -1496,14 +1497,14 @@ class Model {
     const int bint = interp ? chunk_keys : 0;
     const int S = d.img_size;
     const bool same = (H == S && W == S);
-    const bool aa = !(flags & VSB_FLAG_RESIZE_NO_AA);
+    const ResampleMode rm = same ? ResampleMode() : resample_mode(flags);   // (the flags are read only when a resize happens)
     const bool use_jnd = !(flags & VSB_FLAG_NO_ATTENUATION) && d.jnd_in_ch != 0;
     // channels of hmaps * preds_w (broadcast): what `preds_w` holds and what the low-resolution path hands to the blend
     const int PC = use_jnd ? std::max(d.unet_out_ch, d.jnd_out_ch) : d.unet_out_ch;
     const bool lowres = use_jnd && (flags & VSB_FLAG_LOWRES_ATTN);
     const long fstride = (long)3 * H * W;
     const int nkeys = (F + step - 1) / step;
-    ResampleDev* up = same ? nullptr : get_resampler(S, S, H, W, aa);
+    ResampleDev* up = same ? nullptr : get_resampler(S, S, H, W, rm);
     for (int k0 = 0; k0 < nkeys; k0 += kbatch) {
       const int nk = std::min(kbatch, nkeys - k0);
       const int f0 = k0 * step, f1 = std::min(F, (k0 + nk) * step);
@@ -1516,7 +1517,7 @@ class Model {
       const float* frames_res = x;
       if (lowres && !same) {
         float* fr = (float*)stage(6, (size_t)nf * 3 * S * S * sizeof(float));
-        resize_frames(x, fstride, nf, H, W, fr, aa, st);
+        resize_frames(x, fstride, nf, H, W, fr, rm, st);
         frames_res = fr;
       }
       if (!same || step != 1) {
@@ -1525,7 +1526,7 @@ class Model {
           VSB_CUDA(cudaMemcpy2DAsync(pl->x_res, (size_t)3 * S * S * sizeof(float), frames_res, (size_t)step * 3 * S * S * sizeof(float),
                                      (size_t)3 * S * S * sizeof(float), nk, cudaMemcpyDeviceToDevice, st));
         } else {
-          resize_frames(x, (long)step * fstride, nk, H, W, pl->x_res, aa, st);
+          resize_frames(x, (long)step * fstride, nk, H, W, pl->x_res, rm, st);
         }
         x = pl->x_res;
       }
@@ -1553,7 +1554,7 @@ class Model {
         bp.delta = delta; bp.step = step; bp.alternate = balt; bp.interp_chunk = bint; bp.use_jnd = use_jnd ? 1 : 0;
       }
       prof_scope(std::string(bp.use_jnd ? "pw.jnd_blend." : "pw.blend.") + std::to_string(bp.H) + "x" + std::to_string(bp.W) + "@" +
-                     std::to_string(bp.F) + (bp.preds_w ? "+preds" : ""), st, 1, [&] { launch_blend(bp, last_blend, st); });
+                     std::to_string(bp.F) + (bp.preds_w ? "+preds" : ""), st, 1, [&] { launch_blend(bp, up, last_blend, st); });
     }
   }
 
@@ -1570,14 +1571,14 @@ class Model {
     VSB_CHECK(F > 0 && H > 0 && W > 0, "bad detect shape");
     const int S = d.img_size;
     const bool same = (H == S && W == S);
-    const bool aa = !(flags & VSB_FLAG_RESIZE_NO_AA);
+    const ResampleMode rm = same ? ResampleMode() : resample_mode(flags);
     const long fstride = (long)3 * H * W;
     const size_t NO = detect_out_per_frame();
     for (int f0 = 0; f0 < F; f0 += kMaxBatch) {
       const int n = std::min(kMaxBatch, F - f0);
       Plan* pl = get_detect_plan(n);
       const float* x = imgs + (size_t)f0 * fstride;
-      if (!same) { resize_frames(x, fstride, n, H, W, pl->x_res, aa, st); x = pl->x_res; }
+      if (!same) { resize_frames(x, fstride, n, H, W, pl->x_res, rm, st); x = pl->x_res; }
       pl->in_imgs = x;
       pl->out_maps = pixelwise ? logits + (size_t)f0 * NO : nullptr;   // the maps are written in place, at this sub-batch's offset
       pl->run(st);

@@ -1,5 +1,6 @@
 // HBM-bound full-resolution stage of the path (round 2):
-//   K5  resize_sep_kernel    F.interpolate(bilinear, align_corners=False, antialias on/off) as a SEPARABLE resample: groups of input
+//   K5  resize_sep_kernel    F.interpolate(size, **interpolation) as a SEPARABLE resample (any table of resize_blend_host.cuh:
+//                            bilinear / bicubic with or without antialias and align_corners, nearest, area): groups of input
 //                            rows arrive in shared memory as single bulk copies on an mbarrier ring, the horizontal pass runs out of
 //                            shared memory with the thread's taps in registers, the vertical pass out of a second shared buffer.  One
 //                            launch handles key frames that are `frame_stride` apart (video mode).  Replaces the scalar per-output-pixel
@@ -10,7 +11,8 @@
 //                            2-pixel halo (out-of-image = zero fill = the conv padding), a second one the delta tile; double buffer
 //                            over 4 tiles per block; separable 5x5 / Sobel sums and jnd_value in packed fp32, SFU transcendentals.
 //       jnd_blend2_kernel    the same arithmetic with per-thread loads: widths that are not multiples of 4, unaligned tensors,
-//                            anti-aliased delta down-scale, frames smaller than a TMA box.
+//                            delta down-scale, frames smaller than a TMA box.
+//       Both up-scale the delta through <= 2 taps per axis (FASTUP 1) or, for bicubic tables, 3-4 taps (FASTUP 4).
 #pragma once
 #include "conv_gemm.cuh"
 #include "pointwise.cuh"
@@ -193,7 +195,12 @@ __global__ void __launch_bounds__(256) resize_sep_kernel(const float* __restrict
 // ------------------------------------------------------------------------------------------------ K7
 constexpr int kB2TW = 128, kB2TH = 16, kB2LP = 136;   // tile, and the pitch of the luminance tile (image column x0 + j at index 4 + j)
 constexpr int kB2DH = kB2TH + 2, kB2DW = kB2TW + 4;   // delta tile at processing resolution (up-scale: at most 1 source pixel per output pixel + 1)
-constexpr size_t b2_smem(int jin) { return (size_t)(jin * (kB2TH + 4) * kB2LP + 3 * kB2TH * kB2TW + kB2DH * kB2DW) * sizeof(float); }
+// 4-tap up-scale (bicubic): taps floor - 1 .. floor + 2 reach one source row further on each side; the rows / columns read are at most
+// tile + 3 (the host checks every table against these sizes: ResampleDev::blend_rows / blend_cols)
+constexpr int kB2DH4 = kB2TH + 4;
+constexpr size_t b2_smem(int jin, int fastup = 1) {
+  return (size_t)(jin * (kB2TH + 4) * kB2LP + 3 * kB2TH * kB2TW + (fastup == 4 ? kB2DH4 : kB2DH) * kB2DW) * sizeof(float);
+}
 
 __device__ __forceinline__ float lg2_approx(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float ex2_approx_f(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
@@ -288,10 +295,34 @@ __device__ __forceinline__ void jnd_hm_vec4(const float* __restrict__ lum_, int 
     }
 }
 
+// Delta up-scale through 4 taps per axis (bicubic tables, 3 or 4 taps): the taps of output o, as the offset of its first tap from
+// `base` and its weights, zero past its tap count.  The kernels read all 4 samples; those past the count have weight 0 and lie
+// inside the staged tile (kB2DH4 rows; columns: see kB2DH4), which holds finite values everywhere.
+__device__ __forceinline__ int taps4(const int* __restrict__ start, const int* __restrict__ cnt, const float* __restrict__ w, int maxt,
+                                     int o, int base, float (&wo)[4]) {
+  const int c = __ldg(cnt + o);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) wo[i] = i < c ? __ldg(w + (long)o * maxt + i) : 0.f;
+  return __ldg(start + o) - base;
+}
+// sum over the 4 x 4 staged samples from `a` (row pitch P): horizontal sums per source row first, then the vertical one
+template <int P>
+__device__ __forceinline__ float up4(const float* a, const float (&xw)[4], const float (&yw)[4]) {
+  float v = 0.f;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float* r = a + i * P;
+    const float h = fmaf(xw[3], r[3], fmaf(xw[2], r[2], fmaf(xw[1], r[1], xw[0] * r[0])));
+    v = i == 0 ? yw[0] * h : fmaf(yw[i], h, v);
+  }
+  return v;
+}
+
 // VEC 4: W % 4 == 0 and 16-byte aligned tensors: thread = 4 consecutive pixels (128-bit global / shared accesses).
 // VEC 1: any W / alignment: thread = pixels lane, lane+32, lane+64, lane+96 of the tile row (32-bit accesses, fully coalesced).
 // FASTUP 1: the delta is read in place (identity) or up-scaled through <= 2 taps per axis from a tile staged in shared memory
-//           (every input at least as large as the processing size); 0: generic separable tables straight from global memory.
+//           (every input at least as large as the processing size); 4: the same through 3 or 4 taps per axis (kB2DH4 x kB2DW tile,
+//           zero outside the delta); 0: generic separable tables straight from global memory.
 // Thread = 2 rows x 4 pixels.  The 5x5 luminance filter and the Sobel pair are evaluated SEPARABLY while the six luminance rows
 // of the two output rows stream through registers (per row: 5- and 3-sums, the horizontal difference and the [1 2 1] smooth).
 // CD: delta channels (1 for the Y-channel cards, 3 for RGB U-Nets) as a compile-time constant: the per-channel loops and their
@@ -325,8 +356,14 @@ __global__ void __launch_bounds__(256, 3) jnd_blend2_kernel(const BlendParams p)
   }
   auto stage_delta = [&](int c, int s) {
     const float* src = p.delta + ((long)(s ? fk.k1 : fk.k0) * CD + c) * p.PH * p.PW + (long)sy0 * p.PW + sx0;
-    for (int r = warp; r < dnr; r += 8)
-      for (int cc = lane; cc < dnc; cc += 32) dl[r * kB2DW + cc] = __ldg(src + (long)r * p.PW + cc);
+    if constexpr (FASTUP == 4) {         // the whole tile: the 4-tap reads pass the last tap of an edge output (with weight 0)
+      for (int r = warp; r < kB2DH4; r += 8)
+        for (int cc = lane; cc < kB2DW; cc += 32)
+          dl[r * kB2DW + cc] = (sy0 + r < p.PH && sx0 + cc < p.PW) ? __ldg(src + (long)r * p.PW + cc) : 0.f;
+    } else {
+      for (int r = warp; r < dnr; r += 8)
+        for (int cc = lane; cc < dnc; cc += 32) dl[r * kB2DW + cc] = __ldg(src + (long)r * p.PW + cc);
+    }
   };
 
   // ---- phase 1: this thread's pixels (2 rows x 4 pixels x RGB) -> shared; luminance tile with a 2-pixel zero halo
@@ -505,7 +542,35 @@ __global__ void __launch_bounds__(256, 3) jnd_blend2_kernel(const BlendParams p)
     for (int j = 0; j < 2; ++j)
 #pragma unroll
       for (int q = 0; q < 4; ++q) d[c][j][q] = 0.f;
-  if (has_delta) {
+  if constexpr (FASTUP == 4) {           // (launched for up-scales only: never in place)
+    if (has_delta) {
+      int xr[4], yr[2];
+      float xw[4][4], yw[2][4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) xr[q] = taps4(p.tab.xstart, p.tab.xcnt, p.tab.xw, p.tab.maxt_x, min(x0 + col_of(q), p.W - 1), sx0, xw[q]);
+#pragma unroll
+      for (int j = 0; j < 2; ++j) yr[j] = taps4(p.tab.ystart, p.tab.ycnt, p.tab.yw, p.tab.maxt_y, min(y0 + warp * 2 + j, p.H - 1), sy0, yw[j]);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        if (c >= CD) break;
+        for (int s = 0; s < nsrc; ++s) {
+          if ((c | s) != 0) {
+            __syncthreads();
+            stage_delta(c, s);
+            __syncthreads();
+          }
+          const float ws = nsrc == 1 ? 1.f : (s ? 1.f - fk.a : fk.a);
+#pragma unroll
+          for (int j = 0; j < 2; ++j)
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+              const float vs = up4<kB2DW>(dl + yr[j] * kB2DW + xr[q], xw[q], yw[j]);
+              d[c][j][q] = fmaf(ws, vs, d[c][j][q]);
+            }
+        }
+      }
+    }
+  } else if (has_delta) {
     int xr[4] = {0, 0, 0, 0}, xo[4] = {0, 0, 0, 0};
     float xw0[4] = {1.f, 1.f, 1.f, 1.f}, xw1[4] = {0.f, 0.f, 0.f, 0.f};
     int yr[2] = {0, 0}, yo[2] = {0, 0};
@@ -638,18 +703,21 @@ constexpr int kB3NT = 4;
 constexpr int kB3RAW = 3 * (kB2TH + 4) * kB2LP;             // floats of one raw tile (32 640 B, a multiple of 128)
 constexpr int kB3DW = kB2DW + 4;                            // delta tile pitch: the box starts at a 16-byte aligned source column (TMA faults otherwise)
 constexpr int kB3DL = 2464;                                 // floats reserved per delta tile (kB2DH * kB3DW = 2448, rounded to 128 B)
-constexpr size_t b3_smem(int jin) {
-  return (size_t)(2 * kB3RAW + 2 * kB3DL + jin * (kB2TH + 4) * kB2LP) * sizeof(float) + 2 * sizeof(uint64_t) + 128;
+constexpr int kB3DL4 = kB2DH4 * kB3DW;                      // the same for the 4-tap up-scale (2720 floats, a multiple of 128 B)
+constexpr size_t b3_smem(int jin, int fastup = 1) {
+  return (size_t)(2 * kB3RAW + 2 * (fastup == 4 ? kB3DL4 : kB3DL) + jin * (kB2TH + 4) * kB2LP) * sizeof(float) + 2 * sizeof(uint64_t) + 128;
 }
 
-template <int CD, int JIN>
+// FASTUP 1: delta in place or through <= 2 taps per axis; 4: through 3 or 4 taps per axis, from a kB2DH4-row box
+template <int CD, int JIN, int FASTUP = 1>
 __global__ void __launch_bounds__(256, 2) jnd_blend3_kernel(const BlendParams p, const __grid_constant__ CUtensorMap tmI,
                                                             const __grid_constant__ CUtensorMap tmD) {
   extern __shared__ uint8_t b3_smem_[];
   constexpr int LUMP = (kB2TH + 4) * kB2LP;
+  constexpr int DL = FASTUP == 4 ? kB3DL4 : kB3DL, DH = FASTUP == 4 ? kB2DH4 : kB2DH;
   float* raw = reinterpret_cast<float*>(b3_smem_ + ((128u - (smem_u32(b3_smem_) & 127u)) & 127u));   // [2][3][TH + 4][LP], 128-byte aligned
   float* dlb = raw + 2 * kB3RAW;                          // [2][DH][kB3DW]
-  float* lum = dlb + 2 * kB3DL;                           // [JIN][TH + 4][LP]
+  float* lum = dlb + 2 * DL;                              // [JIN][TH + 4][LP]
   uint64_t* full = reinterpret_cast<uint64_t*>(lum + JIN * LUMP);
   const int f = blockIdx.z, x0 = blockIdx.x * kB2TW, Y0 = blockIdx.y * (kB3NT * kB2TH);
   const int plane = p.H * p.W;                            // < 2^31 (host-checked)
@@ -660,14 +728,14 @@ __global__ void __launch_bounds__(256, 2) jnd_blend3_kernel(const BlendParams p,
   const bool staged = !p.identity_resample && has_delta;
   const int ntl = min(kB3NT, (p.H - Y0 + kB2TH - 1) / kB2TH);
   const int sx0 = staged ? (__ldg(p.tab.xstart + x0) & ~3) : 0;      // first source column of the delta tile, rounded down to 16 bytes
-  const uint32_t tx_bytes = (uint32_t)(kB3RAW * sizeof(float)) + (staged ? (uint32_t)(kB2DH * kB3DW * sizeof(float)) : 0u);
+  const uint32_t tx_bytes = (uint32_t)(kB3RAW * sizeof(float)) + (staged ? (uint32_t)(DH * kB3DW * sizeof(float)) : 0u);
 
   auto issue = [&](int t) {                               // thread 0: both boxes of tile t
     const int buf = t & 1, y0 = Y0 + t * kB2TH;
     fence_proxy_async_smem();                             // the buffer was last touched through the generic proxy
     mbar_arrive_expect_tx(&full[buf], tx_bytes);
     tma_load_3d(&tmI, &full[buf], raw + buf * kB3RAW, x0 - 4, y0 - 2, f * 3);
-    if (staged) tma_load_3d(&tmD, &full[buf], dlb + buf * kB3DL, sx0, __ldg(p.tab.ystart + y0), fk.k0 * CD);
+    if (staged) tma_load_3d(&tmD, &full[buf], dlb + buf * DL, sx0, __ldg(p.tab.ystart + y0), fk.k0 * CD);
   };
   if (threadIdx.x == 0) {
     mbar_init(&full[0], 1);
@@ -678,7 +746,13 @@ __global__ void __launch_bounds__(256, 2) jnd_blend3_kernel(const BlendParams p,
   // x taps of this thread's 4 pixels for the delta up-sample (the same for every tile of the block)
   int xr[4] = {0, 0, 0, 0}, xo[4] = {0, 0, 0, 0};
   float xw0[4] = {1.f, 1.f, 1.f, 1.f}, xw1[4] = {0.f, 0.f, 0.f, 0.f};
-  if (staged) {
+  float xw4[FASTUP == 4 ? 4 : 1][4];                      // 4-tap weights
+  if constexpr (FASTUP == 4) {
+    if (staged) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q) xr[q] = taps4(p.tab.xstart, p.tab.xcnt, p.tab.xw, p.tab.maxt_x, min(x0 + lane * 4 + q, p.W - 1), sx0, xw4[q]);
+    }
+  } else if (staged) {
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
       const int ox = min(x0 + lane * 4 + q, p.W - 1);
@@ -697,7 +771,7 @@ __global__ void __launch_bounds__(256, 2) jnd_blend3_kernel(const BlendParams p,
   for (int t = 0; t < ntl; ++t) {
     const int y0 = Y0 + t * kB2TH, buf = t & 1;
     const float* rawb = raw + buf * kB3RAW;
-    float* dl = dlb + buf * kB3DL;
+    float* dl = dlb + buf * DL;
     if (t + 1 < ntl && threadIdx.x == 0) issue(t + 1);    // buffer buf^1 was released by the barrier that ended tile t - 1
     mbar_wait(&full[buf], (t >> 1) & 1);
 
@@ -749,8 +823,13 @@ __global__ void __launch_bounds__(256, 2) jnd_blend3_kernel(const BlendParams p,
       int yr[2] = {0, 0}, yo[2] = {0, 0};
       float yw0[2] = {1.f, 1.f}, yw1[2] = {0.f, 0.f};
       int sy0 = 0, dnr = 0, dnc = 0;
+      float yw4[FASTUP == 4 ? 2 : 1][4];                  // 4-tap weights
       if (staged) {
         sy0 = __ldg(p.tab.ystart + y0);
+        if constexpr (FASTUP == 4) {
+#pragma unroll
+          for (int j = 0; j < 2; ++j) yr[j] = taps4(p.tab.ystart, p.tab.ycnt, p.tab.yw, p.tab.maxt_y, min(y0 + warp * 2 + j, p.H - 1), sy0, yw4[j]);
+        } else {
 #pragma unroll
         for (int j = 0; j < 2; ++j) {
           const int oy = min(y0 + warp * 2 + j, p.H - 1);
@@ -759,6 +838,7 @@ __global__ void __launch_bounds__(256, 2) jnd_blend3_kernel(const BlendParams p,
           yw0[j] = __ldg(p.tab.yw + oy * p.tab.maxt_y);
           yw1[j] = yc > 1 ? __ldg(p.tab.yw + oy * p.tab.maxt_y + 1) : 0.f;
           yo[j] = yc > 1 ? 1 : 0;
+        }
         }
         if (CD * nsrc > 1) {                 // geometry of the tiles staged by hand below
           const int ylast = min(y0 + kB2TH, p.H) - 1, xlast = min(x0 + kB2TW, p.W) - 1;
@@ -788,6 +868,9 @@ __global__ void __launch_bounds__(256, 2) jnd_blend3_kernel(const BlendParams p,
               if (p.identity_resample) {
                 const float4 v4 = __ldg(reinterpret_cast<const float4*>(src + (long)gy * p.PW + x0 + lane * 4));
                 vs[0] = v4.x; vs[1] = v4.y; vs[2] = v4.z; vs[3] = v4.w;
+              } else if constexpr (FASTUP == 4) {
+#pragma unroll
+                for (int q = 0; q < 4; ++q) vs[q] = up4<kB3DW>(dl + yr[j] * kB3DW + xr[q], xw4[q], yw4[j]);
               } else {
 #pragma unroll
                 for (int q = 0; q < 4; ++q) {

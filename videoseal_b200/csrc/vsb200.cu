@@ -352,9 +352,19 @@ int vsb_debug_conv(const vsb_conv_test* t, void* stream) {
 }
 
 int vsb_debug_resample_table(int32_t in, int32_t out, int32_t antialias, int32_t* start, int32_t* cnt, float* weights, int64_t capacity) {
+  return vsb_debug_resample_table2(in, out, VSB_RESIZE_BILINEAR, 0, antialias, start, cnt, weights, capacity);
+}
+
+int vsb_debug_resample_table2(int32_t in, int32_t out, int32_t mode, int32_t align_corners, int32_t antialias, int32_t* start, int32_t* cnt,
+                              float* weights, int64_t capacity) {
   try {
     VSB_CHECK(in > 0 && out > 0 && start && cnt && weights, "bad argument");
-    const ResampleHost t = make_resample(in, out, antialias != 0);
+    VSB_CHECK(mode >= VSB_RESIZE_BILINEAR && mode <= VSB_RESIZE_AREA && (align_corners | antialias) >= 0 && (align_corners | antialias) <= 1,
+              "bad resize mode");
+    const ResampleMode m = resample_mode(VSB_FLAG_RESIZE_MODE(mode) | (align_corners ? VSB_FLAG_RESIZE_ALIGN_CORNERS : 0) |
+                                         (antialias ? 0 : VSB_FLAG_RESIZE_NO_AA));
+    const ResampleHost t = make_resample(in, out, m);
+    check_table(t, in);
     VSB_CHECK(capacity >= (int64_t)out * t.maxt, "weights buffer too small");
     for (int i = 0; i < out; ++i) { start[i] = t.start[i]; cnt[i] = t.cnt[i]; }
     for (size_t i = 0; i < t.w.size(); ++i) weights[i] = t.w[i];

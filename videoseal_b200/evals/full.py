@@ -88,7 +88,7 @@ def evaluate(model, dataset: Iterable, is_video: bool, output_dir: str, num_fram
 def main(argv=None):
     import argparse
     from ..cfg import setup_model_from_checkpoint
-    from .speed import _bool, synthetic_items
+    from .speed import _bool, add_interpolation_args, interpolation_of, synthetic_items
     ap = argparse.ArgumentParser(description="identity-augmentation evaluation of a card / checkpoint on this backend")
     ap.add_argument("--checkpoint", required=True)
     ap.add_argument("--device", default="cuda")
@@ -102,12 +102,13 @@ def main(argv=None):
     ap.add_argument("--output_dir", default="output/full")
     ap.add_argument("--image_metrics", nargs="+", default=["psnr"], choices=IMAGE_METRICS,
                     help="quality columns (psnr ssim msssim gives the reference's; ssim / msssim need the GPU)")
+    add_interpolation_args(ap)
     a = ap.parse_args(argv)
     model = setup_model_from_checkpoint(a.checkpoint).eval().to(a.device)
     if a.scaling_w is not None:
         model.blender.scaling_w = float(a.scaling_w)
     rows = evaluate(model, synthetic_items(a.num_samples, a.is_video, a.num_frames, a.size[0], a.size[-1], a.device), a.is_video,
-                    a.output_dir, a.num_frames, a.video_aggregation, lowres_attenuation=a.lowres_attenuation,
+                    a.output_dir, a.num_frames, a.video_aggregation, interpolation=interpolation_of(a), lowres_attenuation=a.lowres_attenuation,
                     image_metrics=a.image_metrics)
     keys = [k for k in rows[0] if k not in ("iteration", "t", "h", "w")]
     print({k: sum(r[k] for r in rows) / len(rows) for k in keys})

@@ -90,6 +90,20 @@ def _bool(s: str) -> bool:
     return str(s).lower() in ("1", "true", "yes", "y")
 
 
+def add_interpolation_args(ap: argparse.ArgumentParser):
+    """the reference CLIs' resize options (evals/full.py:296-302, evals/speed.py:186-192), same names, choices and defaults"""
+    ap.add_argument("--interpolation_mode", default="bilinear", choices=["nearest", "bilinear", "bicubic", "area"],
+                    help="interpolation mode for resizing")
+    ap.add_argument("--interpolation_align_corners", type=_bool, default=False, help="align corners for interpolation")
+    ap.add_argument("--interpolation_antialias", type=_bool, default=True, help="use antialiasing for interpolation")
+
+
+def interpolation_of(a: argparse.Namespace) -> dict:
+    """the dict the reference builds from those options, all three keys set (evals/full.py:345-349, evals/speed.py:215-219).  As
+    there, nearest and area raise ValueError on frames that are resized: the dict always carries align_corners."""
+    return {"mode": a.interpolation_mode, "align_corners": a.interpolation_align_corners, "antialias": a.interpolation_antialias}
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(description="embed / extraction speed of a card or checkpoint on this backend")
     ap.add_argument("--checkpoint", nargs="+", required=True)
@@ -106,7 +120,7 @@ def main(argv=None):
     ap.add_argument("--videoseal_chunk_size", type=int, default=32)
     ap.add_argument("--videoseal_step_size", type=int, default=4)
     ap.add_argument("--videoseal_mode", default="repeat")
-    ap.add_argument("--interpolation_antialias", type=_bool, default=True)
+    add_interpolation_args(ap)
     ap.add_argument("--output_dir", default="output/speed")
     ap.add_argument("--output_file", default="speed_results.csv")
     a = ap.parse_args(argv)
@@ -119,7 +133,7 @@ def main(argv=None):
         if a.scaling_w is not None:
             model.blender.scaling_w = float(a.scaling_w)
         model.chunk_size, model.step_size, model.video_mode = a.videoseal_chunk_size, a.videoseal_step_size, a.videoseal_mode
-        interp = {"mode": "bilinear", "align_corners": False, "antialias": a.interpolation_antialias}
+        interp = interpolation_of(a)
         res = SpeedTester(a.device).test_speed(model, synthetic_items(a.num_samples, a.is_video, a.num_frames, h, w, a.device),
                                                a.is_video, a.num_frames, a.video_aggregation, a.lowres_attenuation, interp,
                                                a.num_runs, a.warmup_runs)

@@ -19,6 +19,39 @@ from . import _lib
 _DEF_INTERP = {"mode": "bilinear", "align_corners": False, "antialias": True}
 
 
+def resize_flags(interpolation: dict, resizes: bool) -> int:
+    """The resize bits of vsb_flags for the reference's `interpolation` dict, which it passes as F.interpolate(x, size=...,
+    **interpolation) at both resize sites (wam.py:161-164, :183-185; videoseal.py:305, :329).  The reference calls F.interpolate only
+    when the frames are not img_size x img_size (`resizes`); then this raises what F.interpolate raises for the dict: TypeError for
+    a key it does not take, ValueError for align_corners with nearest / area, antialias with them, or a scale_factor next to the
+    size.  Modes other than bilinear, bicubic, nearest and area raise NotImplementedError (as F.interpolate does for 4-D 'linear' /
+    'trilinear'; 'nearest-exact' is not implemented here).  No device work: testable on the CPU."""
+    if not resizes:
+        return 0
+    unknown = sorted(set(interpolation) - {"mode", "align_corners", "antialias", "scale_factor", "recompute_scale_factor"})
+    if unknown:
+        raise TypeError(f"interpolate() got an unexpected keyword argument '{unknown[0]}'")
+    mode = interpolation.get("mode", "nearest")                      # F.interpolate's defaults
+    align_corners = interpolation.get("align_corners")
+    antialias = bool(interpolation.get("antialias", False))
+    if mode in ("nearest", "area", "nearest-exact") and align_corners is not None:
+        raise ValueError("align_corners option can only be set with the interpolating modes: linear | bilinear | bicubic | trilinear")
+    if interpolation.get("scale_factor") is not None:
+        raise ValueError("only one of size or scale_factor should be defined")
+    if interpolation.get("recompute_scale_factor"):
+        raise ValueError("recompute_scale_factor is not meaningful with an explicit size.")
+    if antialias and mode not in ("bilinear", "bicubic"):
+        raise ValueError("Anti-alias option is restricted to bilinear and bicubic modes and requires a 4-D tensor as input")
+    if mode not in _lib.RESIZE_MODES:
+        raise NotImplementedError(f"interpolation mode {mode!r} is not implemented (bilinear, bicubic, nearest, area)")
+    f = _lib.RESIZE_MODES[mode] << _lib.FLAG_RESIZE_MODE_SHIFT
+    if align_corners:
+        f |= _lib.FLAG_RESIZE_ALIGN_CORNERS
+    if not antialias:
+        f |= _lib.FLAG_RESIZE_NO_AA
+    return f
+
+
 def native_desc(spec: dict) -> _lib.ModelDesc:
     """vsb_model_desc of `spec` (cfg.spec_from_card)"""
     d = _lib.ModelDesc()
@@ -159,7 +192,7 @@ class _Detector:
         self._owner = owner
 
     def __call__(self, imgs_res: torch.Tensor) -> torch.Tensor:
-        return self._owner._detect_dev(self._owner._to_dev(imgs_res), True)
+        return self._owner._detect_dev(self._owner._to_dev(imgs_res), 0)
 
 
 class Videoseal(nn.Module):
@@ -289,18 +322,16 @@ class Videoseal(nn.Module):
         # thresholded on the side the tensor lives on: a host tensor (the usual case) costs one small H2D copy and no device kernel
         return (msgs > 0.5).to(torch.uint8).contiguous().to(self.device)
 
-    def _flags(self, interpolation: dict, lowres: bool = False) -> int:
-        if interpolation.get("mode", "bilinear") != "bilinear" or interpolation.get("align_corners", False):
-            raise NotImplementedError("only bilinear, align_corners=False interpolation is implemented")
-        f = 0
+    def _flags(self, interpolation: dict, lowres: bool = False, hw: Optional[tuple] = None) -> int:
+        """vsb_flags of an embed / detect call on H x W frames (hw; None: as if they were resized)"""
+        S = self.spec["img_size"]
+        f = resize_flags(interpolation, hw is None or tuple(hw) != (S, S))
         if self.clamp:
             f |= _lib.FLAG_CLAMP
         if lowres:
             f |= _lib.FLAG_LOWRES_ATTN
         if self.attenuation is None:
             f |= _lib.FLAG_NO_ATTENUATION
-        if not interpolation.get("antialias", False):
-            f |= _lib.FLAG_RESIZE_NO_AA
         return f
 
     # ------------------------------------------------------------------ public API
@@ -314,6 +345,7 @@ class Videoseal(nn.Module):
         if imgs.dim() != 4 or imgs.shape[1] != 3:
             raise ValueError("imgs must be [F, 3, H, W]")
         F_, H, W = imgs.shape[0], imgs.shape[2], imgs.shape[3]
+        flags = self._flags(interpolation, lowres_attenuation, (H, W))
         if msgs is None:
             msgs = self.get_random_msg(F_ if not is_video else 1)
         elif is_video:
@@ -333,7 +365,7 @@ class Videoseal(nn.Module):
         _lib.check(_lib.lib().vsb_embed(
             self._handle(), x.data_ptr(), mm.data_ptr(), mm.shape[0], imgs_w.data_ptr(),
             preds_w.data_ptr() if preds_w is not None else None, F_, H, W, step, _lib.VIDEO_MODES[self.video_mode],
-            int(self.chunk_size), float(self.blender.scaling_i), float(self.blender.scaling_w), self._flags(interpolation, lowres_attenuation),
+            int(self.chunk_size), float(self.blender.scaling_i), float(self.blender.scaling_w), flags,
             self._stream()))
         if is_video:
             return {"imgs_w": imgs_w.to(imgs.device), "msgs": msgs[0:1].repeat(F_, 1)}
@@ -344,7 +376,7 @@ class Videoseal(nn.Module):
         """True when detect() returns per-pixel maps [F, 1+K, P, P] (pixel_decoder.pixelwise of the card)."""
         return bool(self.spec.get("pixel_decoder", {}).get("pixelwise", False))
 
-    def _detect_dev(self, x: torch.Tensor, antialias: bool) -> torch.Tensor:
+    def _detect_dev(self, x: torch.Tensor, flags: int) -> torch.Tensor:
         shape = (x.shape[0], 1 + self.spec["nbits"])
         if self.pixelwise:   # trunk map (img_size / 32, a ViT's img_size / 16) x the product of the stage factors
             P = trunk_map(self.spec)
@@ -352,7 +384,6 @@ class Videoseal(nn.Module):
                 P *= f
             shape += (P, P)
         out = torch.empty(shape, device=x.device, dtype=torch.float32)
-        flags = 0 if antialias else _lib.FLAG_RESIZE_NO_AA
         _lib.check(_lib.lib().vsb_detect(self._handle(), x.data_ptr(), out.data_ptr(), x.shape[0], x.shape[2], x.shape[3], flags,
                                          self._stream()))
         return out
@@ -362,8 +393,8 @@ class Videoseal(nn.Module):
         """models/videoseal.py:352-388; frames are independent so the chunk loop is internal to the library."""
         if not is_video:
             interpolation = _DEF_INTERP       # the reference drops `interpolation` on this branch (videoseal.py:374)
-        self._flags(interpolation)            # validates the interpolation dict
-        preds = self._detect_dev(self._to_dev(imgs), bool(interpolation.get("antialias", False)))
+        flags = resize_flags(interpolation, tuple(imgs.shape[-2:]) != (self.img_size, self.img_size))
+        preds = self._detect_dev(self._to_dev(imgs), flags)
         return {"preds": preds.to(imgs.device)}
 
     def extract_message(self, imgs: torch.Tensor, aggregation: str = "avg",
