@@ -192,6 +192,32 @@ int64_t vsb_quality_workspace_bytes(int32_t B, int32_t C, int32_t H, int32_t W, 
 int vsb_ssim(const float* x_dev, const float* y_dev, int32_t B, int32_t C, int32_t H, int32_t W, float data_range,
              float* ssim_out_dev, float* msssim_out_dev, void* workspace_dev, int64_t workspace_bytes, void* stream);
 
+/* ---- validation augmentations (handle-less)  <-  augmentation/geometric.py, valuemetric.py as get_validation_augs lists them
+ * (evals/full.py:188-239).  x_dev [B,3,H,W] fp32 contiguous, y_dev [B,3,OH,OW] (OH, OW = H, W for every op but crop, resize
+ * and the grid ops); y_dev must not overlap x_dev.  params are host floats, n_params of them:
+ *   VSB_AUG_CROP_FLIP      {i, j, flip}: y = x[..., i:i+OH, j:j+OW], mirrored along W when flip != 0      (F.crop, F.hflip)
+ *   VSB_AUG_GRID_*         {t00, t01, t10, t11, t20, t21, c6, c7, perspective}: torchvision's rescaled theta [3][2] (and the
+ *                          perspective denominator's coefficients); aux_dev holds the base grid, [OW] x then [OH] y values as
+ *                          torch.linspace makes them.  grid_sample, align_corners=False, zero padding    (F.rotate, F.perspective)
+ *   VSB_AUG_BRIGHTNESS / CONTRAST / SATURATION  {f, 1 - f} rounded to fp32: clamp(f x + (1 - f) o, 0, 1), o = 0, the image's mean
+ *                          grayscale, the pixel's grayscale                        (F.adjust_brightness / contrast / saturation)
+ *   VSB_AUG_HUE            {hue_factor}                                             (F.adjust_hue)
+ *   VSB_AUG_GRAYSCALE      {}: 0.299 r + 0.587 g + 0.114 b on all three channels    (the reference's Grayscale)
+ *   VSB_AUG_BLUR           k fp32 taps (k odd, <= 33): the separable form of F.gaussian_blur, reflect padding
+ *   VSB_AUG_JPEG           {quality}: PIL's JPEG save and load (4:2:0, islow DCT, fancy upsampling), bit-exact, then the
+ *                          reference's pass-through (jpeg - x) + x on the clamped input                    (utils/image.py:13-34)
+ *   VSB_AUG_RESIZE         {}: bilinear, antialias=True, align_corners=False, H x W -> OH x OW           (F.resize)
+ * The caller supplies vsb_augment_workspace_bytes(op, B, H, W) bytes of device workspace (16-byte aligned; 0 = none needed).
+ * Deterministic: the contrast mean is a fixed-order fp64 sum.  Runs on x_dev's device; VSB_ERR_UNSUPPORTED on anything but
+ * compute capability 9.0; arguments are checked before any CUDA call. */
+enum vsb_aug_op {
+  VSB_AUG_CROP_FLIP = 0, VSB_AUG_GRID_NEAREST = 1, VSB_AUG_GRID_BILINEAR = 2, VSB_AUG_BRIGHTNESS = 3, VSB_AUG_CONTRAST = 4,
+  VSB_AUG_SATURATION = 5, VSB_AUG_HUE = 6, VSB_AUG_GRAYSCALE = 7, VSB_AUG_BLUR = 8, VSB_AUG_JPEG = 9, VSB_AUG_RESIZE = 10
+};
+int64_t vsb_augment_workspace_bytes(int32_t op, int32_t B, int32_t H, int32_t W);   /* host-only; < 0 on error */
+int vsb_augment(int32_t op, const float* x_dev, float* y_dev, int32_t B, int32_t C, int32_t H, int32_t W, int32_t OH, int32_t OW,
+                const float* params, int32_t n_params, const float* aux_dev, void* workspace_dev, int64_t workspace_bytes, void* stream);
+
 /* ---- debug / test seams (used by tests/ only) ------------------------------------------------------------- */
 /* copy a named intermediate activation of the most recent embed/detect sub-batch to the host as fp32.
  * shape4 receives [B, H, W, C] (NHWC) or [M, C, 1, 1]-style dims; returns the element count or <0. */

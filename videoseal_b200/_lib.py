@@ -14,6 +14,7 @@ EXPORTS = [
     "vsb_model_destroy", "vsb_embed", "vsb_embedder_forward", "vsb_detect", "vsb_jnd_heatmaps", "vsb_embed_host",
     "vsb_detect_host", "vsb_embed_detect_host", "vsb_frames_host_u8", "vsb_launch_count", "vsb_profile_enable", "vsb_profile_read", "vsb_debug_get_tensor", "vsb_debug_keep_inputs", "vsb_debug_conv",
     "vsb_debug_resample_table", "vsb_debug_resample_table2", "vsb_debug_last_dispatch", "vsb_quality_workspace_bytes", "vsb_ssim", "vsb_model_set_vit_extractor",
+    "vsb_augment_workspace_bytes", "vsb_augment",
 ]
 
 FLAG_CLAMP, FLAG_LOWRES_ATTN, FLAG_NO_ATTENUATION, FLAG_RESIZE_NO_AA = 1, 2, 4, 8
@@ -108,6 +109,10 @@ def lib():
     L.vsb_quality_workspace_bytes.restype = C.c_int64
     L.vsb_ssim.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_void_p,
                            C.c_void_p, C.c_int64, C.c_void_p]
+    L.vsb_augment_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32]
+    L.vsb_augment_workspace_bytes.restype = C.c_int64
+    L.vsb_augment.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                              C.POINTER(C.c_float), C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
     _lib = L
     return L
 

@@ -1326,7 +1326,7 @@ class Model {
     for (int i = 0; i < n; i += 16384) {   // gridDim.y limit: split very long frame ranges
       const int m = std::min(16384, n - i);
       prof_scope("pw.resize." + std::to_string(H) + "x" + std::to_string(W) + "@" + std::to_string(m), st, 1, [&] {
-        launch_resize(*r, src + (long)i * frame_stride, frame_stride, m, H, W, S, dst + (size_t)i * 3 * S * S, last_resize, st);
+        launch_resize(*r, src + (long)i * frame_stride, frame_stride, m, H, W, S, S, dst + (size_t)i * 3 * S * S, last_resize, st);
       });
     }
   }

@@ -233,18 +233,18 @@ struct ResampleDev {
   }
 };
 
-// resample n <= 16384 frames that are `frame_stride` floats apart, H x W -> S x S (the table pair r); rec: MT, GST, vec, toy, OW
-inline void launch_resize(const ResampleDev& r, const float* src, long frame_stride, int n, int H, int W, int S, float* dst, int32_t rec[5],
-                          cudaStream_t st) {
+// resample n <= 16384 frames that are `frame_stride` floats apart, H x W -> OH x OW (the table pair r); rec: MT, GST, vec, toy, OW
+inline void launch_resize(const ResampleDev& r, const float* src, long frame_stride, int n, int H, int W, int OH, int OW, float* dst,
+                          int32_t rec[5], cudaStream_t st) {
   // (checked here, not when the table is built: the blend only reads the delta up-sampler's table, whatever its width)
   if (r.smem > 200 * 1024) throw Error("resize: image too wide for the shared-memory resample kernel (not implemented)", kErrUnsupported);
   const int vec = (W % 4 == 0) && (reinterpret_cast<uintptr_t>(src) % 16 == 0) && (frame_stride % 4 == 0);
-  const dim3 grid((S + r.toy - 1) / r.toy, n * 3);
+  const dim3 grid((OH + r.toy - 1) / r.toy, n * 3);
   const int mt = r.tab.maxt_x <= 2 ? 2 : (r.tab.maxt_x <= 8 ? 8 : 0);
-  const int32_t rc[5] = {mt, r.gstage, vec, r.toy, S};
+  const int32_t rc[5] = {mt, r.gstage, vec, r.toy, OW};
   std::copy(rc, rc + 5, rec);
 #define VSB_RS(MT, GS) do { smem_optin<resize_sep_kernel<MT, GS>>(200 * 1024); \
-    resize_sep_kernel<MT, GS><<<grid, 256, r.smem, st>>>(src, frame_stride, dst, H, W, S, S, r.tab, r.toy, r.rin_max, vec); } while (0)
+    resize_sep_kernel<MT, GS><<<grid, 256, r.smem, st>>>(src, frame_stride, dst, H, W, OH, OW, r.tab, r.toy, r.rin_max, vec); } while (0)
   if (r.gstage == 4) { if (mt == 2) VSB_RS(2, 4); else if (mt == 8) VSB_RS(8, 4); else VSB_RS(0, 4); }
   else if (r.gstage == 2) { if (mt == 2) VSB_RS(2, 2); else if (mt == 8) VSB_RS(8, 2); else VSB_RS(0, 2); }
   else { if (mt == 2) VSB_RS(2, 1); else if (mt == 8) VSB_RS(8, 1); else VSB_RS(0, 1); }

@@ -2,6 +2,7 @@
 //   nvcc -std=c++17 -O3 -lineinfo -gencode arch=compute_90a,code=sm_90a -shared -Xcompiler -fPIC vsb200.cu -o libvsb200.so
 #include "model.cuh"
 #include "quality_host.cuh"
+#include "augment_host.cuh"
 
 using namespace vsb;
 
@@ -388,15 +389,22 @@ int64_t vsb_quality_workspace_bytes(int32_t B, int32_t C, int32_t H, int32_t W, 
 }
 
 // device of a CUDA allocation; VSB_ERR_INVALID for host memory
-static int quality_device_of(const void* p, const char* what) {
+static int device_of(const void* p, const char* what, const char* who = "vsb_ssim") {
   cudaPointerAttributes a;
   const cudaError_t e = cudaPointerGetAttributes(&a, p);
   if (e != cudaSuccess) {
     cudaGetLastError();
-    throw Error(std::string("vsb_ssim: cannot query ") + what + ": " + cudaGetErrorString(e), kErrCuda);
+    throw Error(std::string(who) + ": cannot query " + what + ": " + cudaGetErrorString(e), kErrCuda);
   }
-  if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) throw Error(std::string("vsb_ssim: ") + what + " is not CUDA device memory");
+  if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) throw Error(std::string(who) + ": " + what + " is not CUDA device memory");
   return a.device;
+}
+
+static void require_sm90(int dev) {
+  int major = 0, minor = 0;
+  VSB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
+  VSB_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
+  if (major != 9 || minor != 0) throw Error("libvsb200 is built for sm_90a only (found sm_" + std::to_string(major) + std::to_string(minor) + ")", kErrUnsupported);
 }
 
 int vsb_ssim(const float* x, const float* y, int32_t B, int32_t C, int32_t H, int32_t W, float data_range, float* ssim_out,
@@ -409,16 +417,44 @@ int vsb_ssim(const float* x, const float* y, int32_t B, int32_t C, int32_t H, in
   VSB_CHECK(reinterpret_cast<uintptr_t>(workspace) % 16 == 0, "vsb_ssim: workspace must be 16-byte aligned");
   const QualityLayout L = quality_layout(B, C, H, W, msssim_out != nullptr);
   VSB_CHECK(workspace_bytes >= (int64_t)L.bytes, "vsb_ssim: workspace smaller than vsb_quality_workspace_bytes()");
-  const int dev = quality_device_of(x, "x");
-  VSB_CHECK(quality_device_of(y, "y") == dev && quality_device_of(workspace, "workspace") == dev &&
-                (!ssim_out || quality_device_of(ssim_out, "ssim_out") == dev) && (!msssim_out || quality_device_of(msssim_out, "msssim_out") == dev),
+  const int dev = device_of(x, "x");
+  VSB_CHECK(device_of(y, "y") == dev && device_of(workspace, "workspace") == dev &&
+                (!ssim_out || device_of(ssim_out, "ssim_out") == dev) && (!msssim_out || device_of(msssim_out, "msssim_out") == dev),
             "vsb_ssim: x, y, the outputs and the workspace must be on one device");
   DeviceGuard dg(dev);
-  int major = 0, minor = 0;
-  VSB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  VSB_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
-  if (major != 9 || minor != 0) throw Error("libvsb200 is built for sm_90a only (found sm_" + std::to_string(major) + std::to_string(minor) + ")", kErrUnsupported);
+  require_sm90(dev);
   quality_run(L, x, y, B, C, data_range, ssim_out, msssim_out, (char*)workspace, (cudaStream_t)stream);
+  return VSB_OK;
+  VSB_API_END
+}
+
+int64_t vsb_augment_workspace_bytes(int32_t op, int32_t B, int32_t H, int32_t W) {
+  try {
+    return (int64_t)aug_workspace_bytes(op, B, H, W);
+  } catch (const vsb::Error& e) {
+    g_err = e.what();
+    return e.code;
+  } catch (const std::exception& e) {
+    g_err = e.what();
+    return VSB_ERR_INVALID;
+  }
+}
+
+int vsb_augment(int32_t op, const float* x, float* y, int32_t B, int32_t C, int32_t H, int32_t W, int32_t OH, int32_t OW, const float* params,
+                int32_t n_params, const float* aux, void* workspace, int64_t workspace_bytes, void* stream) {
+  VSB_API_BEGIN
+  VSB_CHECK(x && y, "vsb_augment: null argument");
+  aug_check(op, B, C, H, W, OH, OW, params, n_params, aux);
+  const size_t need = aug_workspace_bytes(op, B, H, W);
+  VSB_CHECK(need == 0 || (workspace && workspace_bytes >= (int64_t)need), "vsb_augment: workspace smaller than vsb_augment_workspace_bytes()");
+  VSB_CHECK(reinterpret_cast<uintptr_t>(workspace) % 16 == 0, "vsb_augment: workspace must be 16-byte aligned");
+  const char* who = "vsb_augment";
+  const int dev = device_of(x, "x", who);
+  VSB_CHECK(device_of(y, "y", who) == dev && (!aux || device_of(aux, "aux", who) == dev) && (need == 0 || device_of(workspace, "workspace", who) == dev),
+            "vsb_augment: x, y, aux and the workspace must be on one device");
+  DeviceGuard dg(dev);
+  require_sm90(dev);
+  aug_run(op, x, y, B, H, W, OH, OW, params, n_params, aux, (char*)workspace, (cudaStream_t)stream);
   return VSB_OK;
   VSB_API_END
 }

@@ -4,7 +4,12 @@ column names (`psnr`, `ssim`, `msssim`, `bit_acc_Identity_0`, `pvalue_Identity_0
 `capacity_Identity_0`, `embed_time`, `extract_time`, ...), so that its reports line up with the reference's own runs.
 `image_metrics` picks the quality columns: PSNR by default; "ssim" and "msssim" run on the GPU (evals/metrics.py), and
 image_metrics=("psnr", "ssim", "msssim") gives the reference's columns (full.py:132-142) without LPIPS / VMAF.
-The augmentation bank (JPEG / H264 / crops ...), LPIPS / VMAF and the image dumps need packages outside this path."""
+With only_identity=False each item's imgs_w also goes through the reference's validation bank (augmentation.get_validation_augs,
+run by the GPU kernels of videoseal_b200.augmentation) at frame resolution before detection, and every (augmentation, strength)
+adds its `bit_acc_<key>` / `pvalue_<key>` / `log_pvalue_<key>` / `capacity_<key>` group in the reference's order and key rule
+(full.py:188-239).  Deviation: only_identity defaults to True here (the reference's default is False), so that a default run keeps
+its Identity-only columns; `extract_time` times the Identity detection.  The video codecs (H264 / H265 / VP9), LPIPS / VMAF, the
+detection (mask IoU) columns and the image dumps need packages outside this path."""
 from __future__ import annotations
 
 import math
@@ -29,8 +34,13 @@ def _sync(x: torch.Tensor):
 @torch.no_grad()
 def evaluate(model, dataset: Iterable, is_video: bool, output_dir: str, num_frames: int = 24 * 3, video_aggregation: str = "avg",
              decoding: bool = True, interpolation: dict = _DEF_INTERP, lowres_attenuation: bool = False,
-             skip_image_metrics: bool = False, image_metrics: Iterable[str] = ("psnr",)):
+             skip_image_metrics: bool = False, image_metrics: Iterable[str] = ("psnr",), only_identity: bool = True,
+             only_combined: bool = False, validation_augs: list | None = None):
     image_metrics = set(image_metrics)
+    augs = None
+    if decoding and (validation_augs is not None or not only_identity):
+        from ..augmentation import get_validation_augs
+        augs = validation_augs if validation_augs is not None else get_validation_augs(is_video, only_identity, only_combined)
     unknown = image_metrics - set(IMAGE_METRICS)
     if unknown:
         raise ValueError(f"unknown image metrics {sorted(unknown)}; choose from {IMAGE_METRICS}")
@@ -77,12 +87,38 @@ def evaluate(model, dataset: Iterable, is_video: bool, output_dir: str, num_fram
                 m["pvalue_Identity_0"] = pv
                 m["log_pvalue_Identity_0"] = -math.log10(pv) if pv > 0 else -100
                 m["capacity_Identity_0"] = capacity(bit_preds, tgt).nanmean().item()
+                if augs is not None:
+                    m.update(_augmented_rows(model, imgs_w, tgt, augs, is_video, video_aggregation, interpolation))
             all_metrics.append(m)
             if len(all_metrics) == 1:
                 f.write(",".join(m.keys()) + "\n")
             f.write(",".join(map(str, m.values())) + "\n")
             f.flush()
     return all_metrics
+
+
+def _decode_stats(bit_preds: torch.Tensor, tgt: torch.Tensor, key: str) -> dict:
+    pv = pvalue(bit_preds, tgt).nanmean().item()
+    return {f"bit_acc_{key}": bit_accuracy(bit_preds, tgt).nanmean().item(), f"pvalue_{key}": pv,
+            f"log_pvalue_{key}": -math.log10(pv) if pv > 0 else -100, f"capacity_{key}": capacity(bit_preds, tgt).nanmean().item()}
+
+
+def _augmented_rows(model, imgs_w, tgt, augs, is_video, video_aggregation, interpolation) -> dict:
+    """The column groups of every (augmentation, strength) after Identity_0, which the caller has already written."""
+    from ..augmentation import column_key
+    out = {}
+    for aug, strengths in augs:
+        for strength in strengths:
+            key = column_key(aug, strength)
+            if key == "Identity_0":
+                continue
+            imgs_aug, _ = aug(imgs_w, None, strength)
+            if is_video:
+                bit_preds = model.extract_message(imgs_aug, video_aggregation, interpolation).float() * 2 - 1
+            else:
+                bit_preds = model.detect(imgs_aug, is_video=False)["preds"][:, 1:]
+            out.update(_decode_stats(bit_preds.cpu(), tgt, key))
+    return out
 
 
 def main(argv=None):
@@ -102,6 +138,9 @@ def main(argv=None):
     ap.add_argument("--output_dir", default="output/full")
     ap.add_argument("--image_metrics", nargs="+", default=["psnr"], choices=IMAGE_METRICS,
                     help="quality columns (psnr ssim msssim gives the reference's; ssim / msssim need the GPU)")
+    ap.add_argument("--only_identity", type=_bool, default=True,
+                    help="only the Identity rows (the reference defaults to False: the whole validation bank)")
+    ap.add_argument("--only_combined", type=_bool, default=False, help="with --only_identity False: only the combined augmentations")
     add_interpolation_args(ap)
     a = ap.parse_args(argv)
     model = setup_model_from_checkpoint(a.checkpoint).eval().to(a.device)
@@ -109,7 +148,7 @@ def main(argv=None):
         model.blender.scaling_w = float(a.scaling_w)
     rows = evaluate(model, synthetic_items(a.num_samples, a.is_video, a.num_frames, a.size[0], a.size[-1], a.device), a.is_video,
                     a.output_dir, a.num_frames, a.video_aggregation, interpolation=interpolation_of(a), lowres_attenuation=a.lowres_attenuation,
-                    image_metrics=a.image_metrics)
+                    image_metrics=a.image_metrics, only_identity=a.only_identity, only_combined=a.only_combined)
     keys = [k for k in rows[0] if k not in ("iteration", "t", "h", "w")]
     print({k: sum(r[k] for r in rows) / len(rows) for k in keys})
 
