@@ -45,8 +45,9 @@ propagation `ln_tol` (two-pass fp32 statistics, fallback to the output range whe
 * head linear: a C-term fp32 dot product per lane stride + butterfly + bias, (C / 32 + 8) K22 A.
 
 A ratio err / tol above 1 is a bug to find, never a reason to raise a constant.  Each step family also has mutations: a reference
-with one deliberate defect that the GPU output must violate.  A mutation's footprint is None (anywhere), "last_frame", or an int w:
-the w outermost rows / columns of every map.
+with one deliberate defect that the GPU output must violate.  A mutation's footprint is None (anywhere), "last_frame", an int w:
+the w outermost rows / columns of every map, or "tile_edge": the 3 outermost rows / columns of every 16 x 16 tile (the pixel
+decoder's tiled gathers, tests/pd_kernels.py).
 """
 from __future__ import annotations
 
@@ -111,10 +112,20 @@ def frame_border(h: int, w: int, width: int, device) -> torch.Tensor:
     return m
 
 
+def tile_edge(h: int, w: int, device) -> torch.Tensor:
+    """the 3 outermost rows / columns of every 16 x 16 output tile: the pixels whose bilinear corners (factor 2 or 4) reach into
+    the one-pixel halo of the tile's low-resolution taps"""
+    r, c = torch.arange(h, device=device) % 16, torch.arange(w, device=device) % 16
+    er, ec = (r < 3) | (r >= 13), (c < 3) | (c >= 13)
+    return er[:, None] | ec[None, :]
+
+
 def outside(v: torch.Tensor, where) -> int:
     """violations of a mutation that lie off its footprint"""
     if where == "last_frame":
         return int(v[:-1].sum())
+    if where == "tile_edge":
+        return int((v & ~tile_edge(v.shape[-2], v.shape[-1], v.device)).sum())
     if isinstance(where, int):
         return int((v & ~frame_border(v.shape[-2], v.shape[-1], where, v.device)).sum())
     return 0

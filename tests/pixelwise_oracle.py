@@ -66,10 +66,11 @@ def extractor_forward(sd, spec, x: torch.Tensor, taps: Optional[dict] = None) ->
     The trunk is restate.convnext_extractor_forward's, read from its `stage3` tap; its pooled head runs on zero weights that stand
     in for the pixel-wise decoder's keys (a 3x3 conv on the last map, discarded)."""
     c = spec["convnext"]["dims"][-1]
-    pooled = {D + "output_upscaling.0.upsample_block.2.weight": torch.zeros(c, c, 3, 3),
-              D + "output_upscaling.0.upsample_block.3.weight": torch.ones(c),
-              D + "output_upscaling.0.upsample_block.3.bias": torch.zeros(c),
-              D + "linear.weight": torch.zeros(1, c), D + "linear.bias": torch.zeros(1)}
+    z = dict(dtype=x.dtype)
+    pooled = {D + "output_upscaling.0.upsample_block.2.weight": torch.zeros(c, c, 3, 3, **z),
+              D + "output_upscaling.0.upsample_block.3.weight": torch.ones(c, **z),
+              D + "output_upscaling.0.upsample_block.3.bias": torch.zeros(c, **z),
+              D + "linear.weight": torch.zeros(1, c, **z), D + "linear.bias": torch.zeros(1, **z)}
     t = {} if taps is None else taps
     restate.convnext_extractor_forward({**sd, **pooled}, spec, x, t)
     x = t["stage3"]

@@ -157,14 +157,14 @@ def ln_relu_check(step, got, pre, e, g, beta, muts) -> Check:
     return ck
 
 
-def gather(y: torch.Tensor, C: int, align_corners=False, pad="reflect") -> torch.Tensor:
-    """y [B, 9 C, h, w] (tap-major channels, tap = 3 r + s) -> sum_taps shift(pad(bilinear_x2(y_tap))), [B, C, 2h, 2w]"""
+def gather(y: torch.Tensor, C: int, align_corners=False, pad="reflect", f: int = 2) -> torch.Tensor:
+    """y [B, 9 C, h, w] (tap-major channels, tap = 3 r + s) -> sum_taps shift(pad(bilinear_xf(y_tap))), [B, C, f h, f w]"""
     B, _, h, w = y.shape
-    out = torch.zeros(B, C, 2 * h, 2 * w, dtype=y.dtype, device=y.device)
+    out = torch.zeros(B, C, f * h, f * w, dtype=y.dtype, device=y.device)
     for t in range(9):
         r, s = divmod(t, 3)
-        u = F.interpolate(y[:, t * C:(t + 1) * C], scale_factor=2, mode="bilinear", align_corners=align_corners)
-        out += F.pad(u, (1, 1, 1, 1), mode=pad)[:, :, r:r + 2 * h, s:s + 2 * w]
+        u = F.interpolate(y[:, t * C:(t + 1) * C], scale_factor=f, mode="bilinear", align_corners=align_corners)
+        out += F.pad(u, (1, 1, 1, 1), mode=pad)[:, :, r:r + f * h, s:s + f * w]
     return out
 
 

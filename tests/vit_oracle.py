@@ -28,8 +28,9 @@ Q = "detector.image_encoder."
 SEED = 1234
 
 
-def vit_card(pixelwise: bool = False, img_size: Optional[int] = None, encoder: Optional[dict] = None) -> dict:
-    """videoseal_1.0 args and U-Net + the videoseal_0.0 extractor block (encoder keys overridden by `encoder`)"""
+def vit_card(pixelwise: bool = False, img_size: Optional[int] = None, encoder: Optional[dict] = None, stages=(4, 2, 2)) -> dict:
+    """videoseal_1.0 args and U-Net + the videoseal_0.0 extractor block (encoder keys overridden by `encoder`); a pixel-wise card
+    has the upscale factors `stages`"""
     from tests.util import load_card
     card = load_card("videoseal_1.0")
     card["extractor"] = copy.deepcopy(load_card("videoseal_0.0")["extractor"])
@@ -37,7 +38,7 @@ def vit_card(pixelwise: bool = False, img_size: Optional[int] = None, encoder: O
         card["extractor"]["params"]["encoder"].update(encoder)
     if pixelwise:
         card["extractor"]["model"] = "sam_small_pw"
-        card["extractor"]["params"]["pixel_decoder"].update({"pixelwise": True, "upscale_stages": [4, 2, 2]})
+        card["extractor"]["params"]["pixel_decoder"].update({"pixelwise": True, "upscale_stages": list(stages)})
     if img_size is not None:
         card["args"]["img_size_proc"] = img_size
     return card

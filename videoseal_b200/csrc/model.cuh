@@ -1286,6 +1286,7 @@ class Model {
       ConvGemmOp op; setup_tma_gemm(op, x, Mi, s.kin, ldx);
       op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.out16 = ytap; op.p.ld_out16 = 9 * Co;
       add_conv(pl, op, s.taps, "pd.uptap1x1." + std::to_string(s.cin) + "-" + std::to_string(9 * Co) + "@" + std::to_string(h));
+      dbg(pl, "pd" + std::to_string(i) + "_y", ytap, 1, B, h, h, 9 * Co, 9 * Co);
       UpsGather g;
       g.y = ytap; g.B = B; g.IH = IH; g.C = Co; g.lnw = s.lnw; g.lnb = s.lnb; g.num_sms = nsm; g.optin = kPdMaxSmem;
       g.smem = s.smem;

@@ -51,6 +51,9 @@ inline void launch_ups_gather_t(const UpsGather& g, cudaStream_t st) {
     if (!g.smem) {
       const int ppb = 256 / (g.C / (8 * VPT));
       const long npix = (long)g.B * F * g.IH * F * g.IH;
+      // the G lanes of a pixel share LayerNorm sums through full-warp shuffles, which every lane of a warp must reach: no warp may
+      // hold pixels past npix.  Processing sizes are multiples of 128, so every map is a multiple of 4 pixels and this holds.
+      VSB_CHECK(npix % (32 / (g.C / (8 * VPT))) == 0, "up-gather: pixel count not a multiple of the pixels per warp");
       const unsigned grid = (unsigned)std::min<long>((npix + ppb - 1) / ppb, (long)g.num_sms * 32);
       ups_gather_ln_kernel<VPT, F, ACT><<<grid, 256, 0, st>>>(g.y, g.B, g.IH, g.IH, g.C, g.lnw, g.lnb, 1e-6f, g.out, g.ld_out);
       VSB_CUDA(cudaGetLastError());
