@@ -96,7 +96,7 @@ class Trunk:
         return self.sd[self.blk(s) + "pwconv2.weight"]
 
     def bias2(self, s, beta=True):
-        """pwconv2's bias with GRN beta folded in, in float64 (Model::finalize_convnext then rounds it to fp32 once)"""
+        """pwconv2's bias with GRN beta folded in, in float64 (ConvNeXt::pack then rounds it to fp32 once)"""
         k = self.blk(s)
         b = self.sd[k + "pwconv2.bias"]
         return b + self.w2(s) @ self.sd[k + "grn.beta"].reshape(-1) if beta else b

@@ -1,4 +1,4 @@
-"""Float64 references and forward error bounds for every kernel of the pixel-wise decoder (Model::add_pixel_decoder), judged one
+"""Float64 references and forward error bounds for every kernel of the pixel-wise decoder (Decoder::add_pixel_decoder), judged one
 kernel at a time.
 
 Each stage i is a tap GEMM at the low resolution, y = x W_tap (`pd.uptap1x1`, debug tap pd{i}_y [B, h, h, 9 Co], tap-major
@@ -13,7 +13,7 @@ Error bounds (u = 2^-11, u32 = 2^-24, K22 = 2^-22, as in tests/unet_kernels.py):
 
 * `pd.uptap1x1` (TMA GEMM, fp16 weights rounded once on the host, fp32 accumulation, no bias, fp16 output):
   c u A + K 2^-22 A + 1/2 ulp_fp16, A = |W_tap| |x|, K = C_in + 8.  A stage whose input is narrower than its GEMM K (48 channels
-  at K = 64, Model::pd_gemm_k) runs over zero pad columns: the reference uses the C_in real channels only, so pad columns that
+  at K = 64, Decoder::gemm_k) runs over zero pad columns: the reference uses the C_in real channels only, so pad columns that
   did not read as zero would break the bound.
 * The gather's four-corner mix of each tap is one packed fp16 multiply and three packed fma, each rounding at most u times the
   running partial sum (all corner weights are >= 0, so the partial sums are at most T = sum_corners w |y|), plus 2^-25 where a

@@ -155,7 +155,7 @@ def test_dispatch_is_pinned(cfg):
 
 
 def _vpt(c: int) -> int:
-    """Model::pd_vpt: 16-byte vectors per thread of a C-channel intermediate stage"""
+    """Decoder::vpt: 16-byte vectors per thread of a C-channel intermediate stage"""
     return next(v for v in (1, 3) if c % (8 * v) == 0 and (c // (8 * v)) & (c // (8 * v) - 1) == 0 and c // (8 * v) <= 32)
 
 

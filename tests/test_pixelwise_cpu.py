@@ -159,3 +159,21 @@ def test_set_pixel_decoder_error_codes_on_a_valid_descriptor(built_lib):
         assert call([4, 4, 2], 1) == -2
     finally:
         L.vsb_model_destroy(h)
+
+
+def test_set_pixel_decoder_before_the_trunk_has_a_map(built_lib):
+    """A SAM-ViT spec leaves the ConvNeXt stem stride at 0 (unused); before vsb_model_set_vit_extractor the decoder rules must
+    still answer with a status, deciding pooled vs pixel-wise and the stem rule before they ask for the trunk's map."""
+    from videoseal_b200 import _lib, cfg
+    from videoseal_b200.model import native_desc
+    L = _lib.lib()
+    h = C.c_void_p()
+    d = native_desc(cfg.spec_from_card(load_card("videoseal_1.0")))
+    d.ext_stem_stride = 0
+    assert L.vsb_model_create(C.byref(d), C.byref(h)) == 0
+    try:
+        assert L.vsb_model_set_pixel_decoder(h, 1, (C.c_int32 * 1)(1), 0) == 0
+        assert L.vsb_model_set_pixel_decoder(h, 3, (C.c_int32 * 3)(4, 4, 2), 1) == -2
+        assert "needs a ConvNeXt trunk with stem stride 4" in L.vsb_last_error().decode()
+    finally:
+        L.vsb_model_destroy(h)

@@ -193,7 +193,7 @@ def test_mutations_move_the_reference_beyond_the_bound(case):
     imgs, msgs = _inputs(spec, B=2, seed=1)
     taps = _chain(net, imgs, msgs)
     seen = set()
-    # the phase-folded up-conv exists only for [x 32 | skip 32] -> 16 channels (Model::finalize): other levels keep the tap GEMM
+    # the phase-folded up-conv exists only for [x 32 | skip 32] -> 16 channels (UNet::check): other levels keep the tap GEMM
     phase_ok = lambda n: taps[n].shape[1] == 9 * 16
     for gather_path in (True, False):
         for ck in uk.plan_checks(net, lambda n: taps[n], imgs, msgs, lambda n: n in taps and (gather_path or not phase_ok(n))):

@@ -195,7 +195,7 @@ def test_dispatch_is_pinned(cfg):
 
 def _family(name: str) -> str:
     """profile name -> kernel family; the up gather splits by variant (pointwise_host.cuh launch_unet_upgather and the tile rule
-    of build_embed_plan: tiled when the low-resolution side is a multiple of 8 and ups_tile_smem(2, C) <= 160 KB)"""
+    of UNet::build: tiled when the low-resolution side is a multiple of 8 and ups_tile_smem(2, C) <= 160 KB)"""
     fam = name.split(".")[1]
     if fam == "upgather":
         c, ho = (int(v) for v in name.split(".")[2].split("@"))

@@ -4,7 +4,8 @@
 #include <algorithm>
 #include <string>
 #include "augment.cuh"
-#include "model.cuh"
+#include "plan.cuh"
+#include "resize_blend_host.cuh"
 
 namespace vsb {
 

@@ -131,7 +131,7 @@ inline void launch_direct(const Conv3DirectOp& op, cudaStream_t st) {
 // UBlock up-conv (bilinear x2 -> reflect pad -> conv3x3 -> LN -> ReLU, modules/common.py:45-52 + unet.py:187-190) as ONE 3x3 conv
 // on the LOW-resolution grid with 4 x 16 output columns (one group per output phase (oy&1, ox&1)) and replicate padding:
 // away from the image border the bilinear weights depend only on the phase, so they fold into the conv weights
-// (Model::pack_upconv_phase).  The outermost output rows/columns (reflect padding of the up-sampled map) do not follow the
+// (Weights::upconv_phase).  The outermost output rows/columns (reflect padding of the up-sampled map) do not follow the
 // phase pattern and are recomputed exactly by up_border_fix_kernel afterwards.
 inline void setup_up_phase_direct(Conv3DirectOp& op, const __half* x0, int C0, const __half* x1, int C1, int B, int H, int W,
                                   const __half* wpk, const float* ln_w, const float* ln_b, float eps, __half* out, int num_sms) {
@@ -145,7 +145,7 @@ inline void setup_up_phase_direct(Conv3DirectOp& op, const __half* x0, int C0, c
 
 // DBlock.down (unet.py:75: 3x3, stride 2, pad 1, bias) on x [B,2H,2W,Cin] -> [B,H,W,N]: output (Y,X), tap r reads input row
 // 2Y + r - 1 = row (Y-1, dy=1), (Y, dy=0), (Y, dy=1) of the space-to-depth view, i.e. a conv with offsets {-1, 0} only.
-// wpk: weights re-indexed to [N][(ey,ex)][(dy,dx,c)] (Model::pack_down_s2d) in the direct layout.
+// wpk: weights re-indexed to [N][(ey,ex)][(dy,dx,c)] (Weights::down_s2d) in the direct layout.
 inline void setup_down_s2d_direct(Conv3DirectOp& op, const __half* x, int Cin, int B, int H, int W, int N, const __half* wpk,
                                   const float* bias, __half* out, int num_sms) {
   setup_conv3_direct(op, x, B, H, W, 4 * Cin, N, wpk, num_sms, 3, /*s2d=*/true);

@@ -3,7 +3,7 @@
 #pragma once
 #include <cmath>
 #include <string>
-#include "model.cuh"
+#include "plan.cuh"
 #include "quality.cuh"
 
 namespace vsb {

@@ -60,11 +60,7 @@ int vsb_model_create(const vsb_model_desc* desc, vsb_model** out) {
 int vsb_model_set_tensor(vsb_model* m, const char* name, const float* data, const int64_t* shape, int32_t ndim) {
   VSB_API_BEGIN
   VSB_CHECK(m && name && data && (shape || ndim == 0) && ndim >= 0 && ndim <= 4, "bad tensor argument");
-  if (m->impl.finalized) throw Error("model already finalized", kErrState);
-  HostTensor t;
-  t.shape.assign(shape, shape + ndim);
-  t.data.assign(data, data + t.numel());
-  m->impl.sd[name] = std::move(t);
+  m->impl.set_tensor(name, data, shape, ndim);
   return VSB_OK;
   VSB_API_END
 }
@@ -147,21 +143,7 @@ int vsb_embed_host(vsb_model* m, const float* imgs_h, const uint8_t* msgs_h, int
   VSB_API_BEGIN
   VSB_CHECK(m && imgs_h && msgs_h && imgs_w_h, "null argument");
   VSB_MODEL_SCOPE(m);
-  m->impl.check_ready();
-  const size_t n = (size_t)F * 3 * H * W;
-  const bool use_jnd = !(flags & VSB_FLAG_NO_ATTENUATION) && m->impl.d.jnd_in_ch != 0;
-  const size_t np = (size_t)F * (use_jnd ? std::max(m->impl.d.unet_out_ch, m->impl.d.jnd_out_ch) : m->impl.d.unet_out_ch) * H * W;
-  float* imgs = (float*)m->impl.stage(0, n * sizeof(float));
-  float* out = (float*)m->impl.stage(1, n * sizeof(float));
-  float* pw = preds_w_h ? (float*)m->impl.stage(2, np * sizeof(float)) : nullptr;
-  uint8_t* msgs = (uint8_t*)m->impl.stage(3, (size_t)n_msgs * m->impl.d.nbits + 256);
-  cudaStream_t st = 0;
-  VSB_CUDA(cudaMemcpyAsync(imgs, imgs_h, n * sizeof(float), cudaMemcpyHostToDevice, st));
-  VSB_CUDA(cudaMemcpyAsync(msgs, msgs_h, (size_t)n_msgs * m->impl.d.nbits, cudaMemcpyHostToDevice, st));
-  m->impl.embed(imgs, msgs, n_msgs, out, pw, F, H, W, step, video_mode, chunk_keys, scaling_i, scaling_w, flags, st);
-  VSB_CUDA(cudaMemcpyAsync(imgs_w_h, out, n * sizeof(float), cudaMemcpyDeviceToHost, st));
-  if (pw) VSB_CUDA(cudaMemcpyAsync(preds_w_h, pw, np * sizeof(float), cudaMemcpyDeviceToHost, st));
-  VSB_CUDA(cudaStreamSynchronize(st));
+  m->impl.embed_host(imgs_h, msgs_h, n_msgs, imgs_w_h, preds_w_h, F, H, W, step, video_mode, chunk_keys, scaling_i, scaling_w, flags);
   return VSB_OK;
   VSB_API_END
 }
@@ -170,16 +152,7 @@ int vsb_detect_host(vsb_model* m, const float* imgs_h, float* logits_h, int32_t 
   VSB_API_BEGIN
   VSB_CHECK(m && imgs_h && logits_h, "null argument");
   VSB_MODEL_SCOPE(m);
-  m->impl.check_ready();
-  const size_t n = (size_t)F * 3 * H * W;
-  const size_t nl = (size_t)F * m->impl.detect_out_per_frame();
-  float* imgs = (float*)m->impl.stage(0, n * sizeof(float));
-  float* lg = (float*)m->impl.stage(2, nl * sizeof(float));
-  cudaStream_t st = 0;
-  VSB_CUDA(cudaMemcpyAsync(imgs, imgs_h, n * sizeof(float), cudaMemcpyHostToDevice, st));
-  m->impl.detect(imgs, lg, F, H, W, flags, st);
-  VSB_CUDA(cudaMemcpyAsync(logits_h, lg, nl * sizeof(float), cudaMemcpyDeviceToHost, st));
-  VSB_CUDA(cudaStreamSynchronize(st));
+  m->impl.detect_host(imgs_h, logits_h, F, H, W, flags);
   return VSB_OK;
   VSB_API_END
 }
@@ -220,30 +193,10 @@ int64_t vsb_launch_count(int32_t reset) {
 int64_t vsb_debug_get_tensor(vsb_model* m, const char* name, float* host_out, int64_t capacity, int64_t* shape4) {
   try {
     VSB_CHECK(m && name && shape4, "null argument");
-    Plan* pl = m->impl.last_plan;
-    VSB_CHECK(pl != nullptr, "no plan has run yet");
-    VSB_MODEL_SCOPE(m);
-    auto it = pl->dbg.find(name);
-    if (it == pl->dbg.end()) throw Error(std::string("unknown debug tensor: ") + name);
-    const DebugTensor& t = it->second;
-    const int64_t rows = t.shape[0] * t.shape[1] * t.shape[2], C = t.shape[3];
-    for (int i = 0; i < 4; ++i) shape4[i] = t.shape[i];
-    const int64_t n = rows * C;
-    if (host_out == nullptr) return n;
-    VSB_CHECK(capacity >= n, "debug buffer too small");
-    VSB_CUDA(cudaDeviceSynchronize());
-    if (t.dtype == 0) {
-      VSB_CUDA(cudaMemcpy2D(host_out, C * sizeof(float), t.ptr, t.ld * sizeof(float), C * sizeof(float), rows, cudaMemcpyDeviceToHost));
-    } else {
-      std::vector<__half> h((size_t)n);
-      VSB_CUDA(cudaMemcpy2D(h.data(), C * sizeof(__half), t.ptr, t.ld * sizeof(__half), C * sizeof(__half), rows, cudaMemcpyDeviceToHost));
-      for (int64_t i = 0; i < n; ++i) host_out[i] = __half2float(h[i]);
-    }
-    return n;
-  } catch (const std::exception& e) {
-    g_err = e.what();
-    return -1;
-  }
+    VSB_MODEL_SCOPE(m);   // before the plan is read: another thread may evict it from the cache
+    VSB_CHECK(m->impl.last_plan != nullptr, "no plan has run yet");
+    return m->impl.last_plan->read_tap(name, host_out, capacity, shape4);
+  } catch (const std::exception& e) { return fail(e, -1); }
 }
 
 int vsb_debug_keep_inputs(vsb_model* m, int32_t on) {
@@ -263,10 +216,7 @@ int32_t vsb_debug_last_dispatch(vsb_model* m, int32_t* out, int32_t capacity) {
     std::copy(m->impl.last_resize, m->impl.last_resize + 5, out);
     std::copy(m->impl.last_blend, m->impl.last_blend + 5, out + 5);
     return 10;
-  } catch (const std::exception& e) {
-    g_err = e.what();
-    return -1;
-  }
+  } catch (const std::exception& e) { return fail(e, -1); }
 }
 
 int vsb_debug_conv(const vsb_conv_test* t, void* stream) {
@@ -297,7 +247,7 @@ int vsb_debug_conv(const vsb_conv_test* t, void* stream) {
       VSB_CUDA(cudaMemcpy(hw.data(), t->weights, hw.size() * sizeof(__half), cudaMemcpyDeviceToHost));
       std::vector<float> w(hw.size());
       for (size_t i = 0; i < hw.size(); ++i) w[i] = __half2float(hw[i]);
-      const std::vector<__half> vh = Model::to_half(s2 ? s2d_weights(w, t->N, t->C0) : direct8_weights(w, t->N, t->R));
+      const std::vector<__half> vh = to_half(s2 ? s2d_weights(w, t->N, t->C0) : direct8_weights(w, t->N, t->R));
       VSB_CUDA(cudaMemcpy(wtmp, vh.data(), vh.size() * sizeof(__half), cudaMemcpyHostToDevice));
       pack_direct_weights(wtmp, t->N, s2 ? 4 * t->C0 : 16, wpk, (cudaStream_t)stream, s2 ? 9 : t->R * ((t->R + 1) / 2));
     } else {
@@ -370,22 +320,13 @@ int vsb_debug_resample_table2(int32_t in, int32_t out, int32_t mode, int32_t ali
     for (int i = 0; i < out; ++i) { start[i] = t.start[i]; cnt[i] = t.cnt[i]; }
     for (size_t i = 0; i < t.w.size(); ++i) weights[i] = t.w[i];
     return t.maxt;
-  } catch (const std::exception& e) {
-    g_err = e.what();
-    return -1;
-  }
+  } catch (const std::exception& e) { return fail(e, -1); }
 }
 
 int64_t vsb_quality_workspace_bytes(int32_t B, int32_t C, int32_t H, int32_t W, int32_t multiscale) {
   try {
     return (int64_t)quality_layout(B, C, H, W, multiscale != 0).bytes;
-  } catch (const vsb::Error& e) {
-    g_err = e.what();
-    return e.code;
-  } catch (const std::exception& e) {
-    g_err = e.what();
-    return VSB_ERR_INVALID;
-  }
+  } catch (const vsb::Error& e) { return fail(e, e.code); } catch (const std::exception& e) { return fail(e, VSB_ERR_INVALID); }
 }
 
 // device of a CUDA allocation; VSB_ERR_INVALID for host memory
@@ -431,13 +372,7 @@ int vsb_ssim(const float* x, const float* y, int32_t B, int32_t C, int32_t H, in
 int64_t vsb_augment_workspace_bytes(int32_t op, int32_t B, int32_t H, int32_t W) {
   try {
     return (int64_t)aug_workspace_bytes(op, B, H, W);
-  } catch (const vsb::Error& e) {
-    g_err = e.what();
-    return e.code;
-  } catch (const std::exception& e) {
-    g_err = e.what();
-    return VSB_ERR_INVALID;
-  }
+  } catch (const vsb::Error& e) { return fail(e, e.code); } catch (const std::exception& e) { return fail(e, VSB_ERR_INVALID); }
 }
 
 int vsb_augment(int32_t op, const float* x, float* y, int32_t B, int32_t C, int32_t H, int32_t W, int32_t OH, int32_t OW, const float* params,
