@@ -232,8 +232,22 @@ int64_t vsb_debug_get_tensor(vsb_model* m, const char* name, float* host_out, in
  *   s{s}_ln (s >= 1) the fp16 LayerNorm'd rows the down conv reads;  s{s}_a / s{s}_g  the last block's dwconv + LN output and
  *   its pwconv1 + GELU output (after the in-place GRN on stages that apply it);  s{s}_w2s  [B, C, 1, 4C] the per-sample GRN-scaled
  *   W2 of stages that fold GRN into the weights;  stage{s}  the stream after stage s;  stage3_16  its fp16 copy the head conv
- *   reads;  head_conv;  head_pooled  [B, 1, 1, C] the LayerNorm + GELU + mean the linear head reads. */
+ *   reads;  head_conv;  head_pooled  [B, 1, 1, C] the LayerNorm + GELU + mean the linear head reads.
+ * SAM-ViT detect plans reuse one residual stream, one LayerNorm buffer and one neck buffer; with L the last block, the taps while
+ * on are
+ *   vit.blk{L}.in    fp32 the stream the last block reads        vit.blk{L}.ln1  fp16 its LayerNorm 1 output (LN2 overwrites it)
+ *   vit.blk{L}.mid   fp32 the stream after its attention proj (lin2 updates it in place)
+ *   vit.neck1x1      fp32 the neck's 1x1 output (the 3x3 writes into the same buffer)
+ * and in every SAM-ViT detect plan: vit.patches [B, G, G, 768] fp16 im2col rows (K order c, r, s);  vit.embed  the stream after
+ * the patch GEMM + position table;  vit.blk{L}.qkv / .attn / .ln2 / .hid  the last block's qkv rows, attention output, LayerNorm 2
+ * output and GELU hidden rows (fp16);  vit.blk{L}  the stream after it;  vit.x16  its fp16 copy the neck reads;  vit.neck_ln1  the
+ * fp16 LayerNorm of the 1x1 output;  vit.neck3x3  fp32 the 3x3 output;  vit.neck  the fp16 map the head reads. */
 int vsb_debug_keep_inputs(vsb_model* m, int32_t on);
+/* host-only: the variant finalize_op chose for each tensor-core step of the most recent plan, one line per step in plan order:
+ * "name\tM=..\tN=..\tK=..\tblock_n=..\ttma_store=0|1|2\tb_resident=0|1\tb_fixed_ntile=0|1\tkernel=128|longk\tbias_global=0|1\t
+ * m_tiles=whole|ragged\n".  Written like vsb_profile_read: returns the bytes needed (with the terminating 0), or < 0; buf is
+ * filled when capacity is at least that. */
+int64_t vsb_debug_plan_gemms(vsb_model* m, char* buf, int64_t capacity);
 /* which compiled variant the most recent launch of each full-resolution kernel used (host state, no synchronisation):
  *   out[0..4]  resize_sep_kernel:  MT (x taps in registers: 2, 8, or 0 = any count), GST (input rows per staging round: 4, 2, 1),
  *              vec (1 = bulk copies, 0 = 4-byte cp.async), toy (output rows per block), OW (output width = img_size)

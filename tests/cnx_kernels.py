@@ -304,9 +304,14 @@ def plan_checks(tr: Trunk, tap: Callable[[str], torch.Tensor], has_tap: Callable
             st = tap("stage3")
             yield Check("s3 pwconv2 fp16 copy", tap("stage3_16"), st, half_ulp16(st.abs()), [("the block input instead", xin, None)])
         del xin
-    # ---- head 3x3, reflect padding: stage3_16 -> head_conv
-    x16 = tap("stage3_16")
-    C = dims[3]
+    yield from head_checks(sd, tap("stage3_16"), tap, logits)
+
+
+def head_checks(sd: Dict[str, torch.Tensor], x16: torch.Tensor, tap: Callable[[str], torch.Tensor], logits: torch.Tensor):
+    """the pooled head (decoder.cuh add_head) on the fp16 trunk map x16 [B, C, h, h]: head3x3, head_pool, head_linear; tap(name)
+    -> head_conv [B, C, h, h] / head_pooled [B, C] (float64)"""
+    # ---- head 3x3, reflect padding: x16 -> head_conv
+    C = x16.shape[1]
     w = sd[D + "output_upscaling.0.upsample_block.2.weight"]
     rp = lambda v: F.pad(v, (1, 1, 1, 1), mode="reflect")
     ref = F.conv2d(rp(x16), w)

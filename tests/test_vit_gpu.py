@@ -2,13 +2,13 @@
 detect() against the CPU oracle, the attention kernel on its own inputs against float64, determinism, the C entry points, and
 embed() unchanged by the extractor."""
 import ctypes as C
-import math
 
 import numpy as np
 import pytest
 import torch
 
 from tests import vit_oracle as vo
+from tests.vit_kernels import attention_bound, attention_f64
 
 pytestmark = pytest.mark.gpu
 AGGS = ("avg", "squared_avg", "l1norm_avg", "l2norm_avg")
@@ -166,50 +166,6 @@ def test_detect_parity_pixelwise():
 
 
 # ---------------------------------------------------------------- the attention kernel on its own inputs
-
-def attention_f64(qkv, heads, n, G, rel_h, rel_w, mutate=None):
-    """float64 restatement of vit.py:302-353 + :431-470 on the qkv rows [B, G, G, 3E] of one block (window partition by index);
-    rel_h / rel_w: the fp16-rounded tables or None.  Returns (out [B, G, G, E], A [B, G, G, E]) with A = sum_k p |v| / sum_k p,
-    and the per-row score error scale S_err [B, G, G, heads] for the bound."""
-    B, E = qkv.shape[0], qkv.shape[-1] // 3
-    hd = E // heads
-    shift = 1 if mutate == "shift" else 0     # windows placed one token to the right (with wrap-around)
-    x = qkv.double().roll(-shift, dims=2).reshape(B, G // n, n, G // n, n, 3, heads, hd).permute(5, 0, 1, 3, 6, 2, 4, 7)
-    x = x.reshape(3, -1, n * n, hd)           # [3, B*win*heads, T, hd]
-    q, k, v = x[0], x[1], x[2]
-    scale = hd ** -0.5
-    s = (q * scale) @ k.transpose(-1, -2)
-    serr = (q.abs() * scale) @ k.abs().transpose(-1, -2)
-    if rel_h is not None:
-        idx = torch.arange(n)[:, None] - torch.arange(n)[None, :] + n - 1
-        Rh, Rw = rel_h.double()[idx], rel_w.double()[idx]      # [n, n, hd]
-        if mutate == "transpose":
-            Rh, Rw = Rw, Rh
-        rq = (q * scale if mutate == "scaled" else q).reshape(-1, n, n, hd)
-        rh = torch.einsum("bhwc,hkc->bhwk", rq, Rh)
-        rw = torch.einsum("bhwc,wkc->bhwk", rq, Rw)
-        s = (s.view(-1, n, n, n, n) + rh[:, :, :, :, None] + rw[:, :, :, None, :]).view(-1, n * n, n * n)
-        aq = q.abs().reshape(-1, n, n, hd)
-        eh = torch.einsum("bhwc,hkc->bhwk", aq, Rh.abs())
-        ew = torch.einsum("bhwc,wkc->bhwk", aq, Rw.abs())
-        serr = (serr.view(-1, n, n, n, n) + eh[:, :, :, :, None] + ew[:, :, :, None, :]).view(-1, n * n, n * n)
-    p = torch.softmax(s, dim=-1)
-    o = p @ v
-    a = p @ v.abs()
-    se = serr.amax(dim=-1, keepdim=True).expand(-1, -1, hd)
-
-    def back(t):   # [B*win*heads, T, hd] -> [B, G, G, E]
-        return t.reshape(B, G // n, G // n, heads, n, n, hd).permute(0, 1, 4, 2, 5, 3, 6).reshape(B, G, G, E).roll(shift, dims=2)
-    return back(o), back(a), back(se)
-
-
-def attention_bound(ref, a, se):
-    """per element: fp16 rounding of the output (2^-11 |o|); fp16 rounding of P (2^-11 per p, so 2^-11 sum p|v| / sum p); the fp32
-    score accumulation over 64 products (<= 64 * 2^-24 of the sum of |terms|, twice: it moves a p and the normaliser); fp32 exp,
-    sums and division (a few ulps of A)"""
-    u16, u32 = 2.0 ** -11, 2.0 ** -24
-    return u16 * ref.abs() + (u16 + 2 * 64 * u32 * se + 16 * u32) * a + 1e-7
-
 
 ATTN_CASES = {   # the model's only block (depth 1) is windowed or global, with or without the relative-position tables
     "win_rel": {"depth": 1, "global_attn_indexes": [], "use_rel_pos": True},

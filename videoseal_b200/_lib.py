@@ -12,7 +12,8 @@ LIB_PATH = os.environ.get("VSB200_LIB") or os.path.join(_HERE, "libvsb200.so")
 EXPORTS = [
     "vsb_last_error", "vsb_version", "vsb_model_create", "vsb_model_set_tensor", "vsb_model_set_pixel_decoder", "vsb_model_finalize",
     "vsb_model_destroy", "vsb_embed", "vsb_embedder_forward", "vsb_detect", "vsb_jnd_heatmaps", "vsb_embed_host",
-    "vsb_detect_host", "vsb_embed_detect_host", "vsb_frames_host_u8", "vsb_launch_count", "vsb_profile_enable", "vsb_profile_read", "vsb_debug_get_tensor", "vsb_debug_keep_inputs", "vsb_debug_conv",
+    "vsb_detect_host", "vsb_embed_detect_host", "vsb_frames_host_u8", "vsb_launch_count", "vsb_profile_enable", "vsb_profile_read", "vsb_debug_get_tensor", "vsb_debug_keep_inputs", "vsb_debug_plan_gemms",
+    "vsb_debug_conv",
     "vsb_debug_resample_table", "vsb_debug_resample_table2", "vsb_debug_last_dispatch", "vsb_quality_workspace_bytes", "vsb_ssim", "vsb_model_set_vit_extractor",
     "vsb_augment_workspace_bytes", "vsb_augment",
 ]
@@ -99,6 +100,8 @@ def lib():
     L.vsb_debug_get_tensor.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]
     L.vsb_debug_get_tensor.restype = C.c_int64
     L.vsb_debug_keep_inputs.argtypes = [C.c_void_p, C.c_int32]
+    L.vsb_debug_plan_gemms.argtypes = [C.c_void_p, C.c_char_p, C.c_int64]
+    L.vsb_debug_plan_gemms.restype = C.c_int64
     L.vsb_debug_conv.argtypes = [C.POINTER(ConvTest), C.c_void_p]
     L.vsb_debug_resample_table.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
     L.vsb_debug_resample_table2.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,

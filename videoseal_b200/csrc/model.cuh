@@ -53,7 +53,7 @@ class Model {
   //   resize: MT, GST, vec, toy, OW       blend: 3 (jnd_blend3_kernel) or 2 (jnd_blend2_kernel), VEC, FASTUP, CD, JIN
   int32_t last_resize[5] = {-1, -1, -1, -1, -1};
   int32_t last_blend[5] = {-1, -1, -1, -1, -1};
-  // test seam (vsb_debug_keep_inputs): detect plans copy the ConvNeXt residual stream aside where the blocks read it
+  // test seam (vsb_debug_keep_inputs): detect plans copy the trunk's in-place buffers aside where its steps read them
   bool keep_inputs = false;
   void set_keep_inputs(bool on) {
     keep_inputs = on;
@@ -145,7 +145,7 @@ class Model {
     pl.x_res = pl.pool.alloc_n<float>((size_t)B * 3 * S * S);
     pl.tap("x_res", pl.x_res, 0, B, 3, S, S, S);
     pl.logits = pl.pool.alloc_n<float>((size_t)B * (1 + d.nbits));
-    const FeatureMap m = vit.on ? vit.build(pl, B, S, num_sms) : cnx.build(pl, B, d, num_sms, keep_inputs);
+    const FeatureMap m = vit.on ? vit.build(pl, B, S, num_sms, keep_inputs) : cnx.build(pl, B, d, num_sms, keep_inputs);
     dec.build(pl, B, m, vit.on ? "vit." : "cnx.", d.nbits, num_sms);
   }
   Plan* get_embed_plan(int B) { return get_plan(embed_plans, B, &Model::build_embed_plan); }

@@ -59,6 +59,8 @@ struct Plan {
   uint64_t last_use = 0;    // LRU stamp of the plan cache
   std::vector<Step> steps;
   std::map<std::string, DebugTensor> dbg;
+  // host-only record of the variant finalize_op chose for each tensor-core step, one line per add_conv (vsb_debug_plan_gemms)
+  std::vector<std::string> gemms;
   // embed plan I/O
   const float* in_imgs = nullptr;  // set per call (pointer slot read by the first kernel's lambda)
   long in_frame_stride = 0;

@@ -119,8 +119,9 @@ struct VitTrunk {
   }
 
   // modules/vit.py:111-143 on the fp32 residual stream x [B*G*G][E] (token rows in raster order), ending in the fp16 [B, G, G,
-  // out_chans] map the head reads
-  FeatureMap build(Plan& pl, int B, int S, int nsm) const {
+  // out_chans] map the head reads.  keep_inputs (vsb_debug_keep_inputs): the values the last block and the neck read from buffers
+  // that a later step overwrites are copied aside as they pass (vit.blk{L}.in / .ln1 / .mid, vit.neck1x1)
+  FeatureMap build(Plan& pl, int B, int S, int nsm, bool keep_inputs) const {
     Plan* plp = &pl;
     const int G = map(S), E = vd.embed_dim, H3 = 3 * E, MLP = vd.mlp_dim, oc = vd.out_chans;
     const long M = (long)B * G * G;
@@ -141,6 +142,12 @@ struct VitTrunk {
     auto ln = [&](const char* name, const float* in, int C, const float* lw, const float* lb, float eps, __half* out) {
       pl.add(name, [=](cudaStream_t st) { launch_ln_rows(in, M, C, C, lw, lb, eps, out, C, nsm, st); });
     };
+    auto keep = [&](const std::string& name, const void* src, int dtype, int C) {
+      const size_t bytes = (size_t)M * C * (dtype == 0 ? sizeof(float) : sizeof(__half));
+      void* dst = pl.pool.alloc_n<char>(bytes);
+      pl.add("dbg.keep." + name, [=](cudaStream_t st) { VSB_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st)); }, 0);
+      pl.tap(name, dst, dtype, B, G, G, C, C);
+    };
     {
       // patch embed (vit.py:494-525): im2col of the 16 x 16 patches, GEMM into the fp32 stream, + (pos_embed + folded bias)
       __half* patches = pl.pool.alloc_n<__half>(M * 768);
@@ -148,6 +155,7 @@ struct VitTrunk {
       gemm(patches, 768, patch, ACT_NONE, "vit.patch", [&](ConvGemmParams& p) { p.out32 = x0; p.ld_out32 = E; });
       const float* table = pos;
       pl.add("vit.patch", [=](cudaStream_t st) { launch_vit_pos_add(x0, M, G * G, E, table, nsm, st); });
+      pl.tap("vit.patches", patches, 1, B, G, G, 768, 768);
       pl.tap("vit.embed", x0, 0, B, G, G, E, E);
     }
     for (int i = 0; i < vd.depth; ++i) {
@@ -155,7 +163,10 @@ struct VitTrunk {
       const std::string bi = "vit.blk" + std::to_string(i);
       const bool global = (vd.global_mask >> i) & 1u;
       const float* xin = i == 0 ? x0 : x;   // the block's input stream
+      const bool last = i + 1 == vd.depth;
+      if (keep_inputs && last) keep(bi + ".in", xin, 0, E);
       ln("vit.ln", xin, E, w.n1w, w.n1b, 1e-5f, xn);
+      if (keep_inputs && last) keep(bi + ".ln1", xn, 1, E);
       gemm(xn, E, w.qkv, ACT_NONE, "vit.qkv", [&](ConvGemmParams& p) { p.out16 = qkv; p.ld_out16 = H3; });
       {
         AttnParams ap{};
@@ -167,19 +178,23 @@ struct VitTrunk {
       }
       // in place after block 0: each element is read and written by the same thread
       gemm(att, E, w.proj, ACT_NONE, "vit.proj", [&](ConvGemmParams& p) { p.resid32 = xin; p.ld_res32 = E; p.out32 = x; p.ld_out32 = E; });
+      if (keep_inputs && last) keep(bi + ".mid", x, 0, E);
       ln("vit.ln", x, E, w.n2w, w.n2b, 1e-5f, xn);
       gemm(xn, E, w.lin1, ACT_GELU, "vit.lin1", [&](ConvGemmParams& p) { p.out16 = hid; p.ld_out16 = MLP; });
       gemm(hid, MLP, w.lin2, ACT_NONE, "vit.lin2", [&](ConvGemmParams& p) {
         p.resid32 = x; p.ld_res32 = E; p.out32 = x; p.ld_out32 = E;
-        if (i + 1 == vd.depth) { p.out16 = x16; p.ld_out16 = E; }
+        if (last) { p.out16 = x16; p.ld_out16 = E; }
       });
       // the stream, qkv and att buffers are reused by every block, so they hold the LAST block's values after a run: only its taps
       // exist.  Per-block copies would cost ~0.9 GB per 64-frame 256^2 plan; block k - 1 of a model is compared through the model
       // of depth k built from the same checkpoint prefix (tests/test_vit_gpu.py)
-      if (i + 1 == vd.depth) {
+      if (last) {
         pl.tap(bi + ".qkv", qkv, 1, B, G, G, H3, H3);
         pl.tap(bi + ".attn", att, 1, B, G, G, E, E);
+        pl.tap(bi + ".ln2", xn, 1, B, G, G, E, E);
+        pl.tap(bi + ".hid", hid, 1, B, G, G, MLP, MLP);
         pl.tap(bi, x, 0, B, G, G, E, E);
+        pl.tap("vit.x16", x16, 1, B, G, G, E, E);
       }
     }
     // neck (vit.py:90-109): 1x1 conv, LayerNorm2d, 3x3 conv (zero padding 1), LayerNorm2d; both without bias, eps 1e-6
@@ -187,13 +202,16 @@ struct VitTrunk {
     __half* yn = pl.pool.alloc_n<__half>(M * oc);
     __half* out = pl.pool.alloc_n<__half>(M * oc);
     gemm(x16, E, neck1, ACT_NONE, "vit.neck1x1", [&](ConvGemmParams& p) { p.out32 = y; p.ld_out32 = oc; });
+    if (keep_inputs) keep("vit.neck1x1", y, 0, oc);
     ln("vit.neck_ln", y, oc, nln1w, nln1b, 1e-6f, yn);
+    pl.tap("vit.neck_ln1", yn, 1, B, G, G, oc, oc);
     {
       ConvGemmOp op;
       setup_gather_conv(op, LD_GATHER_CONV, yn, oc, oc, nullptr, 0, 0, B, G, G, G, G, 3, 3, 1, 1, 0);
       op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.out32 = y; op.p.ld_out32 = oc;
       add_conv(pl, op, neck3, "vit.neck3x3", nsm);
     }
+    pl.tap("vit.neck3x3", y, 0, B, G, G, oc, oc);   // the 3x3 output: the last LayerNorm only reads y
     ln("vit.neck_ln", y, oc, nln2w, nln2b, 1e-6f, out);
     pl.tap("vit.neck", out, 1, B, G, G, oc, oc);
     return FeatureMap{out, G, oc, oc};

@@ -208,6 +208,18 @@ int vsb_debug_keep_inputs(vsb_model* m, int32_t on) {
   VSB_API_END
 }
 
+int64_t vsb_debug_plan_gemms(vsb_model* m, char* buf, int64_t capacity) {
+  try {
+    VSB_CHECK(m != nullptr, "null argument");
+    std::lock_guard<std::recursive_mutex> lk(m->impl.mu);   // host state only: no device switch
+    VSB_CHECK(m->impl.last_plan != nullptr, "no plan has run yet");
+    std::string out;
+    for (const std::string& line : m->impl.last_plan->gemms) out += line + "\n";
+    if (buf && capacity > (int64_t)out.size()) memcpy(buf, out.c_str(), out.size() + 1);
+    return (int64_t)out.size() + 1;
+  } catch (const std::exception& e) { return fail(e, -1); }
+}
+
 int32_t vsb_debug_last_dispatch(vsb_model* m, int32_t* out, int32_t capacity) {
   try {
     VSB_CHECK(m && out, "null argument");

@@ -184,6 +184,13 @@ struct Weights {
 inline void add_conv(Plan& pl, ConvGemmOp op, const ConvW& w, const std::string& name, int num_sms, const __half* w_override = nullptr) {
   finalize_op(op, w_override ? w_override : w.w, w.N, w.K, w.ld ? w.ld : w.K, num_sms, 0);
   pl.add(name, [op](cudaStream_t st) { launch(op, st); });
+  const ConvGemmParams& p = op.p;
+  const bool ragged = op.longk ? p.M % kLongM != 0 : (long)p.m_tiles * kBlockM != (long)p.M;
+  pl.gemms.push_back(name + "\tM=" + std::to_string(p.M) + "\tN=" + std::to_string(w.N) + "\tK=" + std::to_string(w.K) +
+                     "\tblock_n=" + std::to_string(p.block_n) + "\ttma_store=" + std::to_string(p.tma_store) +
+                     "\tb_resident=" + std::to_string(p.b_resident) + "\tb_fixed_ntile=" + std::to_string(p.b_fixed_ntile) +
+                     "\tkernel=" + (op.longk ? "longk" : "128") + "\tbias_global=" + std::to_string(p.bias_global) +
+                     "\tm_tiles=" + (ragged ? "ragged" : "whole"));
 }
 
 }  // namespace vsb
