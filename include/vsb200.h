@@ -88,7 +88,12 @@ int vsb_version(void);
  * rings; JND channels 1 or 3.  VSB_ERR_INVALID unless: 2..6 levels, unet_in_ch 1 (yuv) or 3, unet_out_ch 1..3, img_size a multiple
  * of 128, hidden a multiple of 8, ConvNeXt widths even and not shrinking. */
 int vsb_model_create(const vsb_model_desc* desc, vsb_model** out);
-/* one state_dict entry, fp32, host memory, contiguous; `name` is the reference state_dict key */
+/* Temporal U-Net (unet.conv_layer 'conv3d', modules/common.py Conv3dWrapper), called between create and finalize; no CUDA call.
+ * on = 1: every ResnetBlock's 3x3 convs are 3x3x3 over the key frames of one embedder call (see vsb_embed) and its res_conv 1x1x1; the
+ * checkpoint then holds their 5-D weights under the Conv3dWrapper keys (`...double_conv.0.conv.weight`).  on = 0: 'conv2d', the default.
+ * VSB_ERR_UNSUPPORTED for a U-Net width below 16; VSB_ERR_STATE after finalize; VSB_ERR_INVALID for on other than 0 / 1. */
+int vsb_model_set_unet_temporal(vsb_model* m, int32_t on);
+/* one state_dict entry, fp32, host memory, contiguous, at most 5 dimensions; `name` is the reference state_dict key */
 int vsb_model_set_tensor(vsb_model* m, const char* name, const float* data, const int64_t* shape, int32_t ndim);
 /* Pixel-wise extractor head (modules/pixel_decoder.py:44-83 with pixelwise=True), called between create and finalize.  Without
  * this call the model has the pooled head (one [1+nbits] logit vector per frame).  pixelwise = 1 needs 1..8 stage factors, each 2
@@ -127,13 +132,18 @@ void vsb_model_destroy(vsb_model* m);
  * attenuation on, the broadcast of `hmaps * preds_w` in wam.py:189-193, else unet_out_ch);
  * step = 1 for image mode, else frames share the key frame f/step (videoseal.py:292-340);
  * chunk_keys = the model's chunk_size (key frames per reference chunk, videoseal.py:300): it only changes the result in
- * video_mode 'interpolate', where neighbouring key frames of ONE chunk are mixed (videoseal.py:101-113); 1..64 there. */
+ * video_mode 'interpolate', where neighbouring key frames of ONE chunk are mixed (videoseal.py:101-113); 1..64 there.
+ * A temporal U-Net (vsb_model_set_unet_temporal) convolves across the key frames of one group of chunk_keys consecutive key frames (one
+ * reference embedder call: a video chunk, or, in image mode, the whole batch, so pass chunk_keys = F there); the last group may be
+ * shorter, and frames of different groups never interact.  VSB_ERR_UNSUPPORTED when chunk_keys > 64 (a group must fit one
+ * 64-frame sub-batch).  The same holds for vsb_embed_host, vsb_embed_detect_host and vsb_frames_host_u8. */
 int vsb_embed(vsb_model* m, const float* imgs_dev, const uint8_t* msgs_dev, int32_t n_msgs, float* imgs_w_dev,
               float* preds_w_dev, int32_t F, int32_t H, int32_t W, int32_t step, int32_t video_mode, int32_t chunk_keys,
               float scaling_i, float scaling_w, int32_t flags, void* stream);
 
 /* x_dev [B, 3, S, S] RGB fp32 in [0,1] at processing size S = img_size (the Y extraction for yuv cards happens
- * inside, wam.py:168-172); delta_dev [B, unet_out_ch, S, S] */
+ * inside, wam.py:168-172); delta_dev [B, unet_out_ch, S, S].  A temporal U-Net takes the B frames as one group (one reference
+ * embedder call): VSB_ERR_UNSUPPORTED for B > 64. */
 int vsb_embedder_forward(vsb_model* m, const float* x_dev, const uint8_t* msgs_dev, int32_t n_msgs, float* delta_dev,
                          int32_t B, void* stream);
 

@@ -9,6 +9,7 @@ from __future__ import annotations
 
 import math
 import os
+import re
 from pathlib import Path
 from urllib.parse import urlparse
 
@@ -80,6 +81,12 @@ def spec_from_card(card: dict) -> dict:
         raise NotImplementedError("only 'binary+concat' message processors are implemented")
     if str(a.get("blending_method", "additive")) != "additive":
         raise NotImplementedError("only additive blending is implemented (all shipped cards use it)")
+    conv_layer = str(u.get("conv_layer", "conv2d"))
+    if conv_layer not in ("conv2d", "conv3d"):
+        raise NotImplementedError(f"U-Net conv_layer '{conv_layer}' is not implemented (conv2d, or conv3d with BatchNorm + ReLU)")
+    if conv_layer == "conv3d" and (str(u["activation"]) != "relu" or not str(u["normalization"]).startswith("batch")):
+        raise NotImplementedError(f"temporal (conv3d) U-Net with {u['activation']}/{u['normalization']}: only BatchNorm + ReLU is "
+                                  "implemented")
     ep = card["extractor"]["params"]
     pd = ep.get("pixel_decoder", {})
     pixelwise = bool(pd.get("pixelwise", False))
@@ -109,7 +116,7 @@ def spec_from_card(card: dict) -> dict:
             "in_channels": int(u["in_channels"]), "out_channels": int(u["out_channels"]),
             "z": [int(u["z_channels"]) * int(m) for m in u["z_channels_mults"]], "num_blocks": int(u["num_blocks"]),
             "activation": str(u["activation"]), "normalization": str(u["normalization"]),
-            "last_tanh": bool(u.get("last_tanh", True)),
+            "last_tanh": bool(u.get("last_tanh", True)), "temporal": conv_layer == "conv3d",
         },
         **trunk,
         "pixel_decoder": {"pixelwise": pixelwise, "upscale_stages": stages},
@@ -161,12 +168,77 @@ def _vit_trunk(enc: dict) -> dict:
     }}
 
 
+# a Conv3dWrapper checkpoint key of every temporal U-Net (the first ResnetBlock's first conv)
+TEMPORAL_KEY = "embedder.unet.inc.double_conv.0.conv.weight"
+
+
+def is_temporal_state_dict(sd: dict) -> bool:
+    """the U-Net of `sd` was built with conv_layer='conv3d' (5-D Conv3dWrapper weights)"""
+    w = sd.get(TEMPORAL_KEY)
+    return isinstance(w, torch.Tensor) and w.dim() == 5
+
+
+# scripts/inflate_model_to_temporal.py also inflates the extractor (its --extractor_type): a ConvNeXt's downsample convs move under
+# `.1.conv.` next to a temporal conv initialised as the identity, and temporal attention blocks (ConvNeXt stages, or a SAM-ViT's
+# temp_blocks with pos_embed_temporal) are added with a zero output layer.  Temporal extractors do not run here.
+_CNX_DS_CONV = re.compile(r"^(detector\.convnext\.downsample_layers\.\d+\.1)\.conv\.(weight|bias)$")
+_TEMP_BLOCK = re.compile(r"^(detector\.convnext\.stages\.\d+\.\d+\.temp_block\.|detector\.image_encoder\.temp_blocks\.\d+\.)")
+
+
+def strip_identity_temporal_extractor(sd: dict) -> dict:
+    """`sd` without the temporal parts of its extractor, which must be exactly as scripts/inflate_model_to_temporal.py creates them:
+    every temp_conv the identity over time, every temporal attention block's mlp.lin2 zero (weight and bias), pos_embed_temporal
+    zero.  The extractor then computes what the 2-D extractor computes, so its renamed downsample convs are read under their 2-D
+    keys.  Anything else (a trained temporal extractor) raises NotImplementedError: temporal_convs / temporal_attention
+    extractors are not implemented."""
+    renamed = {k: m for k in sd for m in [_CNX_DS_CONV.match(k)] if m}
+    temporal = [k for k in sd if ".temp_conv." in k or _TEMP_BLOCK.match(k) or k == "detector.image_encoder.pos_embed_temporal"]
+    if not renamed and not temporal:
+        return sd
+
+    def refuse(why: str):
+        raise NotImplementedError(f"temporal extractor (temporal_convs / temporal_attention): {why}; only the 2-D extractor runs "
+                                  "here, so a checkpoint whose temporal extractor parts differ from their inflated identity is not "
+                                  "implemented")
+
+    out = {k: v for k, v in sd.items() if k not in renamed and k not in temporal}
+    for k, m in renamed.items():
+        tc = sd.get(m.group(1) + ".temp_conv.weight")
+        if not isinstance(tc, torch.Tensor) or tc.dim() != 5 or tc.shape[0] != tc.shape[1] or tc.shape[2] % 2 != 1 \
+                or tc.shape[3:] != (1, 1):
+            refuse(f"{m.group(1)} has no [C, C, t, 1, 1] temp_conv")
+        ident = torch.zeros_like(tc)
+        ident[:, :, tc.shape[2] // 2, 0, 0] = torch.eye(tc.shape[0], dtype=tc.dtype)
+        if not torch.equal(tc, ident):
+            refuse(f"{m.group(1)}.temp_conv is not the identity")
+        out[f"{m.group(1)}.{m.group(2)}"] = sd[k]
+    blocks = {_TEMP_BLOCK.match(k).group(1) for k in temporal if _TEMP_BLOCK.match(k)}
+    for b in sorted(blocks):
+        for leaf in ("mlp.lin2.weight", "mlp.lin2.bias"):
+            v = sd.get(b + leaf)
+            if not isinstance(v, torch.Tensor) or v.any():
+                refuse(f"{b}{leaf} is not zero")
+    pos = sd.get("detector.image_encoder.pos_embed_temporal")
+    if pos is not None and pos.any():
+        refuse("pos_embed_temporal is not zero")
+    stray = [k for k in temporal if ".temp_conv." in k and k.replace(".temp_conv.", ".conv.") not in renamed]
+    if stray:
+        refuse(f"{stray[0]} belongs to no downsample conv")
+    return out
+
+
 def setup_model(card: dict, ckpt_path):
     from .model import Videoseal
-    spec = spec_from_card(card)
     if not os.path.exists(ckpt_path):
         raise FileNotFoundError(f"Checkpoint path does not exist: {ckpt_path}")
     checkpoint = _safe_load(ckpt_path)
+    checkpoint["model"] = strip_identity_temporal_extractor(checkpoint["model"])
+    # scripts/inflate_model_to_temporal.py turns a 2-D checkpoint into a temporal one in place: it keeps the `args` (which still name
+    # the 2-D preset) and only rewrites the U-Net's weights, so the weights say which conv_layer the U-Net has
+    if is_temporal_state_dict(checkpoint["model"]):
+        emb = card["embedder"]
+        card = {**card, "embedder": {**emb, "params": {**emb["params"], "unet": {**emb["params"]["unet"], "conv_layer": "conv3d"}}}}
+    spec = spec_from_card(card)
     model = Videoseal(spec)
     msg = model.load_state_dict(checkpoint["model"], strict=False)
     print(f"Model loaded successfully from {ckpt_path} with message: {msg}")

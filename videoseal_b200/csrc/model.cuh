@@ -81,6 +81,16 @@ class Model {
     check_unfinalized();
     dec.set(n, f, pw, vit.on || d.ext_stem_stride == 4, d.nbits, [&] { return std::make_pair(trunk_width(), trunk_map()); });
   }
+  // the U-Net's rules and kernel choice again, for a temporal U-Net
+  void set_unet_temporal(int on) {
+    check_unfinalized();
+    VSB_CHECK(on == 0 || on == 1, "temporal must be 0 or 1");
+    UNet u;
+    u.temporal = on != 0;
+    u.check(d);
+    u.choose_kernels();
+    unet = std::move(u);
+  }
   void set_vit_extractor(const vsb_vit_desc& v) {
     check_unfinalized();
     if (dec.pixelwise) throw Error("vsb_model_set_vit_extractor must come before vsb_model_set_pixel_decoder", kErrState);
@@ -117,7 +127,9 @@ class Model {
   }
 
   // Plan cache: one activation arena per distinct batch size, at most `max_plans` per kind (VSB_MAX_PLANS, default 8): a service that sees
-  // many different clip / tail lengths would otherwise accumulate up to 64 arenas of up to 2.3 GB each.  The least recently used plan
+  // many different clip / tail lengths would otherwise accumulate up to 64 arenas of up to 2.3 GB each (a temporal U-Net's embed plan
+  // holds one more buffer, its time-stacked operand: B * S^2 * temporal_stack_width(z0) fp16 values, 512 MiB at 64 x 256^2 and
+  // 4.5 GiB at 64 x 768^2; and its plans are also keyed by the group length).  The least recently used plan
   // is dropped (its cudaFree calls synchronise the device, so work still in flight on it completes first).
   uint64_t plan_clock = 0;
   int max_plans = [] { const char* e = getenv("VSB_MAX_PLANS"); const int v = e ? atoi(e) : 8; return v < 2 ? 2 : v; }();
@@ -139,7 +151,9 @@ class Model {
     }
     return ret;
   }
-  void build_embed_plan(Plan& pl, int B) { unet.build(pl, B); }
+  // embed plans are keyed by B + kPlanGroup * G: a temporal U-Net's plan also depends on its group length G (0 for a 2-D U-Net)
+  static constexpr int kPlanGroup = 128;
+  void build_embed_plan(Plan& pl, int key) { unet.build(pl, key % kPlanGroup, key / kPlanGroup); }
   void build_detect_plan(Plan& pl, int B) {
     const int S = d.img_size;
     pl.x_res = pl.pool.alloc_n<float>((size_t)B * 3 * S * S);
@@ -148,7 +162,17 @@ class Model {
     const FeatureMap m = vit.on ? vit.build(pl, B, S, num_sms, keep_inputs) : cnx.build(pl, B, d, num_sms, keep_inputs);
     dec.build(pl, B, m, vit.on ? "vit." : "cnx.", d.nbits, num_sms);
   }
-  Plan* get_embed_plan(int B) { return get_plan(embed_plans, B, &Model::build_embed_plan); }
+  Plan* get_embed_plan(int B, int G) { return get_plan(embed_plans, B + kPlanGroup * G, &Model::build_embed_plan); }
+  // a temporal U-Net convolves across a group of chunk_keys key frames (one reference embedder call), which must fit one sub-batch
+  int temporal_group(int chunk_keys) const {
+    if (!unet.temporal) return 0;
+    VSB_CHECK(chunk_keys >= 1, "a temporal U-Net needs chunk_keys >= 1 (key frames per embedder call)");
+    if (chunk_keys > kMaxBatch)
+      throw Error("temporal U-Net: a group of " + std::to_string(chunk_keys) + " frames convolved together (one video chunk, or the "
+                  "whole batch in image mode) does not fit one " + std::to_string(kMaxBatch) + "-frame sub-batch; at most " +
+                  std::to_string(kMaxBatch) + " are implemented", kErrUnsupported);
+    return chunk_keys;
+  }
   Plan* get_detect_plan(int B) { return get_plan(detect_plans, B, &Model::build_detect_plan); }
 
 
@@ -226,8 +250,9 @@ class Model {
     }
   }
   // frames that must stay in one batch: a key frame and its step - 1 followers, or in 'interpolate' mode, where neighbouring keys
-  // of one reference chunk are mixed, whole chunks
-  static int key_unit(int step, int video_mode, int chunk_keys) {
+  // of one reference chunk are mixed, and for a temporal U-Net, which convolves across them, whole chunks
+  int key_unit(int step, int video_mode, int chunk_keys) const {
+    if (unet.temporal) return step * temporal_group(chunk_keys);
     return (video_mode == VSB_VIDEO_INTERPOLATE && step > 1) ? step * std::max(1, chunk_keys) : step;
   }
   void embed_detect_host(const float* imgs_h, const uint8_t* msgs_h, int n_msgs, float* imgs_w_h, float* logits_h, int F, int H, int W,
@@ -335,9 +360,9 @@ class Model {
     VSB_CUDA(cudaStreamSynchronize(s_out));
   }
 
-  // U-Net on `n` processing-size RGB frames (contiguous [n,3,S,S]) -> plan->delta
-  Plan* run_unet(const float* x, const uint8_t* msgs, int msg_stride, int n, cudaStream_t st) {
-    Plan* pl = get_embed_plan(n);
+  // U-Net on `n` processing-size RGB frames (contiguous [n,3,S,S]), in temporal groups of G (0: a 2-D U-Net) -> plan->delta
+  Plan* run_unet(const float* x, const uint8_t* msgs, int msg_stride, int n, int G, cudaStream_t st) {
+    Plan* pl = get_embed_plan(n, G);
     pl->in_imgs = x;
     pl->in_frame_stride = (long)3 * d.img_size * d.img_size;
     pl->in_msgs = msgs;
@@ -351,9 +376,10 @@ class Model {
     check_ready();
     VSB_CHECK(n_msgs == 1 || n_msgs == B, "msgs must be [1,K] or [B,K]");
     const int S = d.img_size;
+    const int G = temporal_group(B);   // the B frames are one embedder call
     for (int b0 = 0; b0 < B; b0 += kMaxBatch) {
       const int n = std::min(kMaxBatch, B - b0);
-      Plan* pl = run_unet(x + (size_t)b0 * 3 * S * S, msgs + (n_msgs == 1 ? 0 : (size_t)b0 * d.nbits), n_msgs == 1 ? 0 : d.nbits, n, st);
+      Plan* pl = run_unet(x + (size_t)b0 * 3 * S * S, msgs + (n_msgs == 1 ? 0 : (size_t)b0 * d.nbits), n_msgs == 1 ? 0 : d.nbits, n, G, st);
       VSB_CUDA(cudaMemcpyAsync(delta + (size_t)b0 * d.unet_out_ch * S * S, pl->delta, (size_t)n * d.unet_out_ch * S * S * sizeof(float),
                                cudaMemcpyDeviceToDevice, st));
     }
@@ -368,7 +394,9 @@ class Model {
     // key frames; :101-113 interpolates within the chunk), so U-Net batches are whole chunks in that mode
     const bool interp = (video_mode == VSB_VIDEO_INTERPOLATE) && step > 1;
     if (interp) VSB_CHECK(chunk_keys >= 1 && chunk_keys <= kMaxBatch, "video_mode='interpolate' needs 1 <= chunk_size <= 64");
-    const int kbatch = interp ? (kMaxBatch / chunk_keys) * chunk_keys : kMaxBatch;
+    // a temporal U-Net's sub-batches hold whole groups too: its 3x3x3 convs mix the key frames of one chunk
+    const int G = temporal_group(chunk_keys);
+    const int kbatch = (interp || G) ? (kMaxBatch / chunk_keys) * chunk_keys : kMaxBatch;
     const int bint = interp ? chunk_keys : 0;
     const int S = d.img_size;
     const bool same = (H == S && W == S);
@@ -384,7 +412,7 @@ class Model {
       const int nk = std::min(kbatch, nkeys - k0);
       const int f0 = k0 * step, f1 = std::min(F, (k0 + nk) * step);
       const int nf = f1 - f0;
-      Plan* pl = get_embed_plan(nk);
+      Plan* pl = get_embed_plan(nk, G);
       const float* x = imgs + (size_t)f0 * fstride;
       // low-resolution attenuation needs EVERY frame of the chunk at processing size (wam.py:177-180, videoseal.py:321-324):
       // resample them once into a grow-only scratch buffer of the model (no allocation or synchronisation on the steady-state
@@ -405,7 +433,7 @@ class Model {
         }
         x = pl->x_res;
       }
-      run_unet(x, msgs + (n_msgs == 1 ? 0 : (size_t)k0 * d.nbits), n_msgs == 1 ? 0 : d.nbits, nk, st);
+      run_unet(x, msgs + (n_msgs == 1 ? 0 : (size_t)k0 * d.nbits), n_msgs == 1 ? 0 : d.nbits, nk, G, st);
       const float* delta = pl->delta;
       const int balt = (video_mode == VSB_VIDEO_ALTERNATE) ? 1 : 0;
       BlendParams bp;

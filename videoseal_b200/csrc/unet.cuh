@@ -1,7 +1,10 @@
 // The U-Net embedder (modules/unet.py, BatchNorm + ReLU blocks): its rules and the kernel of every layer, its packed weights and its
-// embed plan.
+// embed plan.  A temporal U-Net (`temporal`, conv_layer 'conv3d') differs in the ResnetBlocks only: their 3x3 convs are 3x3x3 over
+// the frames of a group (temporal.cuh; the first one on CUDA cores, the others as the tensor-core 3x3 conv over the time-stacked
+// operand, never the direct ring conv) and their res_conv is 1x1x1, i.e. an ordinary 1x1 conv.
 #pragma once
 #include "pointwise_host.cuh"
+#include "temporal.cuh"
 #include "weights.cuh"
 
 namespace vsb {
@@ -35,6 +38,7 @@ struct UNet {
   float* msg_table = nullptr;
 
   vsb_model_desc d{};
+  bool temporal = false;   // conv_layer 'conv3d' (vsb_model_set_unet_temporal)
   int nsm = 0;   // SMs of the model's device
 
   // vsb_model_create: the U-Net's rules (no CUDA calls)
@@ -55,6 +59,12 @@ struct UNet {
         throw Error("U-Net width " + std::to_string(z[i]) + " at level " + std::to_string(i) + " is not implemented (8 in the "
                     "leading levels, 16, 32 or a multiple of 64)", kErrUnsupported);
     }
+    // the time-stacked operand of a 3x3x3 conv feeds the TMA conv, which has no 8-channel form
+    if (temporal)
+      for (int i = 0; i < L; ++i)
+        if (z[i] < 16)
+          throw Error("temporal U-Net width " + std::to_string(z[i]) + " at level " + std::to_string(i) + " is not implemented (16, 32 or "
+                      "a multiple of 64)", kErrUnsupported);
     // the tensor-core convs tile maps by 128 pixels
     if ((S >> (L - 1)) < 16)
       throw Error("img_size=" + std::to_string(S) + ": the U-Net's " + std::to_string(L) + " levels leave a " +
@@ -78,10 +88,11 @@ struct UNet {
     };
     // ResnetBlock of C channels on a W-wide map; dense_out: its output has pitch C (the last down level writes the concat buffer)
     auto resblock = [&](int C, int W, bool dense_out) {
+      if (temporal) return ResBlockK{conv3_direct_ok(C, C, W, 1), false, false};
       return ResBlockK{ring8(conv3_direct_ok(C, C, W, 1), C, W), ring8(conv3_direct_ok(C, C, W), C, W),
                        ring8(dense_out && conv3_direct_ok(C, C, W), C, W)};
     };
-    inc_k = ring8(conv3_direct_ok(z[0], z[0], S), z[0], S);
+    inc_k = !temporal && ring8(conv3_direct_ok(z[0], z[0], S), z[0], S);
     for (int i = 0; i < L - 1; ++i) {
       down_k.push_back(ring8(conv3_direct_s2d_ok(z[i], z[i + 1], S >> (i + 1)), z[i + 1], S >> (i + 1)));
       down_rb_k.push_back(resblock(z[i + 1], S >> (i + 1), i < L - 2));
@@ -109,12 +120,33 @@ struct UNet {
   // a conv (3x3 or 1x1, stride 1) in the layout its kernel reads: the direct ring conv's, or the GEMM's (for 3x3 convs up to 16
   // input channels, the halo loader's)
   static ConvW pack_conv(Weights& ws, const std::string& wkey, const std::vector<float>* out_scale, const std::vector<float>& bias, bool direct) {
-    const Taps t = ws.taps(wkey, out_scale);
+    return pack_taps(ws, ws.taps(wkey, out_scale), bias, direct);
+  }
+  static ConvW pack_taps(Weights& ws, const Taps& t, const std::vector<float>& bias, bool direct) {
     if (!direct) return t.R == 3 && use_halo(t.C) ? ws.halo(t, bias) : ws.gemm(t, bias);
     ConvW cw;
     cw.N = t.N;
     cw.wd = ws.direct(t);
     return ws.with_bias(cw, bias);
+  }
+  // a temporal ResnetBlock: Conv3dWrapper keys (`.conv.` inside), 5-D weights
+  static ResBlockW pack_resblock3d(Weights& ws, const std::string& key, const ResBlockK& k) {
+    auto conv = [&](const std::string& wkey, const std::vector<float>* s, const std::vector<float>& b, bool direct) {
+      const HostTensor& w = ws.get(wkey);
+      VSB_CHECK(w.shape.size() == 5, wkey + ": a temporal U-Net needs 5-D Conv3d weights");
+      return pack_taps(ws, conv3d_taps(w, s, temporal_stack_width((int)w.shape[1])), b, direct);
+    };
+    ResBlockW rb;
+    std::vector<float> s, b;
+    ws.bn_fold(key + ".double_conv.1", s, b);
+    rb.c1 = conv(key + ".double_conv.0.conv.weight", &s, b, false);
+    ws.bn_fold(key + ".double_conv.4", s, b);
+    rb.c2 = conv(key + ".double_conv.3.conv.weight", &s, b, false);
+    rb.res = conv(key + ".res_conv.conv.weight", nullptr, ws.get(key + ".res_conv.conv.bias").data, k.res);
+    return rb;
+  }
+  ResBlockW pack_block(Weights& ws, const std::string& key, const ResBlockK& k) const {
+    return temporal ? pack_resblock3d(ws, key, k) : pack_resblock(ws, key, k);
   }
   static ResBlockW pack_resblock(Weights& ws, const std::string& key, const ResBlockK& k) {
     ResBlockW rb;
@@ -134,18 +166,25 @@ struct UNet {
     std::vector<int> z(d.unet_z, d.unet_z + L);
     // ---- inc: first conv on CUDA cores, fp32 weights with BN folded
     {
+      const std::string cv = temporal ? ".conv" : "";   // Conv3dWrapper keys
       std::vector<float> s, b;
       ws.bn_fold(P + "inc.double_conv.1", s, b);
-      const HostTensor& w = ws.get(P + "inc.double_conv.0.weight");
-      VSB_CHECK((int)w.shape[0] == z[0] && (int)w.shape[1] == d.unet_in_ch, "inc conv shape");
+      const HostTensor& w = ws.get(P + "inc.double_conv.0" + cv + ".weight");
+      VSB_CHECK((int)w.shape[0] == z[0] && (int)w.shape[1] == d.unet_in_ch && (int)w.shape.size() == (temporal ? 5 : 4), "inc conv shape");
       std::vector<float> w1(w.data);   // the CUDA-core kernel reads the checkpoint's own layout: each output row scaled
-      const size_t per = (size_t)d.unet_in_ch * 9;
+      const size_t per = (size_t)d.unet_in_ch * (temporal ? 27 : 9);
+      VSB_CHECK(w1.size() == per * z[0], "inc conv shape");
       for (int n = 0; n < z[0]; ++n) for (size_t k = 0; k < per; ++k) w1[n * per + k] *= s[n];
       first_w1 = ws.pool.upload(w1); first_b1 = ws.pool.upload(b);
-      first_wr = ws.vec(P + "inc.res_conv.weight");
-      first_br = ws.vec(P + "inc.res_conv.bias");
+      first_wr = ws.vec(P + "inc.res_conv" + cv + ".weight", (int64_t)z[0] * d.unet_in_ch);
+      first_br = ws.vec(P + "inc.res_conv" + cv + ".bias");
       ws.bn_fold(P + "inc.double_conv.4", s, b);
-      inc_c2 = pack_conv(ws, P + "inc.double_conv.3.weight", &s, b, inc_k);
+      if (temporal) {
+        const HostTensor& w2 = ws.get(P + "inc.double_conv.3.conv.weight");
+        inc_c2 = pack_taps(ws, conv3d_taps(w2, &s, temporal_stack_width(z[0])), b, false);
+      } else {
+        inc_c2 = pack_conv(ws, P + "inc.double_conv.3.weight", &s, b, inc_k);
+      }
     }
     for (int i = 0; i < L - 1; ++i) {
       const std::string D = P + "downs." + std::to_string(i);
@@ -154,9 +193,9 @@ struct UNet {
       if (down_k[i]) { dc.wd = ws.down_s2d(ws.taps(D + ".down.weight")); dc = ws.with_bias(dc, bias); }
       else dc = ws.gemm(ws.taps(D + ".down.weight"), bias);
       down_conv.push_back(dc);
-      down_rb.push_back(pack_resblock(ws, D + ".conv", down_rb_k[i]));
+      down_rb.push_back(pack_block(ws, D + ".conv", down_rb_k[i]));
     }
-    for (int i = 0; i < d.unet_num_blocks; ++i) bott_rb.push_back(pack_resblock(ws, P + "bottleneck.model." + std::to_string(i), bott_rb_k));
+    for (int i = 0; i < d.unet_num_blocks; ++i) bott_rb.push_back(pack_block(ws, P + "bottleneck.model." + std::to_string(i), bott_rb_k));
     std::vector<int> zz(z);
     zz[L - 1] += d.hidden;
     int j = 0;
@@ -173,7 +212,7 @@ struct UNet {
       up_phase_w.push_back(pw); up_border_w.push_back(bw);
       up_lnw.push_back(ws.vec(U + ".up.upsample_block.3.weight"));
       up_lnb.push_back(ws.vec(U + ".up.upsample_block.3.bias"));
-      up_rb.push_back(pack_resblock(ws, U + ".conv", up_rb_k[j]));
+      up_rb.push_back(pack_block(ws, U + ".conv", up_rb_k[j]));
     }
     outc_w = ws.vec(P + "outc.weight");  // [n_out][z0][1][1]
     outc_b = ws.vec(P + "outc.bias");
@@ -186,11 +225,12 @@ struct UNet {
   // packed for it, else the tensor-core GEMM.  Epilogue: bias, ReLU (relu), + the fp16 residual `resid` (pitch w.N), output `out`
   // (pitch ld_out; nullptr: not written) and, fuse_outc, the 1x1 outc + tanh into pl.delta.
   void add_conv(Plan& pl, const ConvW& w, int R, const __half* x, int B, int H, int W, int Cin, int ldx,
-                bool relu, const __half* resid, __half* out, int ld_out, bool fuse_outc = false) const {
+                bool relu, const __half* resid, __half* out, int ld_out, bool fuse_outc = false, const std::string& label = "") const {
     const int N = w.N;
     const bool direct = w.wd != nullptr;
     VSB_CHECK(!direct || (ldx == Cin && (out == nullptr || ld_out == N)), "direct conv: dense input and output");
-    const std::string name = std::string("unet.conv") + (R == 3 ? "3x3" : "1x1") + (direct ? "d" : "") + (fuse_outc ? "+outc." : ".") +
+    const std::string name = !label.empty() ? label :
+                             std::string("unet.conv") + (R == 3 ? "3x3" : "1x1") + (direct ? "d" : "") + (fuse_outc ? "+outc." : ".") +
                              std::to_string(Cin) + "-" + std::to_string(N) + "@" + std::to_string(H);
     if (direct) {
       Conv3DirectOp op; setup_conv3_direct(op, x, B, H, W, Cin, N, w.wd, nsm, R);
@@ -216,10 +256,23 @@ struct UNet {
     vsb::add_conv(pl, op, w, name, nsm);
   }
 
+  // 3x3x3 conv (stride 1, zero pad 1 in space and time) over x [B,H,W,Cin] (pitch ldx) in groups of G frames: the frames' time taps
+  // stacked into the plan's scratch `xs`, then the tensor-core 3x3 conv over it (K = 9 * Cs).  Arguments after ldx as in add_conv.
+  void add_conv3d(Plan& pl, const ConvW& w, const __half* x, int B, int G, int H, int W, int Cin, int ldx, __half* xs,
+                  bool relu, const __half* resid, __half* out, int ld_out, bool fuse_outc = false) const {
+    const int Cs = temporal_stack_width(Cin), sms = nsm;
+    const std::string at = std::to_string(H);
+    pl.add("unet.tstack." + std::to_string(Cin) + "-" + std::to_string(Cs) + "@" + at,
+           [=](cudaStream_t st) { launch_temporal_stack(x, ldx, Cin, (long)H * W, B, G, xs, Cs, sms, st); });
+    add_conv(pl, w, 3, xs, B, H, W, Cs, Cs, relu, resid, out, ld_out, fuse_outc,
+             std::string("unet.conv3x3x3") + (fuse_outc ? "+outc." : ".") + std::to_string(Cin) + "-" + std::to_string(w.N) + "@" + at);
+  }
+
   // ResnetBlock on NHWC fp16 (modules/unet.py:17-39):  out = relu(conv3'(relu(conv3'(x)))) + (conv1(x) + b)
   // `x` has pixel pitch ldx; output written with pitch ld_out.  If fuse_outc: the 1x1 outc + tanh is fused and the
   // block output itself is not written.
-  __half* add_resblock(Plan& pl, const std::string& name, const ResBlockW& w, const __half* x, int B,
+  // G > 0: a temporal block (3x3x3 convs over groups of G frames through the scratch xs, 1x1x1 res conv)
+  __half* add_resblock(Plan& pl, const std::string& name, const ResBlockW& w, const __half* x, int B, int G, __half* xs,
                        int H, int W, int Cin, int ldx, __half* out, int ld_out, bool fuse_outc = false) const {
     const int Cout = w.c1.N;
     const long M = (long)B * H * W;
@@ -227,17 +280,35 @@ struct UNet {
     __half* h = pl.pool.alloc_n<__half>(M * Cout);
     if (!out && !fuse_outc) { out = pl.pool.alloc_n<__half>(M * Cout); ld_out = Cout; }
     add_conv(pl, w.res, 1, x, B, H, W, Cin, ldx, false, nullptr, r, Cout);
-    add_conv(pl, w.c1, 3, x, B, H, W, Cin, ldx, true, nullptr, h, Cout);
-    add_conv(pl, w.c2, 3, h, B, H, W, Cout, Cout, true, r, out, ld_out, fuse_outc);
+    if (G > 0) {
+      add_conv3d(pl, w.c1, x, B, G, H, W, Cin, ldx, xs, true, nullptr, h, Cout);
+      add_conv3d(pl, w.c2, h, B, G, H, W, Cout, Cout, xs, true, r, out, ld_out, fuse_outc);
+    } else {
+      add_conv(pl, w.c1, 3, x, B, H, W, Cin, ldx, true, nullptr, h, Cout);
+      add_conv(pl, w.c2, 3, h, B, H, W, Cout, Cout, true, r, out, ld_out, fuse_outc);
+    }
     pl.tap(name + ".h", h, 1, B, H, W, Cout, Cout);
     pl.tap(name + ".r", r, 1, B, H, W, Cout, Cout);
     if (out) pl.tap(name, out, 1, B, H, W, Cout, ld_out);
     return out;
   }
 
-  void build(Plan& pl, int B) const {
+  // the embed plan of B frames; a temporal U-Net convolves across groups of G consecutive frames (G >= 1, the last group may be
+  // shorter), a 2-D one takes G = 0
+  void build(Plan& pl, int B, int G = 0) const {
     const int S = d.img_size, L = d.unet_levels;
     std::vector<int> z(d.unet_z, d.unet_z + L);
+    VSB_CHECK((G > 0) == (temporal), "temporal group length");
+    // one time-stacked operand buffer for every 3x3x3 conv of the plan (they run one after the other on one stream)
+    __half* xs = nullptr;
+    if (G > 0) {
+      size_t n = 0;
+      for (int i = 0; i < L; ++i) {
+        const int C = (i == L - 1 ? z[i] + d.hidden : z[i]), h = S >> i;
+        n = std::max(n, (size_t)B * h * h * temporal_stack_width(C));
+      }
+      xs = pl.pool.alloc_n<__half>(n);
+    }
     pl.x_res = pl.pool.alloc_n<float>((size_t)B * 3 * S * S);
     pl.tap("x_res", pl.x_res, 0, B, 3, S, S, S);
     pl.delta = pl.pool.alloc_n<float>((size_t)B * d.unet_out_ch * S * S);
@@ -249,14 +320,18 @@ struct UNet {
     {
       const int Z = z[0], yuv = d.yuv, cin = d.unet_in_ch;
       const float *w1 = first_w1, *b1 = first_b1, *wr = first_wr, *br = first_br;
-      pl.add("unet.first", [=](cudaStream_t st) { launch_unet_first(plp->in_imgs, B, S, Z, cin, w1, b1, wr, br, h1, r0, yuv, st); });
+      if (G > 0)
+        pl.add("unet.first3x3x3", [=](cudaStream_t st) { launch_unet_first_t(plp->in_imgs, B, G, S, Z, cin, w1, b1, wr, br, h1, r0, st); });
+      else
+        pl.add("unet.first", [=](cudaStream_t st) { launch_unet_first(plp->in_imgs, B, S, Z, cin, w1, b1, wr, br, h1, r0, yuv, st); });
     }
     pl.tap("first_h", h1, 1, B, S, S, z[0], z[0]);
     pl.tap("first_r", r0, 1, B, S, S, z[0], z[0]);
     std::vector<__half*> skips;  // outputs of inc, downs[0..]
     std::vector<int> skip_ld;
     __half* x = pl.pool.alloc_n<__half>(M0 * z[0]);
-    add_conv(pl, inc_c2, 3, h1, B, S, S, z[0], z[0], true, r0, x, z[0]);
+    if (G > 0) add_conv3d(pl, inc_c2, h1, B, G, S, S, z[0], z[0], xs, true, r0, x, z[0]);
+    else add_conv(pl, inc_c2, 3, h1, B, S, S, z[0], z[0], true, r0, x, z[0]);
     pl.tap("inc", x, 1, B, S, S, z[0], z[0]);
     int ldx = z[0], hs = S;
     const int zb = z[L - 1] + d.hidden;
@@ -282,7 +357,7 @@ struct UNet {
         cat = pl.pool.alloc_n<__half>(Mo * zb);
         out = cat; ld_out = zb;
       }
-      x = add_resblock(pl, "down" + std::to_string(i), down_rb[i], dn, B, ho, ho, z[i + 1], z[i + 1], out, ld_out);
+      x = add_resblock(pl, "down" + std::to_string(i), down_rb[i], dn, B, G, xs, ho, ho, z[i + 1], z[i + 1], out, ld_out);
       ldx = (i == L - 2) ? zb : z[i + 1];
       hs = ho;
       skips.push_back(x); skip_ld.push_back(ldx);
@@ -297,7 +372,7 @@ struct UNet {
     // ---- bottleneck
     x = cat; ldx = zb;
     for (int i = 0; i < d.unet_num_blocks; ++i) {
-      x = add_resblock(pl, "bott" + std::to_string(i), bott_rb[i], x, B, hs, hs, zb, ldx, nullptr, 0);
+      x = add_resblock(pl, "bott" + std::to_string(i), bott_rb[i], x, B, G, xs, hs, hs, zb, ldx, nullptr, 0);
       ldx = zb;
     }
     // ---- ups
@@ -344,7 +419,7 @@ struct UNet {
       }
       pl.tap("up" + std::to_string(j) + "_conv", u, 1, B, ho, ho, Cout, Cout);
       const bool last = (ii == 0);
-      x = add_resblock(pl, "up" + std::to_string(j), up_rb[j], u, B, ho, ho, Cout, Cout, nullptr, 0, /*fuse_outc=*/last);
+      x = add_resblock(pl, "up" + std::to_string(j), up_rb[j], u, B, G, xs, ho, ho, Cout, Cout, nullptr, 0, /*fuse_outc=*/last);
       ldx = Cout; hs = ho;
     }
     pl.tap("delta", pl.delta, 0, B, d.unet_out_ch, S, S, S);

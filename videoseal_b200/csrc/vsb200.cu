@@ -59,7 +59,7 @@ int vsb_model_create(const vsb_model_desc* desc, vsb_model** out) {
 
 int vsb_model_set_tensor(vsb_model* m, const char* name, const float* data, const int64_t* shape, int32_t ndim) {
   VSB_API_BEGIN
-  VSB_CHECK(m && name && data && (shape || ndim == 0) && ndim >= 0 && ndim <= 4, "bad tensor argument");
+  VSB_CHECK(m && name && data && (shape || ndim == 0) && ndim >= 0 && ndim <= 5, "bad tensor argument");   // 5: Conv3d weights
   m->impl.set_tensor(name, data, shape, ndim);
   return VSB_OK;
   VSB_API_END
@@ -70,6 +70,15 @@ int vsb_model_set_pixel_decoder(vsb_model* m, int32_t n_stages, const int32_t* f
   VSB_CHECK(m != nullptr && (factors != nullptr || n_stages == 0), "null argument");
   std::lock_guard<std::recursive_mutex> lk(m->impl.mu);
   m->impl.set_pixel_decoder(n_stages, factors, pixelwise);
+  return VSB_OK;
+  VSB_API_END
+}
+
+int vsb_model_set_unet_temporal(vsb_model* m, int32_t on) {
+  VSB_API_BEGIN
+  VSB_CHECK(m != nullptr, "null argument");
+  std::lock_guard<std::recursive_mutex> lk(m->impl.mu);
+  m->impl.set_unet_temporal(on);
   return VSB_OK;
   VSB_API_END
 }

@@ -59,6 +59,32 @@ inline Taps conv_taps(const HostTensor& w, const std::vector<float>* out_scale =
   return t;
 }
 
+// Conv3d weight [N][C][3][3][3] (3x3x3) or [N][C][1][1][1] times out_scale[n] -> taps.  1x1x1: the 1x1 taps.  3x3x3: the taps of the 3x3
+// conv over the time-stacked operand of temporal.cuh, Cs >= 3C channels [x(t-1) | x(t) | x(t+1) | zeros], K order (r, s, dt, c).
+inline Taps conv3d_taps(const HostTensor& w, const std::vector<float>* out_scale, int Cs) {
+  VSB_CHECK(w.shape.size() == 5 && w.shape[2] == w.shape[3] && w.shape[3] == w.shape[4] && (w.shape[2] == 1 || w.shape[2] == 3),
+            "conv3d weight shape: [N, C, 3, 3, 3] or [N, C, 1, 1, 1]");
+  Taps t;
+  t.N = (int)w.shape[0];
+  const int C = (int)w.shape[1];
+  if (w.shape[2] == 1) {
+    HostTensor w2{w.data, {w.shape[0], w.shape[1], 1, 1}};
+    return conv_taps(w2, out_scale);
+  }
+  VSB_CHECK(Cs >= 3 * C, "conv3d: stacked width");
+  t.C = Cs; t.R = t.S = 3; t.T = 9;
+  t.v.assign((size_t)t.N * 9 * Cs, 0.f);
+  for (int n = 0; n < t.N; ++n)
+    for (int c = 0; c < C; ++c)
+      for (int dt = 0; dt < 3; ++dt)
+        for (int k = 0; k < 9; ++k) {
+          float v = w.data[(((size_t)n * C + c) * 3 + dt) * 9 + k];
+          if (out_scale) v *= (*out_scale)[n];
+          t.v[((size_t)n * 9 + k) * Cs + dt * C + c] = v;
+        }
+  return t;
+}
+
 // The checkpoint as vsb_model_set_tensor delivers it, and the pool of every weight packed from it
 struct Weights {
   std::map<std::string, HostTensor> sd;   // host copies, dropped once the model is finalized

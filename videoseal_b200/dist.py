@@ -8,6 +8,7 @@ training-only (utils/dist.py).  One process per GPU, launched with torchrun.
 """
 from __future__ import annotations
 
+import math
 from typing import Callable, List, Tuple
 
 import torch
@@ -28,6 +29,14 @@ def shard_bounds(num_frames: int, world_size: int, step_size: int = 1) -> List[T
         bounds.append((min(g0 * step_size, num_frames), min(g1 * step_size, num_frames)))
         g0 = g1
     return bounds
+
+
+def shard_unit(model) -> int:
+    """The `step_size` to shard a clip for `model` with: frames that one embed call must see together.  That is a key frame and
+    its step_size - 1 followers, or, for a temporal U-Net, whose 3x3x3 convs mix the key frames of one reference chunk
+    (models/videoseal.py:292-320), whole chunks of chunk_size * step_size frames."""
+    step = int(model.step_size)
+    return step * int(model.chunk_size) if getattr(model, "temporal", False) else step
 
 
 def subshard_bounds(num_frames: int, world_size: int, step_size: int = 1, subshards: int = 2) -> List[List[Tuple[int, int]]]:
@@ -59,11 +68,15 @@ def all_gather_ragged(local: torch.Tensor, sizes: List[int], group=None) -> torc
 
 
 def embed_detect_sharded(embed_fn: Callable, detect_fn: Callable, frames: torch.Tensor, msgs: torch.Tensor, step_size: int,
-                         gather_frames: bool = True, group=None):
-    """Shard `frames` [F,3,H,W] (present on every rank, or at least this rank's range) over the process group, run
+                         gather_frames: bool = True, group=None, model=None):
+    """Shard `frames` [F,3,H,W] (present on every rank, or at least this rank's range) over the process group, cut on multiples
+    of `step_size`, and with `model` given (the Videoseal behind embed_fn) also on multiples of shard_unit(model), so that a temporal
+    U-Net's chunks stay whole; run
     `embed_fn(frames_shard, msgs) -> imgs_w_shard` and `detect_fn(imgs_w_shard) -> logits_shard` locally, and all-gather.
     Returns (imgs_w [F,3,H,W] or the local shard if not gather_frames, logits [F, 1+K], (start, end) of this rank)."""
     world, rank = dist.get_world_size(group), dist.get_rank(group)
+    if model is not None:
+        step_size = math.lcm(step_size, shard_unit(model))
     bounds = shard_bounds(frames.shape[0], world, step_size)
     s, e = bounds[rank]
     local = frames[s:e]

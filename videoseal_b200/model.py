@@ -93,15 +93,17 @@ def trunk_map(spec: dict) -> int:
 
 
 def _create(spec: dict):
-    """Native handle of `spec` without weights or a device.  vsb_model_create, vsb_model_set_vit_extractor and
-    vsb_model_set_pixel_decoder check every rule the kernels place on the model's geometry; a model they do not implement raises
-    NotImplementedError."""
+    """Native handle of `spec` without weights or a device.  vsb_model_create, vsb_model_set_unet_temporal,
+    vsb_model_set_vit_extractor and vsb_model_set_pixel_decoder check every rule the kernels place on the model's geometry; a
+    model they do not implement raises NotImplementedError."""
     L = _lib.lib()
     h = C.c_void_p()
     _lib.check(L.vsb_model_create(C.byref(native_desc(spec)), C.byref(h)))
     pd = spec.get("pixel_decoder", {"pixelwise": False})
     f = pd["upscale_stages"] if pd["pixelwise"] else None
-    rc = L.vsb_model_set_vit_extractor(h, C.byref(native_vit_desc(spec["vit"]))) if "vit" in spec else 0
+    rc = L.vsb_model_set_unet_temporal(h, 1) if spec["unet"].get("temporal", False) else 0
+    if rc == 0 and "vit" in spec:
+        rc = L.vsb_model_set_vit_extractor(h, C.byref(native_vit_desc(spec["vit"])))
     if rc == 0 and f:
         rc = L.vsb_model_set_pixel_decoder(h, len(f), (C.c_int32 * len(f))(*f), 1)
     if rc != 0:
@@ -298,8 +300,10 @@ class Videoseal(nn.Module):
         L = _lib.lib()
         h = _create(self.spec)
         try:
+            temporal = self.temporal
             for k, v in self._sd.items():
-                if k.startswith(("attenuation.", "rgb2yuv.")) or v.dim() > 4:
+                # 5-D tensors: only a temporal U-Net's Conv3d weights are read
+                if k.startswith(("attenuation.", "rgb2yuv.")) or (v.dim() > 4 and not (temporal and k.startswith("embedder.unet."))):
                     continue
                 shape = (C.c_int64 * max(1, v.dim()))(*v.shape)
                 _lib.check(L.vsb_model_set_tensor(h, k.encode(), v.data_ptr(), shape, v.dim()))
@@ -365,11 +369,27 @@ class Videoseal(nn.Module):
         _lib.check(_lib.lib().vsb_embed(
             self._handle(), x.data_ptr(), mm.data_ptr(), mm.shape[0], imgs_w.data_ptr(),
             preds_w.data_ptr() if preds_w is not None else None, F_, H, W, step, _lib.VIDEO_MODES[self.video_mode],
-            int(self.chunk_size), float(self.blender.scaling_i), float(self.blender.scaling_w), flags,
+            self._chunk_keys(is_video, F_), float(self.blender.scaling_i), float(self.blender.scaling_w), flags,
             self._stream()))
         if is_video:
             return {"imgs_w": imgs_w.to(imgs.device), "msgs": msgs[0:1].repeat(F_, 1)}
         return {"msgs": msgs, "preds_w": preds_w.to(imgs.device), "imgs_w": imgs_w.to(imgs.device)}
+
+    @property
+    def temporal(self) -> bool:
+        """True for a temporal U-Net (unet.conv_layer 'conv3d'): its 3x3x3 convs mix the key frames of one embedder call"""
+        return bool(self.spec["unet"].get("temporal", False))
+
+    def _chunk_keys(self, is_video: bool, num_frames: int) -> int:
+        """vsb_embed's chunk_keys: key frames per reference embedder call.  A video call is one chunk of chunk_size key frames
+        (videoseal.py:292-320); in image mode the whole batch is one call (wam.py:134-204), which matters only to a temporal
+        U-Net.  A temporal group must fit one 64-frame sub-batch."""
+        keys = int(self.chunk_size) if is_video or not self.temporal else int(num_frames)
+        if self.temporal and keys > 64:
+            what = f"chunk_size={keys}" if is_video else f"image mode with {keys} images"
+            raise NotImplementedError(f"temporal U-Net: {what} puts more than 64 frames in one 3x3x3 conv group; at most 64 are "
+                                      "implemented")
+        return keys
 
     @property
     def pixelwise(self) -> bool:

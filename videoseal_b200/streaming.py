@@ -44,7 +44,7 @@ def _run(model: Videoseal, clip: np.ndarray, msgs, want_frames: bool, want_logit
         model._handle(), clip.ctypes.data_as(C.c_void_p), m8.ctypes.data_as(C.c_void_p) if m8 is not None else None, n_msgs,
         out.ctypes.data_as(C.c_void_p) if out is not None else None,
         logits.ctypes.data_as(C.c_void_p) if logits is not None else None,
-        F_, H, W, model.step_size if is_video else 1, _lib.VIDEO_MODES[model.video_mode], int(model.chunk_size),
+        F_, H, W, model.step_size if is_video else 1, _lib.VIDEO_MODES[model.video_mode], model._chunk_keys(is_video, F_),
         float(model.blender.scaling_i), float(model.blender.scaling_w), flags))
     return out, (torch.from_numpy(logits) if logits is not None else None), msgs
 
