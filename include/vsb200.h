@@ -86,7 +86,8 @@ int vsb_version(void);
  * VSB_ERR_UNSUPPORTED unless: BatchNorm+ReLU; U-Net widths 16, 32, multiples of 64, or 8 in leading levels but not the last; up
  * blocks of 8 * 2^k <= 512 channels; img_size >> (levels - 1) >= 16; img_size <= 768 with 8 channels, whose layers must fit their
  * rings; JND channels 1 or 3.  VSB_ERR_INVALID unless: 2..6 levels, unet_in_ch 1 (yuv) or 3, unet_out_ch 1..3, img_size a multiple
- * of 128, hidden a multiple of 8, ConvNeXt widths even and not shrinking. */
+ * of 128, hidden a multiple of 8, ConvNeXt widths even and not shrinking.  unet_levels 0 with unet_in_ch = unet_out_ch = 3
+ * leaves the embedder to vsb_model_set_hidden_embedder; the U-Net rules are then checked at finalize if none was set. */
 int vsb_model_create(const vsb_model_desc* desc, vsb_model** out);
 /* Temporal U-Net (unet.conv_layer 'conv3d', modules/common.py Conv3dWrapper), called between create and finalize; no CUDA call.
  * on = 1: every ResnetBlock's 3x3 convs are 3x3x3 over the key frames of one embedder call (see vsb_embed) and its res_conv 1x1x1; the
@@ -123,6 +124,28 @@ typedef struct vsb_vit_desc {
  * 2n - 1 rows of a relative-position table must fit in 64).  VSB_ERR_INVALID for depth < 1, mask bits at or above
  * depth, or flags other than 0 / 1. */
 int vsb_model_set_vit_extractor(vsb_model* m, const vsb_vit_desc* vit);
+/* HiDDeN networks (modules/hidden.py HiddenEncoder / HiddenDecoder; models/embedder.py HiddenEmbedder, models/extractor.py
+ * HiddenExtractor): stacks of ConvBNRelu = 3x3 conv (pad 1, bias) + norm + activation on x = 2 imgs - 1.
+ *   embedder: num_layers ConvBNRelu (3 -> z, then z -> z), the concat [2 m - 1 as nbits constant planes | features | x], one
+ *             ConvBNRelu (nbits + z + 3 -> z), final_layer 1x1 (z -> 3), tanh when last_tanh.  Its output is the delta (3 channels).
+ *   extractor: num_layers ConvBNRelu (num_blocks + 1 of the reference), the mean over the map, Linear(z -> 1 + nbits): the pooled
+ *             logits.
+ * The embedder replaces the U-Net: the descriptor's unet_* fields are then unused (unet_levels 0, unet_in_ch = unet_out_ch = 3).  The extractor replaces the
+ * trunk and the pixel decoder: ext_* zero, no vsb_model_set_vit_extractor, no pixel-wise vsb_model_set_pixel_decoder. */
+typedef struct vsb_hidden_desc {
+  int32_t z_channels;        /* width of every layer */
+  int32_t num_layers;        /* ConvBNRelu layers before the concat (embedder) / before the pooling (extractor) */
+  int32_t norm;              /* 0 BatchNorm2d (eval, eps 1e-5), 1 GroupNorm(8, z) (eps 1e-5, affine) */
+  int32_t act;               /* 0 ReLU, 1 GELU (erf) */
+  int32_t last_tanh;         /* embedder: tanh after final_layer; extractor: 0 */
+} vsb_hidden_desc;
+/* Called after vsb_model_create and before finalize; no CUDA call.  VSB_ERR_STATE after finalize (and for the extractor after a
+ * SAM-ViT trunk or a pixel-wise decoder).  VSB_ERR_UNSUPPORTED unless z_channels is 64 and norm / act are 0 or 1.
+ * VSB_ERR_INVALID for num_layers outside 1..64, last_tanh other than 0 / 1 (0 for the extractor), nbits < 1, img_size not a positive
+ * multiple of 128, or a descriptor that does not leave room for it (unet_levels != 0 or RGB channels other than 3; ext_dims /
+ * ext_depths != 0).  Such a descriptor with no HiDDeN embedder fails at finalize with the U-Net's VSB_ERR_INVALID. */
+int vsb_model_set_hidden_embedder(vsb_model* m, const vsb_hidden_desc* h);
+int vsb_model_set_hidden_extractor(vsb_model* m, const vsb_hidden_desc* h);
 /* fold BN, pack to fp16 KRSC, upload to `device`, build nothing else (plans are built lazily per batch shape) */
 int vsb_model_finalize(vsb_model* m, int32_t device);
 void vsb_model_destroy(vsb_model* m);
@@ -251,7 +274,12 @@ int64_t vsb_debug_get_tensor(vsb_model* m, const char* name, float* host_out, in
  * and in every SAM-ViT detect plan: vit.patches [B, G, G, 768] fp16 im2col rows (K order c, r, s);  vit.embed  the stream after
  * the patch GEMM + position table;  vit.blk{L}.qkv / .attn / .ln2 / .hid  the last block's qkv rows, attention output, LayerNorm 2
  * output and GELU hidden rows (fp16);  vit.blk{L}  the stream after it;  vit.x16  its fp16 copy the neck reads;  vit.neck_ln1  the
- * fp16 LayerNorm of the 1x1 output;  vit.neck3x3  fp32 the 3x3 output;  vit.neck  the fp16 map the head reads. */
+ * fp16 LayerNorm of the 1x1 output;  vit.neck3x3  fp32 the 3x3 output;  vit.neck  the fp16 map the head reads.
+ * HiDDeN plans (embed and detect; setting the seam also drops the cached HiDDeN embed plans) reuse two map buffers and one pre-norm
+ * map; while on, copies of the first two layers' outputs and (GroupNorm) pre-norm maps are taps henc.{0,1} / henc.{0,1}.pre and
+ * hdec.{0,1} / hdec.{0,1}.pre.  Always: the GroupNorm partials <henc|hdec>.{i}.stats (fp64 pairs as four fp32 words), the last
+ * maps henc.{L-1}, hdec.{L-3..L-2}, henc.cat_x (image columns + message table), henc.cat.pre, hdec.{L-1}.pre, henc.msg_table,
+ * head_pooled and delta. */
 int vsb_debug_keep_inputs(vsb_model* m, int32_t on);
 /* host-only: the variant finalize_op chose for each tensor-core step of the most recent plan, one line per step in plan order:
  * "name\tM=..\tN=..\tK=..\tblock_n=..\ttma_store=0|1|2\tb_resident=0|1\tb_fixed_ntile=0|1\tkernel=128|longk\tbias_global=0|1\t

@@ -15,7 +15,8 @@ EXPORTS = [
     "vsb_detect_host", "vsb_embed_detect_host", "vsb_frames_host_u8", "vsb_launch_count", "vsb_profile_enable", "vsb_profile_read", "vsb_debug_get_tensor", "vsb_debug_keep_inputs", "vsb_debug_plan_gemms",
     "vsb_debug_conv",
     "vsb_debug_resample_table", "vsb_debug_resample_table2", "vsb_debug_last_dispatch", "vsb_quality_workspace_bytes", "vsb_ssim", "vsb_model_set_vit_extractor",
-    "vsb_augment_workspace_bytes", "vsb_augment", "vsb_model_set_unet_temporal",
+    "vsb_augment_workspace_bytes", "vsb_augment", "vsb_model_set_unet_temporal", "vsb_model_set_hidden_embedder",
+    "vsb_model_set_hidden_extractor",
 ]
 
 FLAG_CLAMP, FLAG_LOWRES_ATTN, FLAG_NO_ATTENUATION, FLAG_RESIZE_NO_AA = 1, 2, 4, 8
@@ -41,6 +42,10 @@ class VitDesc(C.Structure):
         ("window_size", C.c_int32), ("global_mask", C.c_uint32), ("mlp_dim", C.c_int32), ("out_chans", C.c_int32),
         ("qkv_bias", C.c_int32), ("use_rel_pos", C.c_int32),
     ]
+
+
+class HiddenDesc(C.Structure):
+    _fields_ = [("z_channels", C.c_int32), ("num_layers", C.c_int32), ("norm", C.c_int32), ("act", C.c_int32), ("last_tanh", C.c_int32)]
 
 
 class ConvTest(C.Structure):
@@ -78,6 +83,8 @@ def lib():
     L.vsb_model_set_pixel_decoder.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_int32]
     L.vsb_model_set_vit_extractor.argtypes = [C.c_void_p, C.POINTER(VitDesc)]
     L.vsb_model_set_unet_temporal.argtypes = [C.c_void_p, C.c_int32]
+    L.vsb_model_set_hidden_embedder.argtypes = [C.c_void_p, C.POINTER(HiddenDesc)]
+    L.vsb_model_set_hidden_extractor.argtypes = [C.c_void_p, C.POINTER(HiddenDesc)]
     L.vsb_model_finalize.argtypes = [C.c_void_p, C.c_int32]
     L.vsb_model_destroy.argtypes = [C.c_void_p]
     L.vsb_model_destroy.restype = None

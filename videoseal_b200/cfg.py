@@ -70,24 +70,88 @@ def spec_from_card(card: dict) -> dict:
     img_size = a["img_size_proc"] if "img_size_proc" in a else a["img_size_extractor"]
     emb_name = str(card["embedder"]["model"])
     ext_name = str(card["extractor"]["model"])
-    if not emb_name.startswith("unet"):
-        raise NotImplementedError(f"embedder '{emb_name}': only the unet* family is on the CUDA hot path")
+    if not emb_name.startswith(("unet", "hidden")):
+        raise NotImplementedError(f"embedder '{emb_name}': only the unet* and hidden* families are on the CUDA hot path")
     is_vit = ext_name.startswith("sam")
-    if not (ext_name.startswith("convnext") or is_vit):
-        raise NotImplementedError(f"extractor '{ext_name}': only the convnext* and sam* families are on the CUDA hot path")
-    u = card["embedder"]["params"]["unet"]
-    mp = card["embedder"]["params"].get("msg_processor", {})
-    if mp.get("msg_processor_type", "binary+concat") != "binary+concat":
-        raise NotImplementedError("only 'binary+concat' message processors are implemented")
+    if not (ext_name.startswith(("convnext", "hidden")) or is_vit):
+        raise NotImplementedError(f"extractor '{ext_name}': only the convnext*, sam* and hidden* families are on the CUDA hot path")
     if str(a.get("blending_method", "additive")) != "additive":
         raise NotImplementedError("only additive blending is implemented (all shipped cards use it)")
+    if emb_name.startswith("hidden"):
+        embedder = {"hidden_encoder": _hidden(card["embedder"]["params"], embedder=True)}
+    else:
+        embedder = _unet(card["embedder"]["params"])
+    if ext_name.startswith("hidden"):
+        extractor = {"hidden_decoder": _hidden(card["extractor"]["params"], embedder=False),
+                     "pixel_decoder": {"pixelwise": False, "upscale_stages": [1]}}
+    else:
+        extractor = _trunk(card["extractor"]["params"], nbits, is_vit)
+    att = str(a.get("attenuation", "None"))
+    jnd = (0, 0)
+    if att.lower().startswith("jnd"):
+        att_cfg = yaml.safe_load(open(resolve_config_path(a.get("attenuation_config", "configs/attenuation.yaml"))))
+        jnd = (int(att_cfg[att]["in_channels"]), int(att_cfg[att]["out_channels"]))
+    spec = {
+        "nbits": nbits, "hidden": int(nbits * hsm), "img_size": int(img_size), "yuv": "yuv" in emb_name,
+        "scaling_w": float(a["scaling_w"]), "scaling_i": float(a["scaling_i"]),
+        "chunk_size": int(a.get("videoseal_chunk_size", a.get("videowam_chunk_size", 8))),
+        "step_size": int(a.get("videoseal_step_size", a.get("videowam_step_size", 4))),
+        **embedder,
+        **extractor,
+        "jnd": jnd, "attenuation": att,
+    }
+    # the geometry rules of the kernels (widths, sizes, pixel-decoder stages) live in the native library: a dry run, no GPU needed
+    from .model import check_native
+    check_native(spec)
+    return spec
+
+
+_HIDDEN_NORMS = {"batch": 0, "group": 1}
+_HIDDEN_ACTS = {"relu": 0, "gelu": 1}
+
+
+def _hidden(p: dict, embedder: bool) -> dict:
+    """spec['hidden_encoder'] / spec['hidden_decoder'] of a hidden* preset (modules/hidden.py HiddenEncoder / HiddenDecoder; the
+    preset's num_bits is replaced by args.nbits, embedder.py:263-268, extractor.py:183-188)"""
+    what = "HiDDeN embedder" if embedder else "HiDDeN extractor"
+    norm, act = str(p["normalization"]), str(p["activation"])
+    if not any(norm.startswith(k) for k in _HIDDEN_NORMS):   # common.py get_normalization matches on the prefix
+        raise NotImplementedError(f"{what}: normalization '{norm}' is not implemented (batch, group)")
+    if act not in _HIDDEN_ACTS:
+        raise NotImplementedError(f"{what}: activation '{act}' is not implemented (relu, gelu)")
+    if int(p.get("in_channels", 3)) != 3 or (embedder and int(p.get("out_channels", 3)) != 3):
+        raise NotImplementedError(f"{what}: in_channels / out_channels other than 3 are not implemented")
+    if not embedder and p.get("pixelwise", False):
+        raise NotImplementedError(f"{what}: pixelwise=True (per-pixel maps) is not implemented")
+    h = {"z_channels": int(p["z_channels"]), "num_blocks": int(p["num_blocks"]),
+         "normalization": next(k for k in _HIDDEN_NORMS if norm.startswith(k)), "activation": act}
+    if embedder:
+        h["last_tanh"] = bool(p.get("last_tanh", True))
+    return h
+
+
+def _unet(ep: dict) -> dict:
+    """spec['unet'] of a unet* embedder (embedder.py:270-282)"""
+    u = ep["unet"]
+    mp = ep.get("msg_processor", {})
+    if mp.get("msg_processor_type", "binary+concat") != "binary+concat":
+        raise NotImplementedError("only 'binary+concat' message processors are implemented")
     conv_layer = str(u.get("conv_layer", "conv2d"))
     if conv_layer not in ("conv2d", "conv3d"):
         raise NotImplementedError(f"U-Net conv_layer '{conv_layer}' is not implemented (conv2d, or conv3d with BatchNorm + ReLU)")
     if conv_layer == "conv3d" and (str(u["activation"]) != "relu" or not str(u["normalization"]).startswith("batch")):
         raise NotImplementedError(f"temporal (conv3d) U-Net with {u['activation']}/{u['normalization']}: only BatchNorm + ReLU is "
                                   "implemented")
-    ep = card["extractor"]["params"]
+    return {"unet": {
+        "in_channels": int(u["in_channels"]), "out_channels": int(u["out_channels"]),
+        "z": [int(u["z_channels"]) * int(m) for m in u["z_channels_mults"]], "num_blocks": int(u["num_blocks"]),
+        "activation": str(u["activation"]), "normalization": str(u["normalization"]),
+        "last_tanh": bool(u.get("last_tanh", True)), "temporal": conv_layer == "conv3d",
+    }}
+
+
+def _trunk(ep: dict, nbits: int, is_vit: bool) -> dict:
+    """spec['convnext'] or spec['vit'] and spec['pixel_decoder'] of a convnext* / sam* extractor"""
     pd = ep.get("pixel_decoder", {})
     pixelwise = bool(pd.get("pixelwise", False))
     stages = [int(f) for f in pd.get("upscale_stages", [1])]
@@ -102,30 +166,7 @@ def spec_from_card(card: dict) -> dict:
         raise NotImplementedError(f"pixel decoder: upscale_type '{pd.get('upscale_type')}' is not implemented (only 'bilinear')")
     enc = ep["encoder"]
     trunk = _vit_trunk(enc) if is_vit else _convnext_trunk(ep, enc, nbits, pixelwise)
-    att = str(a.get("attenuation", "None"))
-    jnd = (0, 0)
-    if att.lower().startswith("jnd"):
-        att_cfg = yaml.safe_load(open(resolve_config_path(a.get("attenuation_config", "configs/attenuation.yaml"))))
-        jnd = (int(att_cfg[att]["in_channels"]), int(att_cfg[att]["out_channels"]))
-    spec = {
-        "nbits": nbits, "hidden": int(nbits * hsm), "img_size": int(img_size), "yuv": "yuv" in emb_name,
-        "scaling_w": float(a["scaling_w"]), "scaling_i": float(a["scaling_i"]),
-        "chunk_size": int(a.get("videoseal_chunk_size", a.get("videowam_chunk_size", 8))),
-        "step_size": int(a.get("videoseal_step_size", a.get("videowam_step_size", 4))),
-        "unet": {
-            "in_channels": int(u["in_channels"]), "out_channels": int(u["out_channels"]),
-            "z": [int(u["z_channels"]) * int(m) for m in u["z_channels_mults"]], "num_blocks": int(u["num_blocks"]),
-            "activation": str(u["activation"]), "normalization": str(u["normalization"]),
-            "last_tanh": bool(u.get("last_tanh", True)), "temporal": conv_layer == "conv3d",
-        },
-        **trunk,
-        "pixel_decoder": {"pixelwise": pixelwise, "upscale_stages": stages},
-        "jnd": jnd, "attenuation": att,
-    }
-    # the geometry rules of the kernels (widths, sizes, pixel-decoder stages) live in the native library: a dry run, no GPU needed
-    from .model import check_native
-    check_native(spec)
-    return spec
+    return {**trunk, "pixel_decoder": {"pixelwise": pixelwise, "upscale_stages": stages}}
 
 
 def _convnext_trunk(ep: dict, enc: dict, nbits: int, pixelwise: bool) -> dict:

@@ -7,6 +7,7 @@
 
 #include "convnext.cuh"
 #include "decoder.cuh"
+#include "hidden.cuh"
 #include "resize_blend_host.cuh"
 #include "unet.cuh"
 #include "vit_trunk.cuh"
@@ -25,6 +26,7 @@ class Model {
   ConvNeXt cnx;
   VitTrunk vit;
   Decoder dec;
+  Hidden henc, hdec;   // HiDDeN embedder / extractor, in place of the U-Net / the trunk and decoder (vsb_model_set_hidden_*)
 
   // grow-only device staging for the host-buffer entry points (no cudaMalloc on the steady-state path)
   struct Staging { void* p = nullptr; size_t cap = 0; };
@@ -53,23 +55,52 @@ class Model {
   //   resize: MT, GST, vec, toy, OW       blend: 3 (jnd_blend3_kernel) or 2 (jnd_blend2_kernel), VEC, FASTUP, CD, JIN
   int32_t last_resize[5] = {-1, -1, -1, -1, -1};
   int32_t last_blend[5] = {-1, -1, -1, -1, -1};
-  // test seam (vsb_debug_keep_inputs): detect plans copy the trunk's in-place buffers aside where its steps read them
+  // test seam (vsb_debug_keep_inputs): detect plans (and HiDDeN embed plans) copy buffers that later steps overwrite aside
   bool keep_inputs = false;
   void set_keep_inputs(bool on) {
     keep_inputs = on;
     for (auto& kv : detect_plans) if (kv.second.get() == last_plan) last_plan = nullptr;
     detect_plans.clear();
+    if (henc.on) {   // HiDDeN embed plans have the seam too (Hidden::build)
+      for (auto& kv : embed_plans) if (kv.second.get() == last_plan) last_plan = nullptr;
+      embed_plans.clear();
+    }
   }
 
   // vsb_model_create: every rule that depends only on the descriptor, and the U-Net's kernels (no CUDA calls)
+  // A descriptor with no U-Net levels and 3 input / output channels leaves the embedder to vsb_model_set_hidden_embedder: its U-Net
+  // rules are checked at finalize when no HiDDeN embedder was set (so such a descriptor still fails, with the U-Net's message).
   explicit Model(const vsb_model_desc& desc) : d(desc) {
-    unet.check(d);
+    if (!other_embedder()) unet.check(d);
     if (d.jnd_in_ch != 0 && !((d.jnd_in_ch == 1 || d.jnd_in_ch == 3) && (d.jnd_out_ch == 1 || d.jnd_out_ch == 3)))
       throw Error("JND attenuation: in_channels / out_channels must be 1 or 3 (configs/attenuation.yaml)", kErrUnsupported);
     ConvNeXt::check(d);
-    unet.choose_kernels();
+    if (!other_embedder()) unet.choose_kernels();
   }
+  // no U-Net levels but the embedder's RGB in / out channels: the embedder is set by vsb_model_set_hidden_embedder
+  bool other_embedder() const { return d.unet_levels == 0 && d.unet_in_ch == 3 && d.unet_out_ch == 3; }
   void check_unfinalized() const { if (finalized) throw Error("model already finalized", kErrState); }
+  // channels of the embedder's output delta
+  int delta_ch() const { return henc.on ? 3 : d.unet_out_ch; }
+  void set_hidden_embedder(const vsb_hidden_desc& h) {
+    check_unfinalized();
+    if (!other_embedder())
+      throw Error("vsb_model_set_hidden_embedder: the descriptor describes a U-Net (a HiDDeN embedder needs unet_levels 0 and unet_in_ch / "
+                  "unet_out_ch 3)", kErrInvalid);
+    Hidden e;
+    e.set(h, true, d);
+    henc = e;
+  }
+  void set_hidden_extractor(const vsb_hidden_desc& h) {
+    check_unfinalized();
+    if (vit.on || dec.pixelwise) throw Error("vsb_model_set_hidden_extractor: the model already has a SAM-ViT trunk or a pixel-wise decoder", kErrState);
+    for (int s = 0; s < 4; ++s)
+      if (d.ext_dims[s] != 0 || d.ext_depths[s] != 0)
+        throw Error("vsb_model_set_hidden_extractor: the descriptor also describes a ConvNeXt trunk (ext_dims / ext_depths != 0)", kErrInvalid);
+    Hidden e;
+    e.set(h, false, d);
+    hdec = e;
+  }
   void set_tensor(const char* name, const float* data, const int64_t* shape, int ndim) {
     check_unfinalized();
     HostTensor t;
@@ -79,6 +110,7 @@ class Model {
   }
   void set_pixel_decoder(int n, const int32_t* f, int pw) {
     check_unfinalized();
+    if (hdec.on && pw != 0) throw Error("HiDDeN extractor: per-pixel maps (pixelwise) are not implemented", kErrUnsupported);
     dec.set(n, f, pw, vit.on || d.ext_stem_stride == 4, d.nbits, [&] { return std::make_pair(trunk_width(), trunk_map()); });
   }
   // the U-Net's rules and kernel choice again, for a temporal U-Net
@@ -94,6 +126,7 @@ class Model {
   void set_vit_extractor(const vsb_vit_desc& v) {
     check_unfinalized();
     if (dec.pixelwise) throw Error("vsb_model_set_vit_extractor must come before vsb_model_set_pixel_decoder", kErrState);
+    if (hdec.on) throw Error("vsb_model_set_vit_extractor: the model already has a HiDDeN extractor", kErrState);
     vit.set(v, d.img_size);
   }
   int trunk_width() const { return vit.on ? vit.width() : d.ext_dims[3]; }
@@ -118,10 +151,17 @@ class Model {
     if (prop.major != 9 || prop.minor != 0) throw Error("libvsb200 is built for sm_90a only (found sm_" + std::to_string(prop.major) + std::to_string(prop.minor) + ")", kErrUnsupported);
     device = dev;
     num_sms = prop.multiProcessorCount;
-    unet.pack(ws, num_sms);
-    if (vit.on) vit.pack(ws, d.img_size);
-    else cnx.pack(ws, d);
-    dec.pack(ws, d.nbits);
+    if (henc.on) henc.pack(ws, num_sms);
+    else {
+      if (other_embedder()) unet.check(d);   // neither a U-Net nor a HiDDeN embedder: the U-Net's rules fail
+      unet.pack(ws, num_sms);
+    }
+    if (hdec.on) hdec.pack(ws, num_sms);
+    else {
+      if (vit.on) vit.pack(ws, d.img_size);
+      else cnx.pack(ws, d);
+      dec.pack(ws, d.nbits);
+    }
     ws.sd.clear();  // host copies no longer needed
     finalized = true;
   }
@@ -153,12 +193,19 @@ class Model {
   }
   // embed plans are keyed by B + kPlanGroup * G: a temporal U-Net's plan also depends on its group length G (0 for a 2-D U-Net)
   static constexpr int kPlanGroup = 128;
-  void build_embed_plan(Plan& pl, int key) { unet.build(pl, key % kPlanGroup, key / kPlanGroup); }
+  void build_embed_plan(Plan& pl, int key) {
+    if (!henc.on) { unet.build(pl, key % kPlanGroup, key / kPlanGroup); return; }
+    const int S = d.img_size;
+    pl.x_res = pl.pool.alloc_n<float>((size_t)key * 3 * S * S);
+    pl.tap("x_res", pl.x_res, 0, key, 3, S, S, S);
+    henc.build(pl, key, S, keep_inputs);
+  }
   void build_detect_plan(Plan& pl, int B) {
     const int S = d.img_size;
     pl.x_res = pl.pool.alloc_n<float>((size_t)B * 3 * S * S);
     pl.tap("x_res", pl.x_res, 0, B, 3, S, S, S);
     pl.logits = pl.pool.alloc_n<float>((size_t)B * (1 + d.nbits));
+    if (hdec.on) { hdec.build(pl, B, S, keep_inputs); return; }
     const FeatureMap m = vit.on ? vit.build(pl, B, S, num_sms, keep_inputs) : cnx.build(pl, B, d, num_sms, keep_inputs);
     dec.build(pl, B, m, vit.on ? "vit." : "cnx.", d.nbits, num_sms);
   }
@@ -206,7 +253,7 @@ class Model {
     check_ready();
     const size_t n = (size_t)F * 3 * H * W;
     const bool use_jnd = !(flags & VSB_FLAG_NO_ATTENUATION) && d.jnd_in_ch != 0;
-    const size_t np = (size_t)F * (use_jnd ? std::max(d.unet_out_ch, d.jnd_out_ch) : d.unet_out_ch) * H * W;
+    const size_t np = (size_t)F * (use_jnd ? std::max(delta_ch(), d.jnd_out_ch) : delta_ch()) * H * W;
     float* imgs = (float*)stage(0, n * sizeof(float));
     float* out = (float*)stage(1, n * sizeof(float));
     float* pw = preds_w_h ? (float*)stage(2, np * sizeof(float)) : nullptr;
@@ -380,7 +427,7 @@ class Model {
     for (int b0 = 0; b0 < B; b0 += kMaxBatch) {
       const int n = std::min(kMaxBatch, B - b0);
       Plan* pl = run_unet(x + (size_t)b0 * 3 * S * S, msgs + (n_msgs == 1 ? 0 : (size_t)b0 * d.nbits), n_msgs == 1 ? 0 : d.nbits, n, G, st);
-      VSB_CUDA(cudaMemcpyAsync(delta + (size_t)b0 * d.unet_out_ch * S * S, pl->delta, (size_t)n * d.unet_out_ch * S * S * sizeof(float),
+      VSB_CUDA(cudaMemcpyAsync(delta + (size_t)b0 * delta_ch() * S * S, pl->delta, (size_t)n * delta_ch() * S * S * sizeof(float),
                                cudaMemcpyDeviceToDevice, st));
     }
   }
@@ -403,7 +450,7 @@ class Model {
     const ResampleMode rm = same ? ResampleMode() : resample_mode(flags);   // (the flags are read only when a resize happens)
     const bool use_jnd = !(flags & VSB_FLAG_NO_ATTENUATION) && d.jnd_in_ch != 0;
     // channels of hmaps * preds_w (broadcast): what `preds_w` holds and what the low-resolution path hands to the blend
-    const int PC = use_jnd ? std::max(d.unet_out_ch, d.jnd_out_ch) : d.unet_out_ch;
+    const int PC = use_jnd ? std::max(delta_ch(), d.jnd_out_ch) : delta_ch();
     const bool lowres = use_jnd && (flags & VSB_FLAG_LOWRES_ATTN);
     const long fstride = (long)3 * H * W;
     const int nkeys = (F + step - 1) / step;
@@ -440,7 +487,7 @@ class Model {
       memset(&bp, 0, sizeof(bp));
       bp.imgs = imgs + (size_t)f0 * fstride; bp.imgs_w = imgs_w + (size_t)f0 * fstride;
       bp.preds_w = preds_w ? preds_w + (size_t)f0 * PC * H * W : nullptr;
-      bp.F = nf; bp.H = H; bp.W = W; bp.PH = S; bp.PW = S; bp.CD = d.unet_out_ch;
+      bp.F = nf; bp.H = H; bp.W = W; bp.PH = S; bp.PW = S; bp.CD = delta_ch();
       bp.jnd_in = d.jnd_in_ch ? d.jnd_in_ch : 1; bp.jnd_out = d.jnd_out_ch ? d.jnd_out_ch : 1;
       bp.clamp = (flags & VSB_FLAG_CLAMP) ? 1 : 0; bp.identity_resample = same ? 1 : 0;
       bp.scaling_i = scaling_i; bp.scaling_w = scaling_w;
@@ -450,7 +497,7 @@ class Model {
         float* lowres_buf = (float*)stage(7, (size_t)nf * PC * S * S * sizeof(float));
         VSB_CHECK(nf <= 65535, "too many frames per key-frame batch");
         prof_scope("pw.jnd_lowres@" + std::to_string(nf), st, 1, [&] {
-          launch_jnd_lowres(frames_res, delta, lowres_buf, nf, S, S, d.unet_out_ch, step, balt, bint, bp.jnd_in, bp.jnd_out, st);
+          launch_jnd_lowres(frames_res, delta, lowres_buf, nf, S, S, delta_ch(), step, balt, bint, bp.jnd_in, bp.jnd_out, st);
         });
         bp.delta = lowres_buf; bp.step = 1; bp.alternate = 0; bp.interp_chunk = 0; bp.use_jnd = 0; bp.CD = PC;
       } else {

@@ -92,6 +92,24 @@ int vsb_model_set_vit_extractor(vsb_model* m, const vsb_vit_desc* vit) {
   VSB_API_END
 }
 
+int vsb_model_set_hidden_embedder(vsb_model* m, const vsb_hidden_desc* h) {
+  VSB_API_BEGIN
+  VSB_CHECK(m != nullptr && h != nullptr, "null argument");
+  std::lock_guard<std::recursive_mutex> lk(m->impl.mu);
+  m->impl.set_hidden_embedder(*h);
+  return VSB_OK;
+  VSB_API_END
+}
+
+int vsb_model_set_hidden_extractor(vsb_model* m, const vsb_hidden_desc* h) {
+  VSB_API_BEGIN
+  VSB_CHECK(m != nullptr && h != nullptr, "null argument");
+  std::lock_guard<std::recursive_mutex> lk(m->impl.mu);
+  m->impl.set_hidden_extractor(*h);
+  return VSB_OK;
+  VSB_API_END
+}
+
 int vsb_model_finalize(vsb_model* m, int32_t device) {
   VSB_API_BEGIN
   VSB_CHECK(m != nullptr, "null model");

@@ -56,17 +56,20 @@ def native_desc(spec: dict) -> _lib.ModelDesc:
     """vsb_model_desc of `spec` (cfg.spec_from_card)"""
     d = _lib.ModelDesc()
     d.nbits, d.hidden, d.img_size, d.yuv = spec["nbits"], spec["hidden"], spec["img_size"], int(spec["yuv"])
-    u = spec["unet"]
-    d.unet_in_ch, d.unet_out_ch, d.unet_levels = u["in_channels"], u["out_channels"], len(u["z"])
-    for i, z in enumerate(u["z"]):
-        d.unet_z[i] = z
-    d.unet_num_blocks = u["num_blocks"]
-    acts, norms = {"relu": 0, "silu": 1}, {"batch": 0, "rms": 1}
-    if u["activation"] not in acts or not any(u["normalization"].startswith(k) for k in norms):
-        raise NotImplementedError(f"U-Net activation/normalization {u['activation']}/{u['normalization']} not implemented")
-    d.unet_act = acts[u["activation"]]
-    d.unet_norm = 0 if u["normalization"].startswith("batch") else 1
-    d.unet_last_tanh = int(u["last_tanh"])
+    u = spec.get("unet")          # a HiDDeN embedder spec leaves the U-Net fields zero but its RGB channels
+    if u is None:
+        d.unet_in_ch, d.unet_out_ch = 3, 3
+    else:
+        d.unet_in_ch, d.unet_out_ch, d.unet_levels = u["in_channels"], u["out_channels"], len(u["z"])
+        for i, z in enumerate(u["z"]):
+            d.unet_z[i] = z
+        d.unet_num_blocks = u["num_blocks"]
+        acts, norms = {"relu": 0, "silu": 1}, {"batch": 0, "rms": 1}
+        if u["activation"] not in acts or not any(u["normalization"].startswith(k) for k in norms):
+            raise NotImplementedError(f"U-Net activation/normalization {u['activation']}/{u['normalization']} not implemented")
+        d.unet_act = acts[u["activation"]]
+        d.unet_norm = 0 if u["normalization"].startswith("batch") else 1
+        d.unet_last_tanh = int(u["last_tanh"])
     cn = spec.get("convnext")     # a SAM-ViT spec leaves the ConvNeXt fields zero
     if cn is not None:
         for i in range(4):
@@ -87,6 +90,26 @@ def native_vit_desc(vit: dict) -> _lib.VitDesc:
     return v
 
 
+def native_hidden_desc(h: dict, embedder: bool) -> _lib.HiddenDesc:
+    """vsb_hidden_desc of spec['hidden_encoder'] / spec['hidden_decoder'] (cfg.spec_from_card): the encoder's conv_bns hold
+    num_blocks ConvBNRelu, the decoder's layers num_blocks + 1"""
+    v = _lib.HiddenDesc()
+    v.z_channels, v.num_layers = h["z_channels"], h["num_blocks"] + (0 if embedder else 1)
+    v.norm = {"batch": 0, "group": 1}[h["normalization"]]
+    v.act = {"relu": 0, "gelu": 1}[h["activation"]]
+    v.last_tanh = int(h.get("last_tanh", False))
+    return v
+
+
+def delta_channels(spec: dict) -> int:
+    """channels of the embedder's output (the U-Net's out_channels; 3 for a HiDDeN encoder)"""
+    return spec["unet"]["out_channels"] if "unet" in spec else 3
+
+
+def embedder_in_channels(spec: dict) -> int:
+    return spec["unet"]["in_channels"] if "unet" in spec else 3
+
+
 def trunk_map(spec: dict) -> int:
     """side of the extractor trunk's output map: img_size / 16 tokens for a SAM-ViT, img_size / 32 for the ConvNeXt trunks"""
     return spec["img_size"] // (16 if "vit" in spec else 32)
@@ -94,14 +117,21 @@ def trunk_map(spec: dict) -> int:
 
 def _create(spec: dict):
     """Native handle of `spec` without weights or a device.  vsb_model_create, vsb_model_set_unet_temporal,
-    vsb_model_set_vit_extractor and vsb_model_set_pixel_decoder check every rule the kernels place on the model's geometry; a
+    vsb_model_set_hidden_embedder / _extractor, vsb_model_set_vit_extractor and vsb_model_set_pixel_decoder check every rule the kernels place on the model's geometry; a
     model they do not implement raises NotImplementedError."""
     L = _lib.lib()
+    if "hidden_encoder" not in spec and not spec["unet"]["z"]:
+        # the descriptor of a U-Net without levels looks like one a HiDDeN embedder completes: reject it here, at load
+        raise RuntimeError("libvsb200 error -1: unet levels: a U-Net needs 2 to 6 levels (z_channels_mults is empty)")
     h = C.c_void_p()
     _lib.check(L.vsb_model_create(C.byref(native_desc(spec)), C.byref(h)))
     pd = spec.get("pixel_decoder", {"pixelwise": False})
     f = pd["upscale_stages"] if pd["pixelwise"] else None
-    rc = L.vsb_model_set_unet_temporal(h, 1) if spec["unet"].get("temporal", False) else 0
+    rc = L.vsb_model_set_unet_temporal(h, 1) if spec.get("unet", {}).get("temporal", False) else 0
+    if rc == 0 and "hidden_encoder" in spec:
+        rc = L.vsb_model_set_hidden_embedder(h, C.byref(native_hidden_desc(spec["hidden_encoder"], True)))
+    if rc == 0 and "hidden_decoder" in spec:
+        rc = L.vsb_model_set_hidden_extractor(h, C.byref(native_hidden_desc(spec["hidden_decoder"], False)))
     if rc == 0 and "vit" in spec:
         rc = L.vsb_model_set_vit_extractor(h, C.byref(native_vit_desc(spec["vit"])))
     if rc == 0 and f:
@@ -161,9 +191,9 @@ class _Embedder:
         m = self._owner
         if bool(v) != bool(m.spec["yuv"]):
             want = 1 if v else 3
-            if m.spec["unet"]["in_channels"] != want:
-                raise ValueError(f"embedder.yuv={bool(v)} needs a U-Net with {want} input channel(s); this checkpoint has "
-                                 f"{m.spec['unet']['in_channels']}")
+            if embedder_in_channels(m.spec) != want:
+                raise ValueError(f"embedder.yuv={bool(v)} needs an embedder with {want} input channel(s); this checkpoint has "
+                                 f"{embedder_in_channels(m.spec)}")
             m._respec(yuv=bool(v))
 
     def get_random_msg(self, bsz: int = 1, nb_repetitions: int = 1) -> torch.Tensor:
@@ -180,7 +210,7 @@ class _Embedder:
         S = m.spec["img_size"]
         assert x.shape[1:] == (3, S, S), "embedder seam takes RGB frames at processing size (Y extraction is fused)"
         mm = m._msgs_u8(msgs)
-        out = torch.empty((x.shape[0], m.spec["unet"]["out_channels"], S, S), device=x.device, dtype=torch.float32)
+        out = torch.empty((x.shape[0], delta_channels(m.spec), S, S), device=x.device, dtype=torch.float32)
         _lib.check(_lib.lib().vsb_embedder_forward(m._handle(), x.data_ptr(), mm.data_ptr(), mm.shape[0], out.data_ptr(),
                                                    x.shape[0], m._stream()))
         return out
@@ -362,7 +392,7 @@ class Videoseal(nn.Module):
         imgs_w = torch.empty_like(x)
         preds_w = None
         if not is_video:
-            pc = self.spec["unet"]["out_channels"]
+            pc = delta_channels(self.spec)
             if self.attenuation is not None:       # hmaps * preds_w broadcasts to max(out_channels) channels (wam.py:189-193)
                 pc = max(pc, self.attenuation.out_channels)
             preds_w = torch.empty((F_, pc, H, W), device=x.device, dtype=torch.float32)
@@ -378,7 +408,7 @@ class Videoseal(nn.Module):
     @property
     def temporal(self) -> bool:
         """True for a temporal U-Net (unet.conv_layer 'conv3d'): its 3x3x3 convs mix the key frames of one embedder call"""
-        return bool(self.spec["unet"].get("temporal", False))
+        return bool(self.spec.get("unet", {}).get("temporal", False))
 
     def _chunk_keys(self, is_video: bool, num_frames: int) -> int:
         """vsb_embed's chunk_keys: key frames per reference embedder call.  A video call is one chunk of chunk_size key frames
