@@ -1071,16 +1071,22 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 //
 //   warpgroup 0    : producer; gives its registers away (setmaxnreg) and one elected thread runs the TMA loop: per K block of 64
 //                    a [256 x 64] A tile (one box: tile_h x tile_w = 256 pixels of the map, or 256 GEMM rows) and a [BN x 64] B tile
+//                    (of the tile's sample with per-sample weights)
 //   warpgroups 1,2 : consumers; warpgroup h owns rows [128h, 128h + 128) of the tile as two m64 wgmma chains that read the same B
-//                    tile, 2 x BN / 2 accumulators per thread, and runs the epilogue of its rows straight from the fragments:
-//                    acc + bias -> ReLU -> + fp16 residual -> clamp -> fp16, staged per warp in swizzled [16 rows] boxes that leave
-//                    through TMA stores
+//                    tile, 2 x BN / 2 accumulators per thread, and runs the epilogue of its rows straight from the fragments.  Chain c
+//                    reads the 8-row groups 2g + c (g = 0..7) of the warpgroup's rows (descriptor group stride 2048 B), so warp wq
+//                    holds the 32 consecutive rows [32 wq, 32 wq + 32): fragment half hh of chain c is row 32 wq + 8c + 16hh + lane / 4.
+//   epilogues      : F32 = false, ACT ReLU / none: acc + bias -> ReLU -> + fp16 residual -> clamp -> fp16
+//                    F32 = false, ACT GELU:        acc + bias -> GELU -> fp16, and the column sums of squares of every 32 rows (GRN
+//                                                  partial rows, [M / 32][N])
+//                    F32 = true (ACT none):        fp32 stream += acc + bias in place (pwconv2), optional fp16 copy
+//                    fp16 outputs are staged per warp in swizzled [8 rows] boxes that leave through TMA stores.
 //
 // Against the 128-row kernel a K block moves 48 KB instead of 2 x 32 KB from L2 for the same 4.2 MFLOP, a pipeline stage is worth
 // twice the MMA time, and no accumulator crosses shared memory.  The price: a warpgroup's epilogue does not overlap its own next
-// main loop (the producer keeps filling the ring meanwhile), so finalize_op selects this kernel for long main loops only.  The
-// K-block order, the k16 order inside a block and the epilogue arithmetic are those of conv_gemm_kernel's lean affine path: both
-// kernels produce the same bits.
+// main loop (the producer keeps filling the ring meanwhile).  The K-block order, the k16 order inside a block, the epilogue
+// arithmetic and the order of the GRN row sums (32 rows paired by row bit 4, 3, 2, 1, 0) are those of conv_gemm_kernel's lean
+// paths: both kernels produce the same bits.
 constexpr int kLongM = 256;
 constexpr int kLongThreads = 384;
 constexpr int kLongHeaderBytes = 1024;                // full / empty barriers
@@ -1099,10 +1105,11 @@ __device__ __forceinline__ float2 ld_nc_f32x2(const float* g) {
   return v;
 }
 
-template <int BN, int ACT>
+template <int BN, int ACT, bool F32 = false>
 __global__ void __launch_bounds__(kLongThreads, 1)
 conv_gemm_longk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                        const __grid_constant__ CUtensorMap tmO, const __grid_constant__ ConvGemmParams p) {
+  static_assert(!F32 || ACT == ACT_NONE, "the fp32 residual-stream epilogue has no activation");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem);
@@ -1119,7 +1126,7 @@ conv_gemm_longk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     fence_barrier_init();
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    tma_prefetch_desc(&tmO);
+    if (!F32) tma_prefetch_desc(&tmO);
   }
   __syncthreads();
   // nothing above reads or writes a tensor produced by an earlier kernel
@@ -1133,7 +1140,8 @@ conv_gemm_longk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        const int m_tile = p.fd_ntiles.div(tile), brow = (tile - m_tile * p.n_tiles) * BN;
+        const int m_tile = p.fd_ntiles.div(tile);
+        const int brow = (tile - m_tile * p.n_tiles) * BN + (p.b_sample_rows ? p.fd_tps.div(m_tile) * p.b_sample_rows : 0);
         int cb = 0, cx = 0, cy = 0;
         if (p.a_is_conv) {
           cb = p.fd_tpi.div(m_tile);
@@ -1163,19 +1171,24 @@ conv_gemm_longk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     setmaxnreg_inc<232>();
     const int h = (warp >> 2) - 1, wq = warp & 3;
     const int rl = lane >> 2, q = lane & 3;
-    // staging boxes of this warp: [16 rows][kBoxCols] fp16 in the TMA swizzle of that row width; fragment row rl and rl + 8 share
-    // the XOR term, and the 4-byte stores of a warp instruction (8 rows x 4 lanes) fall into 32 different banks
+    // staging boxes of this warp: [BN / kBoxCols][2 halves] boxes of [8 rows][kBoxCols] fp16 in the TMA swizzle of that row width;
+    // the 4-byte stores of a warp instruction (8 rows x 4 lanes) fall into 32 different banks
     constexpr int kBoxCols = BN % 64 == 0 ? 64 : 16;
-    constexpr uint32_t kBoxRowB = kBoxCols * 2, kBoxBytes = 16 * kBoxRowB;
+    constexpr uint32_t kBoxRowB = kBoxCols * 2, kBoxBytes = 8 * kBoxRowB;
     const uint32_t swz_x = kBoxCols == 64 ? (uint32_t)rl : (uint32_t)((rl >> 2) & 1);
     uint8_t* ost = smem + p.ostage_off + (size_t)(warp - 4) * kLongOstWarpBytes;
-    const bool has_res = p.resid16 != nullptr;
+    auto box_ptr = [&](int j /*8-column group*/, int hh) -> uint8_t* {
+      return ost + (uint32_t)(((8 * j) / kBoxCols) * 2 + hh) * kBoxBytes + (uint32_t)rl * kBoxRowB +
+             (((uint32_t)(((8 * j) % kBoxCols) >> 3) ^ swz_x) << 4) + 4u * q;
+    };
+    const bool has_res = !F32 && p.resid16 != nullptr;
     constexpr uint32_t kRowBytes = 128;                           // K block of 64 fp16
     const uint32_t a_off = (uint32_t)h * 128u * kRowBytes;
     float d[2][BN / 2];
-    // The epilogue walks the 2 x BN / 8 eight-column groups of the two chains in kGrp-sized steps; the bias pairs and residual
-    // half2 of step t + 1 are loaded while step t is converted.  Only two steps' worth sit in registers beside the 2 x BN / 2
-    // accumulators (the whole tile's would not fit), and the loads are ordered statements so that they stay where they are put.
+    // The fp16 affine epilogue walks the 2 x BN / 8 eight-column groups of the two chains in kGrp-sized steps; the bias pairs and
+    // residual half2 of step t + 1 are loaded while step t is converted.  Only two steps' worth sit in registers beside the
+    // 2 x BN / 2 accumulators (the whole tile's would not fit), and the loads are ordered statements so that they stay where they
+    // are put.
     constexpr int kGrp = BN % 32 == 0 ? 4 : 5, kSteps = BN / 8 / kGrp;     // steps per chain
     static_assert(kGrp * kSteps * 8 == BN, "block_n must split into whole epilogue steps");
     float2 gb0[kGrp], gb1[kGrp];
@@ -1184,13 +1197,13 @@ conv_gemm_longk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
       const int m_tile = p.fd_ntiles.div(tile), n0 = (tile - m_tile * p.n_tiles) * BN;
-      const long m_warp = (long)m_tile * kLongM + h * 128 + wq * 16;     // first row of this warp's chain-0 fragment
+      const long m_warp = (long)m_tile * kLongM + h * 128 + wq * 32;     // first of this warp's 32 rows
       int prev = -1;
       for (int kb = 0; kb < p.num_kb; ++kb) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t sa = smem_u32(tiles + (size_t)stage * p.stage_bytes);
-        const uint64_t adesc0 = make_smem_desc(sa + a_off, kRowBytes);
-        const uint64_t adesc1 = make_smem_desc(sa + a_off + 64u * kRowBytes, kRowBytes);
+        const uint64_t adesc0 = make_smem_desc(sa + a_off, kRowBytes, 16 * kRowBytes);
+        const uint64_t adesc1 = make_smem_desc(sa + a_off + 8u * kRowBytes, kRowBytes, 16 * kRowBytes);
         const uint64_t bdesc = make_smem_desc(sa + p.a_stage_bytes, kRowBytes);
         wgmma_fence_regs(d[0]);
         wgmma_fence_regs(d[1]);
@@ -1212,67 +1225,185 @@ conv_gemm_longk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
         prev = stage;
         if (++stage == p.stages) { stage = 0; phase ^= 1u; }
       }
-      auto load_step = [&](float2 (&gb)[kGrp], uint32_t (&gr)[2 * kGrp], int t) {
-        const int c = t / kSteps, j0 = (t % kSteps) * kGrp;
-        const __half* r0 = p.resid16 + (m_warp + 64 * c + rl) * p.ld_res16 + n0 + 8 * j0 + 2 * q;
-        const __half* r1 = r0 + 8 * (long)p.ld_res16;
+      // TMA stores of chain c's staging boxes
+      auto store_chain = [&](int c) {
+        fence_proxy_async_smem();     // generic-proxy writes of the staging boxes -> async proxy
+        __syncwarp();
+        if (lane == 0) {
 #pragma unroll
-        for (int jj = 0; jj < kGrp; ++jj) {
-          gb[jj] = p.bias != nullptr ? ld_nc_f32x2(p.bias + n0 + 8 * (j0 + jj) + 2 * q) : make_float2(0.f, 0.f);
-          if (has_res) {
-            gr[2 * jj] = ld_nc_u32(r0 + 8 * jj);
-            gr[2 * jj + 1] = ld_nc_u32(r1 + 8 * jj);
-          }
+          for (int b = 0; b < BN / kBoxCols; ++b)
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh)
+              tma_store_2d(&tmO, ost + (2 * b + hh) * kBoxBytes, n0 + b * kBoxCols, (int)(m_warp + 8 * c + 16 * hh));
+          bulk_commit_group();
         }
       };
-      load_step(gb0, gr0, 0);       // in flight while the last wgmma group drains
-      wgmma_wait<0>();
-      wgmma_fence_regs(d[0]);
-      wgmma_fence_regs(d[1]);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      if (F32) {
+        // pwconv2: the fp32 residual stream, read and written in place by the same thread, += acc + bias (+ fp16 copy).  Row t =
+        // (chain t / 2, half t % 2) of the thread: its residual is loaded while the last wgmma group drains (t = 0) or, below
+        // block_n 128 (where a second row buffer fits in registers), while row t - 1 is written.
+        constexpr bool kPipe = BN < 128;
+        float2 ra[BN / 8], rb[kPipe ? BN / 8 : 1];
+        auto load_row = [&](float2 (&r)[BN / 8], int t) {
+          const float* rr = p.resid32 + (m_warp + 8 * (t >> 1) + 16 * (t & 1) + rl) * p.ld_res32 + n0 + 2 * q;
 #pragma unroll
-      for (int t = 0; t < 2 * kSteps; ++t) {
-        const int c = t / kSteps, g = t % kSteps;
-        if (g == 0) {
+          for (int j = 0; j < BN / 8; ++j) r[j] = *reinterpret_cast<const float2*>(rr + 8 * j);
+        };
+        auto store_row = [&](const float2 (&r)[BN / 8], int t) {
+          const int c = t >> 1, hh = t & 1;
+          const long row = m_warp + 8 * c + 16 * hh + rl;
+          float* o = p.out32 + row * p.ld_out32 + n0 + 2 * q;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const float2 b = p.bias != nullptr ? ld_nc_f32x2(p.bias + n0 + 8 * j + 2 * q) : make_float2(0.f, 0.f);
+            const float v0 = d[c][4 * j + 2 * hh] + (b.x + r[j].x), v1 = d[c][4 * j + 2 * hh + 1] + (b.y + r[j].y);
+            *reinterpret_cast<float2*>(o + 8 * j) = make_float2(v0, v1);
+            if (p.out16 != nullptr)
+              *reinterpret_cast<__half2*>(p.out16 + row * p.ld_out16 + n0 + 8 * j + 2 * q) =
+                  __floats2half2_rn(fminf(fmaxf(v0, -65504.f), 65504.f), fminf(fmaxf(v1, -65504.f), 65504.f));
+          }
+        };
+        load_row(ra, 0);
+        wgmma_wait<0>();
+        wgmma_fence_regs(d[0]);
+        wgmma_fence_regs(d[1]);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        if constexpr (kPipe) {
+          load_row(rb, 1);
+          store_row(ra, 0);
+          load_row(ra, 2);
+          store_row(rb, 1);
+          load_row(rb, 3);
+          store_row(ra, 2);
+          store_row(rb, 3);
+        } else {
+#pragma unroll
+          for (int t = 0; t < 4; ++t) {
+            if (t > 0) load_row(ra, t);
+            store_row(ra, t);
+          }
+        }
+      } else if (ACT == ACT_GELU) {
+        // pwconv1: bias + GELU + fp16 store, then the GRN column sums of squares of the warp's 32 rows
+        wgmma_wait<0>();
+        wgmma_fence_regs(d[0]);
+        wgmma_fence_regs(d[1]);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
           if (lane == 0) bulk_wait_group_read0();     // the previous stores of this warp have finished reading the staging boxes
           __syncwarp();
-        }
-        auto convert_step = [&](const float2 (&gb)[kGrp], const uint32_t (&gr)[2 * kGrp]) {
 #pragma unroll
-          for (int jj = 0; jj < kGrp; ++jj) {
-            const int j = g * kGrp + jj;
-            uint8_t* obox = ost + (uint32_t)((8 * j) / kBoxCols) * kBoxBytes + ((((uint32_t)((8 * j) % kBoxCols) >> 3) ^ swz_x) << 4) + 4u * q;
+          for (int j = 0; j < BN / 8; ++j) {
+            const float2 b = p.bias != nullptr ? ld_nc_f32x2(p.bias + n0 + 8 * j + 2 * q) : make_float2(0.f, 0.f);
 #pragma unroll
             for (int hh = 0; hh < 2; ++hh) {
-              float v0 = d[c][4 * j + 2 * hh] + gb[jj].x, v1 = d[c][4 * j + 2 * hh + 1] + gb[jj].y;
-              if (ACT == ACT_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-              if (has_res) {
-                const uint32_t rbits = gr[2 * jj + hh];
-                const float2 rf = __half22float2(*reinterpret_cast<const __half2*>(&rbits));
-                v0 += rf.x; v1 += rf.y;
-              }
-              v0 = fminf(v0, 65504.f); v1 = fminf(v1, 65504.f);
-              if (ACT == ACT_NONE || has_res) { v0 = fmaxf(v0, -65504.f); v1 = fmaxf(v1, -65504.f); }   // ReLU >= 0
-              *reinterpret_cast<__half2*>(obox + (uint32_t)(rl + 8 * hh) * kBoxRowB) = __floats2half2_rn(v0, v1);
+              const float2 w = gelu_erf_p(f2add(make_float2(d[c][4 * j + 2 * hh], d[c][4 * j + 2 * hh + 1]), b));
+              d[c][4 * j + 2 * hh] = w.x; d[c][4 * j + 2 * hh + 1] = w.y;
+              uint32_t hv;
+              asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(hv) : "f"(w.y), "f"(w.x));   // {hi, lo}
+              *reinterpret_cast<uint32_t*>(box_ptr(j, hh)) = hv;
+            }
+          }
+          store_chain(c);
+        }
+        if (p.grn_stats != nullptr) {
+          // row x of the 32 is (c, hh, rl) = (bit 3, bit 4, bits 0-2): pair rows x, x + 16 (hh), then x, x + 8 (c) in the thread,
+          // then rows 4, 2, 1 apart across lanes 16, 8, 4 apart (halving butterfly).  Column of value i: 8 (i / 2) + 2q + i % 2.
+          constexpr int kV = BN / 4;
+          float s[kV];
+#pragma unroll
+          for (int i = 0; i < kV; ++i) {
+            const int k = 4 * (i >> 1) + (i & 1);
+            const float t0 = __fmul_rn(d[0][k], d[0][k]) + __fmul_rn(d[0][k + 2], d[0][k + 2]);
+            const float t1 = __fmul_rn(d[1][k], d[1][k]) + __fmul_rn(d[1][k + 2], d[1][k + 2]);
+            s[i] = t0 + t1;
+          }
+          int base = 0;
+#pragma unroll
+          for (int i = 0; i < kV / 2; ++i) {
+            const float send = (lane & 16) ? s[i] : s[i + kV / 2];
+            const float keep = (lane & 16) ? s[i + kV / 2] : s[i];
+            s[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
+          }
+          if (lane & 16) base += kV / 2;
+#pragma unroll
+          for (int i = 0; i < kV / 4; ++i) {
+            const float send = (lane & 8) ? s[i] : s[i + kV / 4];
+            const float keep = (lane & 8) ? s[i + kV / 4] : s[i];
+            s[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
+          }
+          if (lane & 8) base += kV / 4;
+#pragma unroll
+          for (int i = 0; i < kV / 8; ++i) {
+            const float send = (lane & 4) ? s[i] : s[i + kV / 8];
+            const float keep = (lane & 4) ? s[i + kV / 8] : s[i];
+            s[i] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
+          }
+          if (lane & 4) base += kV / 8;
+          float* grow = p.grn_stats + (m_warp >> 5) * p.N + n0 + 2 * q;
+#pragma unroll
+          for (int i = 0; i < kV / 8; ++i) {
+            const int v = base + i;
+            grow[8 * (v >> 1) + (v & 1)] = s[i];
+          }
+        }
+      } else {
+        auto load_step = [&](float2 (&gb)[kGrp], uint32_t (&gr)[2 * kGrp], int t) {
+          const int c = t / kSteps, j0 = (t % kSteps) * kGrp;
+          const __half* r0 = p.resid16 + (m_warp + 8 * c + rl) * p.ld_res16 + n0 + 8 * j0 + 2 * q;
+          const __half* r1 = r0 + 16 * (long)p.ld_res16;
+#pragma unroll
+          for (int jj = 0; jj < kGrp; ++jj) {
+            gb[jj] = p.bias != nullptr ? ld_nc_f32x2(p.bias + n0 + 8 * (j0 + jj) + 2 * q) : make_float2(0.f, 0.f);
+            if (has_res) {
+              gr[2 * jj] = ld_nc_u32(r0 + 8 * jj);
+              gr[2 * jj + 1] = ld_nc_u32(r1 + 8 * jj);
             }
           }
         };
-        if ((t & 1) == 0) {
-          if (t + 1 < 2 * kSteps) load_step(gb1, gr1, t + 1);
-          convert_step(gb0, gr0);
-        } else {
-          if (t + 1 < 2 * kSteps) load_step(gb0, gr0, t + 1);
-          convert_step(gb1, gr1);
-        }
-        if (g == kSteps - 1) {
-          fence_proxy_async_smem();     // generic-proxy writes of the staging boxes -> async proxy
-          __syncwarp();
-          if (lane == 0) {
+        load_step(gb0, gr0, 0);       // in flight while the last wgmma group drains
+        wgmma_wait<0>();
+        wgmma_fence_regs(d[0]);
+        wgmma_fence_regs(d[1]);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
 #pragma unroll
-            for (int b = 0; b < BN / kBoxCols; ++b) tma_store_2d(&tmO, ost + b * kBoxBytes, n0 + b * kBoxCols, (int)(m_warp + 64 * c));
-            bulk_commit_group();
+        for (int t = 0; t < 2 * kSteps; ++t) {
+          const int c = t / kSteps, g = t % kSteps;
+          if (g == 0) {
+            if (lane == 0) bulk_wait_group_read0();     // the previous stores of this warp have finished reading the staging boxes
+            __syncwarp();
           }
+          auto convert_step = [&](const float2 (&gb)[kGrp], const uint32_t (&gr)[2 * kGrp]) {
+#pragma unroll
+            for (int jj = 0; jj < kGrp; ++jj) {
+              const int j = g * kGrp + jj;
+#pragma unroll
+              for (int hh = 0; hh < 2; ++hh) {
+                float v0 = d[c][4 * j + 2 * hh] + gb[jj].x, v1 = d[c][4 * j + 2 * hh + 1] + gb[jj].y;
+                if (ACT == ACT_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                if (has_res) {
+                  const uint32_t rbits = gr[2 * jj + hh];
+                  const float2 rf = __half22float2(*reinterpret_cast<const __half2*>(&rbits));
+                  v0 += rf.x; v1 += rf.y;
+                }
+                v0 = fminf(v0, 65504.f); v1 = fminf(v1, 65504.f);
+                if (ACT == ACT_NONE || has_res) { v0 = fmaxf(v0, -65504.f); v1 = fmaxf(v1, -65504.f); }   // ReLU >= 0
+                *reinterpret_cast<__half2*>(box_ptr(j, hh)) = __floats2half2_rn(v0, v1);
+              }
+            }
+          };
+          if ((t & 1) == 0) {
+            if (t + 1 < 2 * kSteps) load_step(gb1, gr1, t + 1);
+            convert_step(gb0, gr0);
+          } else {
+            if (t + 1 < 2 * kSteps) load_step(gb0, gr0, t + 1);
+            convert_step(gb1, gr1);
+          }
+          if (g == kSteps - 1) store_chain(c);
         }
       }
     }

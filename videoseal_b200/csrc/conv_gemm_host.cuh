@@ -144,23 +144,47 @@ inline bool longk_conv_tile(int H, int W, int& tile_w, int& tile_h) {
   return tile_w * tile_h == kLongM && W % tile_w == 0 && H % tile_h == 0;
 }
 
-// Everything but the tile count: a TMA-fed op with a long main loop whose epilogue is the lean affine one (bias, ReLU or none,
-// optional fp16 residual, fp16 output), in whole 256 x block_n tiles of a width the kernel is instantiated for.
-inline bool longk_eligible(const ConvGemmOp& op, int N) {
+// The output-tile width the long-K kernel would run this op at, or 0 when it cannot run it.  Everything but the tile count: a
+// TMA-fed op with 64-wide K blocks in whole 256-row tiles, and one of the kernel's epilogues at a width it is instantiated for:
+//   - the lean affine one (bias, ReLU or none, optional fp16 residual, fp16 output) on long main loops, at the 128-row kernel's
+//     block_n (128 or 80);
+//   - ConvNeXt pwconv1: bias + GELU, fp16 output, GRN statistics as per-32-row partial rows, block_n 128 (the float-atomic GRN
+//     mode and GELU GEMMs without GRN, the ViT MLP, stay on the 128-row kernel: not measured on this one);
+//   - ConvNeXt pwconv2: no activation, fp32 residual stream updated in place, optional fp16 copy, per-sample weights whose samples
+//     are whole 256-row tiles, block_n 128 or 96.
+inline int longk_block_n(const ConvGemmOp& op, int N, int block_n_override) {
   const ConvGemmParams& p = op.p;
   int tw, th;
-  return op.loader == LD_TMA && op.a_rank != 0 && op.w_samples == 1 && p.kblk == 64 && p.num_kb >= 24 &&
-         p.epi == EPI_AFFINE && (p.act == ACT_NONE || p.act == ACT_RELU) &&
-         p.out16 != nullptr && p.out32 == nullptr && p.resid32 == nullptr && p.outc_w == nullptr && p.grn_stats == nullptr &&
-         (reinterpret_cast<uintptr_t>(p.out16) & 15) == 0 && p.ld_out16 % 8 == 0 && (reinterpret_cast<uintptr_t>(p.bias) & 7) == 0 &&
-         (p.resid16 == nullptr || ((reinterpret_cast<uintptr_t>(p.resid16) & 3) == 0 && p.ld_res16 % 8 == 0)) &&
-         (p.block_n == 128 || p.block_n == 80) && N % p.block_n == 0 && p.M % kLongM == 0 &&
-         (!p.a_is_conv || longk_conv_tile(p.H, p.W, tw, th));
+  if (!(op.loader == LD_TMA && op.a_rank != 0 && p.kblk == 64 && p.num_kb >= 2 && p.epi == EPI_AFFINE && p.outc_w == nullptr &&
+        p.M % kLongM == 0 && (reinterpret_cast<uintptr_t>(p.bias) & 7) == 0 && (!p.a_is_conv || longk_conv_tile(p.H, p.W, tw, th))))
+    return 0;
+  const bool out16_ok = p.out16 != nullptr && (reinterpret_cast<uintptr_t>(p.out16) & 15) == 0 && p.ld_out16 % 8 == 0;
+  int bn = 0;
+  if (p.act == ACT_GELU) {
+    if (out16_ok && p.out32 == nullptr && p.resid16 == nullptr && p.resid32 == nullptr && op.w_samples == 1 &&
+        p.grn_stats != nullptr && p.grn_part && p.rows_per_sample > 0 && p.rows_per_sample % 32 == 0)
+      bn = 128;
+  } else if (p.resid32 != nullptr) {
+    if (p.act == ACT_NONE && p.out32 != nullptr && p.resid16 == nullptr && p.grn_stats == nullptr &&
+        (reinterpret_cast<uintptr_t>(p.out32) & 7) == 0 && p.ld_out32 % 2 == 0 &&
+        (reinterpret_cast<uintptr_t>(p.resid32) & 7) == 0 && p.ld_res32 % 2 == 0 &&
+        (p.out16 == nullptr || ((reinterpret_cast<uintptr_t>(p.out16) & 3) == 0 && p.ld_out16 % 2 == 0)) &&
+        (op.w_samples == 1 || (!p.a_is_conv && p.rows_per_sample > 0 && p.rows_per_sample % kLongM == 0)))
+      bn = N % 128 == 0 ? 128 : (N % 96 == 0 ? 96 : 0);
+  } else if (p.num_kb >= 24 && (p.act == ACT_NONE || p.act == ACT_RELU) && out16_ok && p.out32 == nullptr && p.grn_stats == nullptr &&
+             op.w_samples == 1 && (p.resid16 == nullptr || ((reinterpret_cast<uintptr_t>(p.resid16) & 3) == 0 && p.ld_res16 % 8 == 0)) &&
+             (p.block_n == 128 || p.block_n == 80)) {
+    bn = p.block_n;
+  }
+  if (bn == 0 || N % bn != 0 || (block_n_override != 0 && block_n_override != bn)) return 0;
+  return bn;
 }
 
-inline void finalize_longk(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw, int num_sms) {
+inline void finalize_longk(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw, int num_sms, int block_n) {
   ConvGemmParams& p = op.p;
   op.longk = 1;
+  p.block_n = block_n;
+  p.n_tiles = N / block_n;
   p.group = 1;
   p.m_tiles = p.M / kLongM;
   p.num_tiles = p.m_tiles * p.n_tiles;
@@ -173,25 +197,32 @@ inline void finalize_longk(ConvGemmOp& op, const __half* W, int N, int Kw, int l
   }
   encode_map(&op.tmA, op.a_base, op.a_rank, op.a_dims, op.a_strides, abox, 64);
   p.fd_ntiles = make_fastdiv(p.n_tiles); p.fd_tpi = make_fastdiv(p.tiles_per_img); p.fd_tx = make_fastdiv(p.tiles_x);
+  p.b_sample_rows = 0;
+  if (op.w_samples > 1) {   // weights [w_samples][N][K]; every 256-row tile lies inside one sample (longk_block_n)
+    p.b_sample_rows = N;
+    p.fd_tps = make_fastdiv(p.rows_per_sample / kLongM);
+  }
   p.a_stage_bytes = (uint32_t)(kLongM * 64 * 2);
   p.b_stage_bytes = (uint32_t)(p.block_n * 64 * 2);
   p.stage_bytes = p.a_stage_bytes + ((p.b_stage_bytes + 1023u) & ~1023u);
-  // shared memory: [barriers | stages x (A|B) | staging boxes of the 8 consumer warps]; 4 stages of 48 KB at block_n 128
-  const size_t ostage_total = (size_t)kLongConsumerWarps * kLongOstWarpBytes;
+  // shared memory: [barriers | stages x (A|B) | staging boxes of the 8 consumer warps (fp16 outputs)]; 4 stages of 48 KB at
+  // block_n 128.  The fp32 residual-stream epilogue stores from registers and spends the staging bytes on a pipeline stage.
+  const bool staged = p.resid32 == nullptr;
+  const size_t ostage_total = staged ? (size_t)kLongConsumerWarps * kLongOstWarpBytes : 0;
   int stages = (int)((226 * 1024 - kLongHeaderBytes - ostage_total) / p.stage_bytes);
   if (stages > kMaxStages) stages = kMaxStages;
   VSB_CHECK(stages >= 3, "long-K tile does not fit in shared memory");
   p.stages = stages;
   p.ostage_off = (uint32_t)(kLongHeaderBytes + (size_t)stages * p.stage_bytes);
   op.smem = 1024 /*align slack*/ + p.ostage_off + ostage_total;
-  {  // output map [M rows][N cols]; box = one staging box: 16 fragment rows x 64 columns (128-byte swizzle) or x 16 (32-byte swizzle)
+  if (staged) {  // output map [M rows][N cols]; box = one staging box: 8 fragment rows x 64 columns (128-byte swizzle) or x 16 (32-byte)
     const int box_cols = p.block_n % 64 == 0 ? 64 : 16;
     uint64_t odims[2] = {(uint64_t)N, (uint64_t)p.M};
     uint64_t ostrides[1] = {(uint64_t)p.ld_out16 * 2};
-    uint32_t obox[2] = {(uint32_t)box_cols, 16u};
+    uint32_t obox[2] = {(uint32_t)box_cols, 8u};
     encode_map(&op.tmO, p.out16, 2, odims, ostrides, obox, 0, /*no_swizzle=*/true, false, box_cols * 2);
   }
-  uint64_t dims[2] = {(uint64_t)Kw, (uint64_t)N};
+  uint64_t dims[2] = {(uint64_t)Kw, (uint64_t)N * (uint64_t)op.w_samples};
   uint64_t strides[1] = {(uint64_t)ldw * 2};
   uint32_t box[2] = {64u, (uint32_t)p.block_n};
   encode_map(&op.tmB, W, 2, dims, strides, box, 64);
@@ -214,11 +245,17 @@ inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw,
   {
     // Long main loops run on 256-row tiles when there are at least two of them per SM.  Below that the 128-row kernel fills the
     // machine better: it has twice the tiles to spread, and the last wave of 256-row tiles would leave SMs idle for a whole
-    // 256-row main loop.  (Not measured below the threshold; the bottleneck convs at 64 frames have 5.8 tiles per SM.)
-    const bool eligible = longk_eligible(op, N);
-    VSB_CHECK(kernel_sel != kKernelLongK || eligible, "the long-K kernel cannot run this op");
-    if (eligible && kernel_sel != kKernel128 && (kernel_sel == kKernelLongK || (long)(p.M / kLongM) * p.n_tiles >= 2L * num_sms)) {
-      finalize_longk(op, W, N, Kw, ldw, num_sms);
+    // 256-row main loop.  (Not measured below the threshold; the bottleneck convs at 64 frames have 5.8 tiles per SM, the
+    // ConvNeXt pwconv1s and stage 1's pwconv2 at 64 frames 2.9 or more.)
+    const int lbn = longk_block_n(op, N, block_n_override);
+    VSB_CHECK(kernel_sel != kKernelLongK || lbn != 0, "the long-K kernel cannot run this op");
+    // The fp32 residual-stream epilogue also needs 12 K blocks: below that the tile's 8 bytes of stream traffic per output outlast
+    // its main loop, and the 128-row kernel, which overlaps the two, is faster (videoseal_1.0 stage 0's pwconv2, K = 384: 188
+    // against 196 us on an H100 SXM at 700 W).
+    const long ltiles = (long)(p.M / kLongM) * (lbn ? N / lbn : 0);
+    const bool long_enough = p.resid32 == nullptr || p.num_kb >= 12;
+    if (lbn != 0 && kernel_sel != kKernel128 && (kernel_sel == kKernelLongK || (ltiles >= 2L * num_sms && long_enough))) {
+      finalize_longk(op, W, N, Kw, ldw, num_sms, lbn);
       return;
     }
   }
@@ -518,17 +555,20 @@ inline void launch_one(const ConvGemmOp& op, cudaStream_t st) {
   launch_pdl(conv_gemm_kernel<LOADER, ACT>, dim3(op.grid), dim3(op.threads), op.smem, st, op.tmA, op.tmA2, op.tmB, op.tmO, op.p);
 }
 
-template <int BN, int ACT>
+template <int BN, int ACT, bool F32 = false>
 inline void launch_longk(const ConvGemmOp& op, cudaStream_t st) {
-  smem_optin<conv_gemm_longk_kernel<BN, ACT>>(227 * 1024);
-  launch_pdl(conv_gemm_longk_kernel<BN, ACT>, dim3(op.grid), dim3(op.threads), op.smem, st, op.tmA, op.tmB, op.tmO, op.p);
+  smem_optin<conv_gemm_longk_kernel<BN, ACT, F32>>(227 * 1024);
+  launch_pdl(conv_gemm_longk_kernel<BN, ACT, F32>, dim3(op.grid), dim3(op.threads), op.smem, st, op.tmA, op.tmB, op.tmO, op.p);
 }
 
 // instantiated (loader, activation) pairs: only what the networks need, to bound compile time
 inline void launch(const ConvGemmOp& op, cudaStream_t st) {
   const int a = op.p.act;
-  if (op.longk) {   // block_n 128 / 80 and ReLU / none: longk_eligible
-    if (op.p.block_n == 128) { if (a == ACT_RELU) launch_longk<128, ACT_RELU>(op, st); else launch_longk<128, ACT_NONE>(op, st); }
+  if (op.longk) {   // the (block_n, epilogue) pairs of longk_block_n
+    const int bn = op.p.block_n;
+    if (op.p.resid32 != nullptr) { if (bn == 128) launch_longk<128, ACT_NONE, true>(op, st); else launch_longk<96, ACT_NONE, true>(op, st); }
+    else if (a == ACT_GELU) launch_longk<128, ACT_GELU>(op, st);
+    else if (bn == 128) { if (a == ACT_RELU) launch_longk<128, ACT_RELU>(op, st); else launch_longk<128, ACT_NONE>(op, st); }
     else { if (a == ACT_RELU) launch_longk<80, ACT_RELU>(op, st); else launch_longk<80, ACT_NONE>(op, st); }
     VSB_CUDA(cudaGetLastError());
     return;

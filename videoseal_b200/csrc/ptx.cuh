@@ -219,11 +219,11 @@ template <> struct Wgmma<128> {
 
 // wgmma shared-memory matrix descriptor for a K-major operand tile whose rows are `row_bytes`
 // (= 32 / 64 / 128) wide and stored with the matching 32B/64B/128B swizzle; 8-row groups are
-// 8*row_bytes apart (SBO).  Bits: [0,14) addr>>4, [16,30) LBO>>4, [32,46) SBO>>4,
-// [62,64) layout type (1 = SW128, 2 = SW64, 3 = SW32).
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t row_bytes) {
+// group_bytes apart (SBO; 0: 8*row_bytes, the dense tile).  Bits: [0,14) addr>>4, [16,30) LBO>>4,
+// [32,46) SBO>>4, [62,64) layout type (1 = SW128, 2 = SW64, 3 = SW32).
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t row_bytes, uint32_t group_bytes = 0) {
   uint64_t layout = row_bytes == 128 ? 1ull : (row_bytes == 64 ? 2ull : 3ull);
-  uint64_t sbo = (8ull * row_bytes) >> 4;
+  uint64_t sbo = (group_bytes ? (uint64_t)group_bytes : 8ull * row_bytes) >> 4;
   return (uint64_t)((saddr & 0x3FFFF) >> 4) | (1ull << 16) | (sbo << 32) | (layout << 62);
 }
 

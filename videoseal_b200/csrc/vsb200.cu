@@ -330,8 +330,11 @@ int vsb_debug_conv(const vsb_conv_test* t, void* stream) {
   p.out32 = t->out32; p.ld_out32 = ld_out;
   p.ln_w = t->ln_w; p.ln_b = t->ln_b; p.ln_eps = 1e-6f;
   p.outc_w = t->outc_w; p.outc_b = t->outc_b; p.n_out = t->n_out; p.delta = t->delta; p.hw = OH * OW; p.outc_tanh = 1;
-  p.grn_stats = t->grn_stats;
+  VSB_CHECK(t->grn_part == 0 || (t->grn_stats != nullptr && t->rows_per_sample > 0 && t->rows_per_sample % 32 == 0),
+            "GRN partial rows need rows_per_sample a multiple of 32");
+  p.grn_stats = t->grn_stats; p.grn_part = t->grn_part;
   if (t->rows_per_sample) p.rows_per_sample = t->rows_per_sample;
+  if (t->w_samples > 1) op.w_samples = t->w_samples;
   VSB_CHECK(t->kernel >= kKernelAuto && t->kernel <= kKernelLongK, "bad kernel selector");
   finalize_op(op, (const __half*)t->weights, t->N, K, t->ldw ? t->ldw : K, num_sms, t->block_n, t->kernel);
   if (t->kernel_ran) *t->kernel_ran = op.longk ? kKernelLongK : kKernel128;
