@@ -134,10 +134,12 @@ inline void aug_run(int op, const float* x, float* y, int B, int H, int W, int O
       break;
     }
     case VSB_AUG_RESIZE: {
-      // F.resize(size, antialias=True): the embedder's own separable resample tables and kernel (bilinear, align_corners=False)
+      // F.resize(size, antialias=True): the embedder's own separable resample tables and kernel (bilinear, align_corners=False);
+      // the profile name carries the variant, resize_sep_kernel<MT, GST>
       ResampleDev r(H, W, OH, OW, ResampleMode{});
       int32_t rec[5];
-      prof_scope("aug.resize" + tag, st, 1, [&] { launch_resize(r, x, 3 * HW, B, H, W, OH, OW, y, rec, st); });
+      const std::string variant = ".mt" + std::to_string(resize_mt(r)) + "g" + std::to_string(r.gstage);
+      prof_scope("aug.resize" + variant + tag, st, 1, [&] { launch_resize(r, x, 3 * HW, B, H, W, OH, OW, y, rec, st); });
       VSB_CUDA(cudaStreamSynchronize(st));   // the tables are freed with r
       break;
     }

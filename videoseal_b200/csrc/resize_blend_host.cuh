@@ -233,6 +233,9 @@ struct ResampleDev {
   }
 };
 
+// the MT template argument of resize_sep_kernel for this table pair: taps per output column, 2, <= 8, or any (0)
+inline int resize_mt(const ResampleDev& r) { return r.tab.maxt_x <= 2 ? 2 : (r.tab.maxt_x <= 8 ? 8 : 0); }
+
 // resample n <= 16384 frames that are `frame_stride` floats apart, H x W -> OH x OW (the table pair r); rec: MT, GST, vec, toy, OW
 inline void launch_resize(const ResampleDev& r, const float* src, long frame_stride, int n, int H, int W, int OH, int OW, float* dst,
                           int32_t rec[5], cudaStream_t st) {
@@ -240,7 +243,7 @@ inline void launch_resize(const ResampleDev& r, const float* src, long frame_str
   if (r.smem > 200 * 1024) throw Error("resize: image too wide for the shared-memory resample kernel (not implemented)", kErrUnsupported);
   const int vec = (W % 4 == 0) && (reinterpret_cast<uintptr_t>(src) % 16 == 0) && (frame_stride % 4 == 0);
   const dim3 grid((OH + r.toy - 1) / r.toy, n * 3);
-  const int mt = r.tab.maxt_x <= 2 ? 2 : (r.tab.maxt_x <= 8 ? 8 : 0);
+  const int mt = resize_mt(r);
   const int32_t rc[5] = {mt, r.gstage, vec, r.toy, OW};
   std::copy(rc, rc + 5, rec);
 #define VSB_RS(MT, GS) do { smem_optin<resize_sep_kernel<MT, GS>>(200 * 1024); \
