@@ -146,6 +146,15 @@ typedef struct vsb_hidden_desc {
  * ext_depths != 0).  Such a descriptor with no HiDDeN embedder fails at finalize with the U-Net's VSB_ERR_INVALID. */
 int vsb_model_set_hidden_embedder(vsb_model* m, const vsb_hidden_desc* h);
 int vsb_model_set_hidden_extractor(vsb_model* m, const vsb_hidden_desc* h);
+/* DVMark extractor (modules/dvmark.py DVMarkDecoder; models/extractor.py build_extractor 'dvmark'): 3x3x3 Conv3d over the frames of
+ * one detector call, 3 -> 128 (ReLU), 128 -> 128 (ReLU), avgpool (1,2,2), 128 -> 256 (ReLU), avgpool (1,2,2), 256 -> 1 + nbits, the
+ * mean over the map: pooled logits.  The frames are read in [0, 1] (no preprocess).  Checkpoint keys detector.layers.layer{1..4}.
+ * {weight,bias}, 5-D weights.  It replaces the trunk and the pixel decoder like the HiDDeN extractor: ext_* zero, no
+ * vsb_model_set_vit_extractor / vsb_model_set_hidden_extractor, no pixel-wise vsb_model_set_pixel_decoder (VSB_ERR_STATE /
+ * VSB_ERR_INVALID / VSB_ERR_UNSUPPORTED).  Called after vsb_model_create and before finalize; no CUDA call.  VSB_ERR_INVALID for
+ * nbits < 1 or nbits other than the descriptor's (any nbits >= 1 is implemented); VSB_ERR_UNSUPPORTED for an img_size that is not a
+ * positive multiple of 128.  A group of frames convolved together is at most 64 long (vsb_detect_grouped). */
+int vsb_model_set_dvmark_extractor(vsb_model* m, int32_t nbits);
 /* fold BN, pack to fp16 KRSC, upload to `device`, build nothing else (plans are built lazily per batch shape) */
 int vsb_model_finalize(vsb_model* m, int32_t device);
 void vsb_model_destroy(vsb_model* m);
@@ -177,6 +186,14 @@ int vsb_embedder_forward(vsb_model* m, const float* x_dev, const uint8_t* msgs_d
  * return VSB_ERR_UNSUPPORTED for pixel-wise models. */
 int vsb_detect(vsb_model* m, const float* imgs_dev, float* logits_dev, int32_t F, int32_t H, int32_t W, int32_t flags,
                void* stream);
+/* vsb_detect with the frames in groups of `group` consecutive frames (the last group may be shorter): one reference detector call
+ * each, a video chunk of chunk_size frames (videoseal.py:373-379) or, in image mode, the whole batch (wam.py:206-234).  Only a DVMark
+ * extractor convolves across the frames of a group; frames of different groups never interact, and the other extractors ignore
+ * `group`.  DVMark: VSB_ERR_INVALID for group < 1, VSB_ERR_UNSUPPORTED for group > 64 (a group must fit one 64-frame sub-batch).
+ * vsb_detect and vsb_detect_host take the whole call as one group (group = F).  vsb_embed_detect_host and vsb_frames_host_u8 with
+ * logits_host != NULL, whose slices would split the groups, return VSB_ERR_UNSUPPORTED for a DVMark extractor. */
+int vsb_detect_grouped(vsb_model* m, const float* imgs_dev, float* logits_dev, int32_t F, int32_t H, int32_t W, int32_t group,
+                       int32_t flags, void* stream);
 
 /* imgs_dev [F,3,H,W] -> hmaps_dev [F,jnd_out_ch,H,W] */
 int vsb_jnd_heatmaps(vsb_model* m, const float* imgs_dev, float* hmaps_dev, int32_t F, int32_t H, int32_t W, void* stream);

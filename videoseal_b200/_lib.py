@@ -16,7 +16,7 @@ EXPORTS = [
     "vsb_debug_conv",
     "vsb_debug_resample_table", "vsb_debug_resample_table2", "vsb_debug_last_dispatch", "vsb_quality_workspace_bytes", "vsb_ssim", "vsb_model_set_vit_extractor",
     "vsb_augment_workspace_bytes", "vsb_augment", "vsb_model_set_unet_temporal", "vsb_model_set_hidden_embedder",
-    "vsb_model_set_hidden_extractor",
+    "vsb_model_set_hidden_extractor", "vsb_model_set_dvmark_extractor", "vsb_detect_grouped",
 ]
 
 FLAG_CLAMP, FLAG_LOWRES_ATTN, FLAG_NO_ATTENUATION, FLAG_RESIZE_NO_AA = 1, 2, 4, 8
@@ -86,6 +86,7 @@ def lib():
     L.vsb_model_set_unet_temporal.argtypes = [C.c_void_p, C.c_int32]
     L.vsb_model_set_hidden_embedder.argtypes = [C.c_void_p, C.POINTER(HiddenDesc)]
     L.vsb_model_set_hidden_extractor.argtypes = [C.c_void_p, C.POINTER(HiddenDesc)]
+    L.vsb_model_set_dvmark_extractor.argtypes = [C.c_void_p, C.c_int32]
     L.vsb_model_finalize.argtypes = [C.c_void_p, C.c_int32]
     L.vsb_model_destroy.argtypes = [C.c_void_p]
     L.vsb_model_destroy.restype = None
@@ -93,6 +94,8 @@ def lib():
                             C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_int32, C.c_void_p]
     L.vsb_embedder_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]
     L.vsb_detect.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
+    L.vsb_detect_grouped.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                     C.c_void_p]
     L.vsb_jnd_heatmaps.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     L.vsb_embed_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                  C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_int32]

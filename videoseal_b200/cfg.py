@@ -73,8 +73,9 @@ def spec_from_card(card: dict) -> dict:
     if not emb_name.startswith(("unet", "hidden")):
         raise NotImplementedError(f"embedder '{emb_name}': only the unet* and hidden* families are on the CUDA hot path")
     is_vit = ext_name.startswith("sam")
-    if not (ext_name.startswith(("convnext", "hidden")) or is_vit):
-        raise NotImplementedError(f"extractor '{ext_name}': only the convnext*, sam* and hidden* families are on the CUDA hot path")
+    if not (ext_name.startswith(("convnext", "hidden", "dvmark")) or is_vit):
+        raise NotImplementedError(f"extractor '{ext_name}': only the convnext*, sam*, hidden* and dvmark* families are on the CUDA hot "
+                                  "path")
     if str(a.get("blending_method", "additive")) != "additive":
         raise NotImplementedError("only additive blending is implemented (all shipped cards use it)")
     if emb_name.startswith("hidden"):
@@ -84,6 +85,9 @@ def spec_from_card(card: dict) -> dict:
     if ext_name.startswith("hidden"):
         extractor = {"hidden_decoder": _hidden(card["extractor"]["params"], embedder=False),
                      "pixel_decoder": {"pixelwise": False, "upscale_stages": [1]}}
+    elif ext_name.startswith("dvmark"):
+        # build_extractor: DVMarkDecoder(nbits); the preset has no parameters (params: [])
+        extractor = {"dvmark_decoder": {"nbits": nbits}, "pixel_decoder": {"pixelwise": False, "upscale_stages": [1]}}
     else:
         extractor = _trunk(card["extractor"]["params"], nbits, is_vit)
     att = str(a.get("attenuation", "None"))

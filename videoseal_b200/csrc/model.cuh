@@ -7,6 +7,7 @@
 
 #include "convnext.cuh"
 #include "decoder.cuh"
+#include "dvmark.cuh"
 #include "hidden.cuh"
 #include "resize_blend_host.cuh"
 #include "unet.cuh"
@@ -27,6 +28,7 @@ class Model {
   VitTrunk vit;
   Decoder dec;
   Hidden henc, hdec;   // HiDDeN embedder / extractor, in place of the U-Net / the trunk and decoder (vsb_model_set_hidden_*)
+  DVMark dvdec;        // DVMark extractor, in place of the trunk and decoder (vsb_model_set_dvmark_extractor)
 
   // grow-only device staging for the host-buffer entry points (no cudaMalloc on the steady-state path)
   struct Staging { void* p = nullptr; size_t cap = 0; };
@@ -101,6 +103,23 @@ class Model {
     e.set(h, false, d);
     hdec = e;
   }
+  void set_dvmark_extractor(int nbits) {
+    check_unfinalized();
+    if (vit.on || dec.pixelwise || hdec.on)
+      throw Error("vsb_model_set_dvmark_extractor: the model already has a SAM-ViT trunk, a pixel-wise decoder or a HiDDeN extractor", kErrState);
+    for (int s = 0; s < 4; ++s)
+      if (d.ext_dims[s] != 0 || d.ext_depths[s] != 0)
+        throw Error("vsb_model_set_dvmark_extractor: the descriptor also describes a ConvNeXt trunk (ext_dims / ext_depths != 0)", kErrInvalid);
+    DVMark e;
+    e.set(nbits, d);
+    dvdec = e;
+  }
+  // the entry points that detect slices of a stream cut it on their own boundaries, not on the DVMark extractor's groups
+  void check_frame_independent_detect(const std::string& what) const {
+    if (dvdec.on)
+      throw Error(what + ": a DVMark extractor convolves across the frames of a group, which the streamed slices would split; use "
+                  "vsb_detect_grouped", kErrUnsupported);
+  }
   void set_tensor(const char* name, const float* data, const int64_t* shape, int ndim) {
     check_unfinalized();
     HostTensor t;
@@ -111,6 +130,7 @@ class Model {
   void set_pixel_decoder(int n, const int32_t* f, int pw) {
     check_unfinalized();
     if (hdec.on && pw != 0) throw Error("HiDDeN extractor: per-pixel maps (pixelwise) are not implemented", kErrUnsupported);
+    if (dvdec.on && pw != 0) throw Error("DVMark extractor: per-pixel maps (pixelwise) are not implemented", kErrUnsupported);
     dec.set(n, f, pw, vit.on || d.ext_stem_stride == 4, d.nbits, [&] { return std::make_pair(trunk_width(), trunk_map()); });
   }
   // the U-Net's rules and kernel choice again, for a temporal U-Net
@@ -126,7 +146,7 @@ class Model {
   void set_vit_extractor(const vsb_vit_desc& v) {
     check_unfinalized();
     if (dec.pixelwise) throw Error("vsb_model_set_vit_extractor must come before vsb_model_set_pixel_decoder", kErrState);
-    if (hdec.on) throw Error("vsb_model_set_vit_extractor: the model already has a HiDDeN extractor", kErrState);
+    if (hdec.on || dvdec.on) throw Error("vsb_model_set_vit_extractor: the model already has a HiDDeN or DVMark extractor", kErrState);
     vit.set(v, d.img_size);
   }
   int trunk_width() const { return vit.on ? vit.width() : d.ext_dims[3]; }
@@ -157,6 +177,7 @@ class Model {
       unet.pack(ws, num_sms);
     }
     if (hdec.on) hdec.pack(ws, num_sms);
+    else if (dvdec.on) dvdec.pack(ws, num_sms);
     else {
       if (vit.on) vit.pack(ws, d.img_size);
       else cnx.pack(ws, d);
@@ -169,7 +190,8 @@ class Model {
   // Plan cache: one activation arena per distinct batch size, at most `max_plans` per kind (VSB_MAX_PLANS, default 8): a service that sees
   // many different clip / tail lengths would otherwise accumulate up to 64 arenas of up to 2.3 GB each (a temporal U-Net's embed plan
   // holds one more buffer, its time-stacked operand: B * S^2 * temporal_stack_width(z0) fp16 values, 512 MiB at 64 x 256^2 and
-  // 4.5 GiB at 64 x 768^2; and its plans are also keyed by the group length).  The least recently used plan
+  // 4.5 GiB at 64 x 768^2; and its plans are also keyed by the group length; a DVMark detect plan holds three maps, 40 KiB * S^2 in all at
+  // 64 frames, and at most 512 MiB of time-stacked operand: 3 GiB at 64 x 256^2, 23 GiB at 64 x 768^2).  The least recently used plan
   // is dropped (its cudaFree calls synchronise the device, so work still in flight on it completes first).
   uint64_t plan_clock = 0;
   int max_plans = [] { const char* e = getenv("VSB_MAX_PLANS"); const int v = e ? atoi(e) : 8; return v < 2 ? 2 : v; }();
@@ -200,12 +222,15 @@ class Model {
     pl.tap("x_res", pl.x_res, 0, key, 3, S, S, S);
     henc.build(pl, key, S, keep_inputs);
   }
-  void build_detect_plan(Plan& pl, int B) {
+  // detect plans are keyed by B + kPlanGroup * G: a DVMark extractor's plan also depends on its group length G (0 for the others)
+  void build_detect_plan(Plan& pl, int key) {
+    const int B = key % kPlanGroup, G = key / kPlanGroup;
     const int S = d.img_size;
     pl.x_res = pl.pool.alloc_n<float>((size_t)B * 3 * S * S);
     pl.tap("x_res", pl.x_res, 0, B, 3, S, S, S);
     pl.logits = pl.pool.alloc_n<float>((size_t)B * (1 + d.nbits));
     if (hdec.on) { hdec.build(pl, B, S, keep_inputs); return; }
+    if (dvdec.on) { dvdec.build(pl, B, G, S); return; }
     const FeatureMap m = vit.on ? vit.build(pl, B, S, num_sms, keep_inputs) : cnx.build(pl, B, d, num_sms, keep_inputs);
     dec.build(pl, B, m, vit.on ? "vit." : "cnx.", d.nbits, num_sms);
   }
@@ -220,7 +245,10 @@ class Model {
                   std::to_string(kMaxBatch) + " are implemented", kErrUnsupported);
     return chunk_keys;
   }
-  Plan* get_detect_plan(int B) { return get_plan(detect_plans, B, &Model::build_detect_plan); }
+  Plan* get_detect_plan(int B, int G) { return get_plan(detect_plans, B + kPlanGroup * G, &Model::build_detect_plan); }
+  // a DVMark extractor convolves across a group of `group` frames (one reference detector call); the other extractors take frames
+  // one at a time and ignore it
+  int detect_group(int group) const { return dvdec.on ? DVMark::group(group, kMaxBatch) : 0; }
 
 
   ResampleDev* get_resampler(int ih, int iw, int oh, int ow, ResampleMode m) {
@@ -266,7 +294,7 @@ class Model {
     if (pw) VSB_CUDA(cudaMemcpyAsync(preds_w_h, pw, np * sizeof(float), cudaMemcpyDeviceToHost, st));
     VSB_CUDA(cudaStreamSynchronize(st));
   }
-  void detect_host(const float* imgs_h, float* logits_h, int F, int H, int W, int flags) {
+  void detect_host(const float* imgs_h, float* logits_h, int F, int H, int W, int group, int flags) {
     check_ready();
     const size_t n = (size_t)F * 3 * H * W;
     const size_t nl = (size_t)F * detect_out_per_frame();
@@ -274,7 +302,7 @@ class Model {
     float* lg = (float*)stage(2, nl * sizeof(float));
     cudaStream_t st = 0;
     VSB_CUDA(cudaMemcpyAsync(imgs, imgs_h, n * sizeof(float), cudaMemcpyHostToDevice, st));
-    detect(imgs, lg, F, H, W, flags, st);
+    detect(imgs, lg, F, H, W, group, flags, st);
     VSB_CUDA(cudaMemcpyAsync(logits_h, lg, nl * sizeof(float), cudaMemcpyDeviceToHost, st));
     VSB_CUDA(cudaStreamSynchronize(st));
   }
@@ -346,7 +374,7 @@ class Model {
       VSB_CUDA(cudaMemcpyAsync(imgs_w_h + (size_t)f0 * fpx, out + (size_t)f0 * fpx, (size_t)n * fpx * sizeof(float), cudaMemcpyDeviceToHost, s_out));
       if (f0 + n - g0 >= kMaxBatch || k == nsl - 1) {   // a full extractor batch (or the tail) is complete: detect its frames
         const int gn = f0 + n - g0;
-        detect(out + (size_t)g0 * fpx, lg + (size_t)g0 * NO, gn, H, W, flags & VSB_FLAG_RESIZE_BITS, s_cmp);
+        detect(out + (size_t)g0 * fpx, lg + (size_t)g0 * NO, gn, H, W, 0, flags & VSB_FLAG_RESIZE_BITS, s_cmp);
         VSB_CUDA(cudaEventRecord(ev_cmp[nsl], s_cmp));
         VSB_CUDA(cudaStreamWaitEvent(s_out, ev_cmp[nsl], 0));
         VSB_CUDA(cudaMemcpyAsync(logits_h + (size_t)g0 * NO, lg + (size_t)g0 * NO, (size_t)gn * NO * sizeof(float), cudaMemcpyDeviceToHost, s_out));
@@ -397,7 +425,7 @@ class Model {
         g_launches += 1;
         det_in = out + (size_t)f0 * fpx;
       }
-      if (do_detect) detect(det_in, lg + (size_t)f0 * NO, n, H, W, flags & VSB_FLAG_RESIZE_BITS, s_cmp);
+      if (do_detect) detect(det_in, lg + (size_t)f0 * NO, n, H, W, 0, flags & VSB_FLAG_RESIZE_BITS, s_cmp);
       VSB_CUDA(cudaGetLastError());
       VSB_CUDA(cudaEventRecord(ev_cmp[k], s_cmp));
       VSB_CUDA(cudaStreamWaitEvent(s_out, ev_cmp[k], 0));
@@ -516,17 +544,21 @@ class Model {
     g_launches += 1;
   }
 
-  void detect(const float* imgs, float* logits, int F, int H, int W, int flags, cudaStream_t st) {
+  // group: frames per DVMark detector call (the last group may be shorter); sub-batches then hold whole groups.  A group longer
+  // than the call is the whole call, and a plan's group is at most its frames, so equal computations share one plan.
+  void detect(const float* imgs, float* logits, int F, int H, int W, int group, int flags, cudaStream_t st) {
     check_ready();
     VSB_CHECK(F > 0 && H > 0 && W > 0, "bad detect shape");
+    const int G = detect_group(std::min(group, F));
+    const int batch = G ? (kMaxBatch / G) * G : kMaxBatch;
     const int S = d.img_size;
     const bool same = (H == S && W == S);
     const ResampleMode rm = same ? ResampleMode() : resample_mode(flags);
     const long fstride = (long)3 * H * W;
     const size_t NO = detect_out_per_frame();
-    for (int f0 = 0; f0 < F; f0 += kMaxBatch) {
-      const int n = std::min(kMaxBatch, F - f0);
-      Plan* pl = get_detect_plan(n);
+    for (int f0 = 0; f0 < F; f0 += batch) {
+      const int n = std::min(batch, F - f0);
+      Plan* pl = get_detect_plan(n, std::min(G, n));
       const float* x = imgs + (size_t)f0 * fstride;
       if (!same) { resize_frames(x, fstride, n, H, W, pl->x_res, rm, st); x = pl->x_res; }
       pl->in_imgs = x;

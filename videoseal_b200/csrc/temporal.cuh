@@ -3,7 +3,8 @@
 // group.  A sub-batch of B frames holds whole groups: frames [g*G, min((g+1)*G, B)), so only the last one may be shorter.
 //   temporal_stack_kernel      the time taps of a 3x3x3 conv as channels: xs[b, p] = [x[b-1, p] | x[b, p] | x[b+1, p] | 0 ...], a
 //                              neighbour outside b's group reading as zeros.  The 3x3x3 conv over x is then the 3x3 conv over xs
-//                              (K = 9 * Cs, spatial tap major, then time, then channel), which runs on the tensor-core convs.
+//                              (K = 9 * Cs, spatial tap major, then time, then channel), which runs on the tensor-core convs.  It
+//                              can stack a slice of the batch's frames, and (POOL) the 2x2 mean of x (the DVMark extractor, dvmark.cuh).
 //   unet_first_t_kernel        the `inc` block's first conv as 3x3x3 over 1 or 3 input channels (27 taps) + folded BN + ReLU, and
 //                              its 1x1x1 res conv, on CUDA cores (the temporal form of unet_first_kernel).
 #pragma once
@@ -20,26 +21,54 @@ __device__ __forceinline__ bool same_group(int b, int dt, int B, int G) {
   return t >= 0 && t < B && t / G == b / G;
 }
 
-// xs [B, HW, Cs] fp16 (dense), x [B, HW, C] fp16 with pixel pitch ldx; C and ldx multiples of 8.  One 16-byte vector per thread.
-__global__ void __launch_bounds__(256) temporal_stack_kernel(const __half* __restrict__ x, int ldx, int C, long HW, int B, int G,
-                                                             __half* __restrict__ xs, int Cs) {
+// xs [n, HW, Cs] fp16 (dense): frames b0 .. b0 + n - 1 of the B-frame batch.  x [B, HW, C] fp16 with pixel pitch ldx, or with POOL
+// x [B, 2h, 2h, C] (HW = h * h), stacked as its 2x2 mean (AvgPool3d (1,2,2): the four fp16 values summed in fp32, rounded once).
+// C and ldx multiples of 8.  One 16-byte vector per thread.
+template <bool POOL>
+__global__ void __launch_bounds__(256) temporal_stack_kernel(const __half* __restrict__ x, int ldx, int C, long HW, int h, int b0, int n,
+                                                             int B, int G, __half* __restrict__ xs, int Cs) {
   const int vpp = Cs / 8;
-  const long n = (long)B * HW * vpp;
-  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+  const long total = (long)n * HW * vpp;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const long pix = i / vpp;
     const int c8 = (int)(i - pix * vpp) * 8;
-    const int b = (int)(pix / HW), dt = c8 / C, c = c8 - dt * C;
+    const int b = b0 + (int)(pix / HW), dt = c8 / C, c = c8 - dt * C;
+    const long p = pix % HW;
     uint4 v = make_uint4(0u, 0u, 0u, 0u);
-    if (dt < 3 && same_group(b, dt - 1, B, G)) v = __ldg(reinterpret_cast<const uint4*>(x + (pix + (long)(dt - 1) * HW) * ldx + c));
+    if (dt < 3 && same_group(b, dt - 1, B, G)) {
+      const int bs = b + dt - 1;
+      if (!POOL) {
+        v = __ldg(reinterpret_cast<const uint4*>(x + ((long)bs * HW + p) * ldx + c));
+      } else {
+        const int y = (int)(p / h), xx = (int)(p % h), w2 = 2 * h;
+        const __half* s0 = x + (((long)bs * w2 + 2 * y) * w2 + 2 * xx) * ldx + c;
+        const uint4 u[4] = {__ldg(reinterpret_cast<const uint4*>(s0)), __ldg(reinterpret_cast<const uint4*>(s0 + ldx)),
+                            __ldg(reinterpret_cast<const uint4*>(s0 + (long)w2 * ldx)),
+                            __ldg(reinterpret_cast<const uint4*>(s0 + (long)w2 * ldx + ldx))};
+        __align__(16) __half o[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          float s = 0.f;
+#pragma unroll
+          for (int q = 0; q < 4; ++q) s += __half2float(reinterpret_cast<const __half*>(&u[q])[j]);
+          o[j] = __float2half_rn(0.25f * s);
+        }
+        v = *reinterpret_cast<const uint4*>(o);
+      }
+    }
     reinterpret_cast<uint4*>(xs)[i] = v;
   }
 }
 
-inline void launch_temporal_stack(const __half* x, int ldx, int C, long HW, int B, int G, __half* xs, int Cs, int num_sms, cudaStream_t st) {
+// frames [b0, b0 + n) of the batch; pool: x is at 2h x 2h and HW = h * h
+inline void launch_temporal_stack(const __half* x, int ldx, int C, long HW, int b0, int n, int B, int G, __half* xs, int Cs, int num_sms,
+                                  cudaStream_t st, bool pool = false, int h = 0) {
   VSB_CHECK(C % 8 == 0 && ldx % 8 == 0 && Cs % 8 == 0 && Cs >= 3 * C && G >= 1, "temporal stack: channel layout");
-  const long n = (long)B * HW * (Cs / 8);
-  const long blocks = std::min<long>((n + 255) / 256, (long)num_sms * 16);
-  temporal_stack_kernel<<<(unsigned)blocks, 256, 0, st>>>(x, ldx, C, HW, B, G, xs, Cs);
+  VSB_CHECK(b0 >= 0 && n >= 1 && b0 + n <= B && (!pool || (long)h * h == HW), "temporal stack: frame slice / pooled map");
+  const long total = (long)n * HW * (Cs / 8);
+  const long blocks = std::min<long>((total + 255) / 256, (long)num_sms * 16);
+  if (pool) temporal_stack_kernel<true><<<(unsigned)blocks, 256, 0, st>>>(x, ldx, C, HW, h, b0, n, B, G, xs, Cs);
+  else temporal_stack_kernel<false><<<(unsigned)blocks, 256, 0, st>>>(x, ldx, C, HW, h, b0, n, B, G, xs, Cs);
   VSB_CUDA(cudaGetLastError());
 }
 

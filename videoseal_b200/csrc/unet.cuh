@@ -263,7 +263,7 @@ struct UNet {
     const int Cs = temporal_stack_width(Cin), sms = nsm;
     const std::string at = std::to_string(H);
     pl.add("unet.tstack." + std::to_string(Cin) + "-" + std::to_string(Cs) + "@" + at,
-           [=](cudaStream_t st) { launch_temporal_stack(x, ldx, Cin, (long)H * W, B, G, xs, Cs, sms, st); });
+           [=](cudaStream_t st) { launch_temporal_stack(x, ldx, Cin, (long)H * W, 0, B, B, G, xs, Cs, sms, st); });
     add_conv(pl, w, 3, xs, B, H, W, Cs, Cs, relu, resid, out, ld_out, fuse_outc,
              std::string("unet.conv3x3x3") + (fuse_outc ? "+outc." : ".") + std::to_string(Cin) + "-" + std::to_string(w.N) + "@" + at);
   }

@@ -110,6 +110,15 @@ int vsb_model_set_hidden_extractor(vsb_model* m, const vsb_hidden_desc* h) {
   VSB_API_END
 }
 
+int vsb_model_set_dvmark_extractor(vsb_model* m, int32_t nbits) {
+  VSB_API_BEGIN
+  VSB_CHECK(m != nullptr, "null argument");
+  std::lock_guard<std::recursive_mutex> lk(m->impl.mu);
+  m->impl.set_dvmark_extractor(nbits);
+  return VSB_OK;
+  VSB_API_END
+}
+
 int vsb_model_finalize(vsb_model* m, int32_t device) {
   VSB_API_BEGIN
   VSB_CHECK(m != nullptr, "null model");
@@ -150,7 +159,17 @@ int vsb_detect(vsb_model* m, const float* imgs, float* logits, int32_t F, int32_
   VSB_API_BEGIN
   VSB_CHECK(m && imgs && logits, "null argument");
   VSB_MODEL_SCOPE(m);
-  m->impl.detect(imgs, logits, F, H, W, flags, (cudaStream_t)stream);
+  m->impl.detect(imgs, logits, F, H, W, F, flags, (cudaStream_t)stream);
+  return VSB_OK;
+  VSB_API_END
+}
+
+int vsb_detect_grouped(vsb_model* m, const float* imgs, float* logits, int32_t F, int32_t H, int32_t W, int32_t group, int32_t flags,
+                       void* stream) {
+  VSB_API_BEGIN
+  VSB_CHECK(m && imgs && logits, "null argument");
+  VSB_MODEL_SCOPE(m);
+  m->impl.detect(imgs, logits, F, H, W, group, flags, (cudaStream_t)stream);
   return VSB_OK;
   VSB_API_END
 }
@@ -179,7 +198,7 @@ int vsb_detect_host(vsb_model* m, const float* imgs_h, float* logits_h, int32_t 
   VSB_API_BEGIN
   VSB_CHECK(m && imgs_h && logits_h, "null argument");
   VSB_MODEL_SCOPE(m);
-  m->impl.detect_host(imgs_h, logits_h, F, H, W, flags);
+  m->impl.detect_host(imgs_h, logits_h, F, H, W, F, flags);
   return VSB_OK;
   VSB_API_END
 }
@@ -191,6 +210,7 @@ int vsb_embed_detect_host(vsb_model* m, const float* imgs_h, const uint8_t* msgs
   VSB_CHECK(m && imgs_h && msgs_h && imgs_w_h && logits_h, "null argument");
   VSB_MODEL_SCOPE(m);
   m->impl.check_pooled_head("vsb_embed_detect_host");
+  m->impl.check_frame_independent_detect("vsb_embed_detect_host");
   m->impl.embed_detect_host(imgs_h, msgs_h, n_msgs, imgs_w_h, logits_h, F, H, W, step, video_mode, chunk_keys, scaling_i, scaling_w,
                             flags);
   return VSB_OK;
@@ -205,6 +225,7 @@ int vsb_frames_host_u8(vsb_model* m, const uint8_t* frames_h, const uint8_t* msg
   VSB_MODEL_SCOPE(m);
   VSB_CHECK(F > 0 && H > 0 && W > 0 && step >= 1, "bad shape");
   if (logits_h) m->impl.check_pooled_head("vsb_frames_host_u8 with logits");
+  if (logits_h) m->impl.check_frame_independent_detect("vsb_frames_host_u8 with logits");
   m->impl.frames_host_u8(frames_h, msgs_h, n_msgs, frames_w_h, logits_h, F, H, W, step, video_mode, chunk_keys, scaling_i, scaling_w,
                          flags);
   return VSB_OK;

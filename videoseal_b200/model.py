@@ -117,7 +117,7 @@ def trunk_map(spec: dict) -> int:
 
 def _create(spec: dict):
     """Native handle of `spec` without weights or a device.  vsb_model_create, vsb_model_set_unet_temporal,
-    vsb_model_set_hidden_embedder / _extractor, vsb_model_set_vit_extractor and vsb_model_set_pixel_decoder check every rule the kernels place on the model's geometry; a
+    vsb_model_set_hidden_embedder / _extractor, vsb_model_set_dvmark_extractor, vsb_model_set_vit_extractor and vsb_model_set_pixel_decoder check every rule the kernels place on the model's geometry; a
     model they do not implement raises NotImplementedError."""
     L = _lib.lib()
     if "hidden_encoder" not in spec and not spec["unet"]["z"]:
@@ -132,6 +132,8 @@ def _create(spec: dict):
         rc = L.vsb_model_set_hidden_embedder(h, C.byref(native_hidden_desc(spec["hidden_encoder"], True)))
     if rc == 0 and "hidden_decoder" in spec:
         rc = L.vsb_model_set_hidden_extractor(h, C.byref(native_hidden_desc(spec["hidden_decoder"], False)))
+    if rc == 0 and "dvmark_decoder" in spec:
+        rc = L.vsb_model_set_dvmark_extractor(h, int(spec["dvmark_decoder"]["nbits"]))
     if rc == 0 and "vit" in spec:
         rc = L.vsb_model_set_vit_extractor(h, C.byref(native_vit_desc(spec["vit"])))
     if rc == 0 and f:
@@ -330,10 +332,11 @@ class Videoseal(nn.Module):
         L = _lib.lib()
         h = _create(self.spec)
         try:
-            temporal = self.temporal
+            temporal, dvmark = self.temporal, self.dvmark
             for k, v in self._sd.items():
-                # 5-D tensors: only a temporal U-Net's Conv3d weights are read
-                if k.startswith(("attenuation.", "rgb2yuv.")) or (v.dim() > 4 and not (temporal and k.startswith("embedder.unet."))):
+                # 5-D tensors: only the Conv3d weights of a temporal U-Net and of a DVMark extractor are read
+                if k.startswith(("attenuation.", "rgb2yuv.")) or (v.dim() > 4 and not (temporal and k.startswith("embedder.unet."))
+                                                                   and not (dvmark and k.startswith("detector.layers."))):
                     continue
                 shape = (C.c_int64 * max(1, v.dim()))(*v.shape)
                 _lib.check(L.vsb_model_set_tensor(h, k.encode(), v.data_ptr(), shape, v.dim()))
@@ -422,11 +425,28 @@ class Videoseal(nn.Module):
         return keys
 
     @property
+    def dvmark(self) -> bool:
+        """True for a DVMark extractor: its 3x3x3 convs mix the frames of one detector call"""
+        return "dvmark_decoder" in self.spec
+
+    def _detect_group(self, is_video: bool, num_frames: int) -> int:
+        """vsb_detect_grouped's group: frames per reference detector call.  A video is detected in chunks of chunk_size frames
+        (videoseal.py:373-379), so a clip shorter than chunk_size is one call of all its frames; in image mode the whole batch is
+        one call (wam.py:206-234).  This matters only to a DVMark extractor, whose group must fit one 64-frame sub-batch."""
+        g = min(int(self.chunk_size), int(num_frames)) if is_video else int(num_frames)
+        if self.dvmark and g > 64:
+            what = f"chunk_size={g}" if is_video else f"image mode with {g} images"
+            raise NotImplementedError(f"DVMark extractor: {what} puts more than 64 frames in one 3x3x3 conv group; at most 64 are "
+                                      "implemented")
+        return g
+
+    @property
     def pixelwise(self) -> bool:
         """True when detect() returns per-pixel maps [F, 1+K, P, P] (pixel_decoder.pixelwise of the card)."""
         return bool(self.spec.get("pixel_decoder", {}).get("pixelwise", False))
 
-    def _detect_dev(self, x: torch.Tensor, flags: int) -> torch.Tensor:
+    def _detect_dev(self, x: torch.Tensor, flags: int, group: Optional[int] = None) -> torch.Tensor:
+        """vsb_detect_grouped in groups of `group` frames (None: the whole batch is one detector call)"""
         shape = (x.shape[0], 1 + self.spec["nbits"])
         if self.pixelwise:   # trunk map (img_size / 32, a ViT's img_size / 16) x the product of the stage factors
             P = trunk_map(self.spec)
@@ -434,17 +454,19 @@ class Videoseal(nn.Module):
                 P *= f
             shape += (P, P)
         out = torch.empty(shape, device=x.device, dtype=torch.float32)
-        _lib.check(_lib.lib().vsb_detect(self._handle(), x.data_ptr(), out.data_ptr(), x.shape[0], x.shape[2], x.shape[3], flags,
-                                         self._stream()))
+        g = self._detect_group(False, x.shape[0]) if group is None else group
+        _lib.check(_lib.lib().vsb_detect_grouped(self._handle(), x.data_ptr(), out.data_ptr(), x.shape[0], x.shape[2], x.shape[3], g,
+                                                 flags, self._stream()))
         return out
 
     @torch.no_grad()
     def detect(self, imgs: torch.Tensor, is_video: bool = True, interpolation: dict = _DEF_INTERP) -> dict:
-        """models/videoseal.py:352-388; frames are independent so the chunk loop is internal to the library."""
+        """models/videoseal.py:352-388; the chunk loop is internal to the library (only a DVMark extractor mixes the frames of a
+        chunk)."""
         if not is_video:
             interpolation = _DEF_INTERP       # the reference drops `interpolation` on this branch (videoseal.py:374)
         flags = resize_flags(interpolation, tuple(imgs.shape[-2:]) != (self.img_size, self.img_size))
-        preds = self._detect_dev(self._to_dev(imgs), flags)
+        preds = self._detect_dev(self._to_dev(imgs), flags, self._detect_group(is_video, imgs.shape[0]))
         return {"preds": preds.to(imgs.device)}
 
     def extract_message(self, imgs: torch.Tensor, aggregation: str = "avg",
