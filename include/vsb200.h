@@ -155,6 +155,17 @@ int vsb_model_set_hidden_extractor(vsb_model* m, const vsb_hidden_desc* h);
  * nbits < 1 or nbits other than the descriptor's (any nbits >= 1 is implemented); VSB_ERR_UNSUPPORTED for an img_size that is not a
  * positive multiple of 128.  A group of frames convolved together is at most 64 long (vsb_detect_grouped). */
 int vsb_model_set_dvmark_extractor(vsb_model* m, int32_t nbits);
+/* DVMark embedder (modules/dvmark.py DVMarkEncoder; models/embedder.py DVMarkEmbedder, build_embedder 'dvmark'): Conv3d layers with
+ * bias over the key frames of one embedder call on x = 2 imgs - 1, the message bits of each frame as nbits constant 0 / 1 planes:
+ * (1,3,3) convs 3 -> 64 -> 64 -> 64 and a 3x3x3 64 -> 64 (ReLU); [x | planes] -> 256 -> 128 -> 128 (3x3x3, ReLU): x_skip;
+ * [avgpool (1,2,2) of x_skip | planes] -> 512 -> 256 -> 256 (3x3x3, ReLU); bilinear up-sample (align_corners=True); [x_skip | up]
+ * -> 256 -> 128 (3x3x3, ReLU) -> 3 (3x3x3), tanh: the delta (3 channels).  Checkpoint keys embedder.unet.{transform_layer.{0,2,4,6},
+ * emb_layer{1,2,3}.{0,2,4}}.{weight,bias}, 5-D weights.  It replaces the U-Net like the HiDDeN embedder: unet_levels 0, unet_in_ch
+ * = unet_out_ch = 3 (else VSB_ERR_INVALID).  Called after vsb_model_create and before finalize; no CUDA call.  VSB_ERR_STATE after
+ * finalize or when the model already has a HiDDeN embedder or a temporal U-Net; VSB_ERR_INVALID for nbits < 1 or nbits other than
+ * the descriptor's (any nbits >= 1 is implemented); VSB_ERR_UNSUPPORTED for an img_size that is not a positive multiple of 128 or
+ * is above 512.  vsb_embed groups its key frames as for a temporal U-Net: at most 64 per group (chunk_keys). */
+int vsb_model_set_dvmark_embedder(vsb_model* m, int32_t nbits);
 /* fold BN, pack to fp16 KRSC, upload to `device`, build nothing else (plans are built lazily per batch shape) */
 int vsb_model_finalize(vsb_model* m, int32_t device);
 void vsb_model_destroy(vsb_model* m);
@@ -168,13 +179,13 @@ void vsb_model_destroy(vsb_model* m);
  * A temporal U-Net (vsb_model_set_unet_temporal) convolves across the key frames of one group of chunk_keys consecutive key frames (one
  * reference embedder call: a video chunk, or, in image mode, the whole batch, so pass chunk_keys = F there); the last group may be
  * shorter, and frames of different groups never interact.  VSB_ERR_UNSUPPORTED when chunk_keys > 64 (a group must fit one
- * 64-frame sub-batch).  The same holds for vsb_embed_host, vsb_embed_detect_host and vsb_frames_host_u8. */
+ * 64-frame sub-batch).  A DVMark embedder (vsb_model_set_dvmark_embedder) groups its key frames the same way.  The same holds for vsb_embed_host, vsb_embed_detect_host and vsb_frames_host_u8. */
 int vsb_embed(vsb_model* m, const float* imgs_dev, const uint8_t* msgs_dev, int32_t n_msgs, float* imgs_w_dev,
               float* preds_w_dev, int32_t F, int32_t H, int32_t W, int32_t step, int32_t video_mode, int32_t chunk_keys,
               float scaling_i, float scaling_w, int32_t flags, void* stream);
 
 /* x_dev [B, 3, S, S] RGB fp32 in [0,1] at processing size S = img_size (the Y extraction for yuv cards happens
- * inside, wam.py:168-172); delta_dev [B, unet_out_ch, S, S].  A temporal U-Net takes the B frames as one group (one reference
+ * inside, wam.py:168-172); delta_dev [B, unet_out_ch, S, S].  A temporal U-Net or a DVMark embedder takes the B frames as one group (one reference
  * embedder call): VSB_ERR_UNSUPPORTED for B > 64. */
 int vsb_embedder_forward(vsb_model* m, const float* x_dev, const uint8_t* msgs_dev, int32_t n_msgs, float* delta_dev,
                          int32_t B, void* stream);

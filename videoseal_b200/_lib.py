@@ -17,6 +17,7 @@ EXPORTS = [
     "vsb_debug_resample_table", "vsb_debug_resample_table2", "vsb_debug_last_dispatch", "vsb_quality_workspace_bytes", "vsb_ssim", "vsb_model_set_vit_extractor",
     "vsb_augment_workspace_bytes", "vsb_augment", "vsb_model_set_unet_temporal", "vsb_model_set_hidden_embedder",
     "vsb_model_set_hidden_extractor", "vsb_model_set_dvmark_extractor", "vsb_detect_grouped",
+    "vsb_model_set_dvmark_embedder",
 ]
 
 FLAG_CLAMP, FLAG_LOWRES_ATTN, FLAG_NO_ATTENUATION, FLAG_RESIZE_NO_AA = 1, 2, 4, 8
@@ -87,6 +88,7 @@ def lib():
     L.vsb_model_set_hidden_embedder.argtypes = [C.c_void_p, C.POINTER(HiddenDesc)]
     L.vsb_model_set_hidden_extractor.argtypes = [C.c_void_p, C.POINTER(HiddenDesc)]
     L.vsb_model_set_dvmark_extractor.argtypes = [C.c_void_p, C.c_int32]
+    L.vsb_model_set_dvmark_embedder.argtypes = [C.c_void_p, C.c_int32]
     L.vsb_model_finalize.argtypes = [C.c_void_p, C.c_int32]
     L.vsb_model_destroy.argtypes = [C.c_void_p]
     L.vsb_model_destroy.restype = None

@@ -70,8 +70,8 @@ def spec_from_card(card: dict) -> dict:
     img_size = a["img_size_proc"] if "img_size_proc" in a else a["img_size_extractor"]
     emb_name = str(card["embedder"]["model"])
     ext_name = str(card["extractor"]["model"])
-    if not emb_name.startswith(("unet", "hidden")):
-        raise NotImplementedError(f"embedder '{emb_name}': only the unet* and hidden* families are on the CUDA hot path")
+    if not emb_name.startswith(("unet", "hidden", "dvmark")):
+        raise NotImplementedError(f"embedder '{emb_name}': only the unet*, hidden* and dvmark* families are on the CUDA hot path")
     is_vit = ext_name.startswith("sam")
     if not (ext_name.startswith(("convnext", "hidden", "dvmark")) or is_vit):
         raise NotImplementedError(f"extractor '{ext_name}': only the convnext*, sam*, hidden* and dvmark* families are on the CUDA hot "
@@ -80,6 +80,9 @@ def spec_from_card(card: dict) -> dict:
         raise NotImplementedError("only additive blending is implemented (all shipped cards use it)")
     if emb_name.startswith("hidden"):
         embedder = {"hidden_encoder": _hidden(card["embedder"]["params"], embedder=True)}
+    elif emb_name.startswith("dvmark"):
+        # build_embedder: DVMarkEmbedder(DVMarkEncoder(nbits)); the preset has no parameters (params: [])
+        embedder = {"dvmark_encoder": {"nbits": nbits}}
     else:
         embedder = _unet(card["embedder"]["params"])
     if ext_name.startswith("hidden"):

@@ -154,6 +154,31 @@ __global__ void __launch_bounds__(kDvC3) dvmark_head_kernel(const float* __restr
   }
 }
 
+// frames of one conv launch whose stacked operand (frame_elems fp16 values per frame) stays within kDvStackBudget, at least one
+inline int dv_slice_frames(size_t frame_elems, int B) {
+  return (int)std::max<size_t>(1, std::min<size_t>(B, kDvStackBudget / (frame_elems * sizeof(__half))));
+}
+
+// A 3x3x3 conv over the time taps of x [B][h*h][C] (pitch C; POOL: of the 2x2 mean of x [B][2h][2h][C]) at h x h, in groups of G:
+// per slice of at most `fps` frames, temporal_stack_kernel into xs (xs_cap fp16 values), then the tensor-core 3x3 conv over xs,
+// whose epilogue `epi(op, b0)` sets for the slice that starts at frame b0.  The DVMark extractor and embedder share it.
+template <bool POOL, class Epi>
+void add_conv3d_sliced(Plan& pl, const ConvW& w, const __half* x, int C, int h, int B, int G, __half* xs, size_t xs_cap, int fps,
+                       int nsm, const std::string& unit, const std::string& name, Epi epi) {
+  const int Cs = temporal_stack_width(C);
+  const long hw = (long)h * h;
+  VSB_CHECK((size_t)fps * hw * Cs <= xs_cap, "DVMark: a frame slice's stacked operand exceeds its scratch buffer");
+  for (int b0 = 0; b0 < B; b0 += fps) {
+    const int n = std::min(fps, B - b0);
+    pl.add(unit + ".tstack" + std::string(POOL ? "+pool." : ".") + std::to_string(C) + "-" + std::to_string(Cs) + "@" + std::to_string(h),
+           [=](cudaStream_t st) { launch_temporal_stack(x, C, C, hw, b0, n, B, G, xs, Cs, nsm, st, POOL, h); });
+    ConvGemmOp op;
+    setup_tma_conv(op, xs, n, h, h, Cs, Cs, 3, 3, 1);
+    epi(op, b0);
+    vsb::add_conv(pl, op, w, name, nsm);
+  }
+}
+
 struct DVMark {
   bool on = false;
   int nbits = 0, nsm = 0;
@@ -212,23 +237,16 @@ struct DVMark {
     b4 = ws.pool.upload(conv_b(ws, 4, NO));
   }
 
-  // a 3x3x3 conv over the time taps of x (POOL: of its 2x2 mean) at h x h, frames in slices of at most `fps`, -> out [B][h*h][N];
-  // xs holds xs_cap fp16 values
+  // layer2 / layer3: bias + ReLU -> out [B][h*h][N]
   template <bool POOL>
   void add_conv3d(Plan& pl, const ConvW& w, const __half* x, int C, int h, int B, int G, __half* xs, size_t xs_cap, int fps,
                   __half* out, const std::string& name) const {
-    const int Cs = temporal_stack_width(C), sms = nsm;
     const long hw = (long)h * h;
-    VSB_CHECK((size_t)fps * hw * Cs <= xs_cap, "DVMark: a frame slice's stacked operand exceeds its scratch buffer");
-    for (int b0 = 0; b0 < B; b0 += fps) {
-      const int n = std::min(fps, B - b0);
-      pl.add("dvmark.tstack" + std::string(POOL ? "+pool." : ".") + std::to_string(C) + "-" + std::to_string(Cs) + "@" + std::to_string(h),
-             [=](cudaStream_t st) { launch_temporal_stack(x, C, C, hw, b0, n, B, G, xs, Cs, sms, st, POOL, h); });
-      ConvGemmOp op;
-      setup_tma_conv(op, xs, n, h, h, Cs, Cs, 3, 3, 1);
-      op.p.epi = EPI_AFFINE; op.p.act = ACT_RELU; op.p.bias = w.bias; op.p.out16 = out + b0 * hw * w.N; op.p.ld_out16 = w.N;
-      vsb::add_conv(pl, op, w, name, nsm);
-    }
+    const float* bias = w.bias;
+    const int N = w.N;
+    add_conv3d_sliced<POOL>(pl, w, x, C, h, B, G, xs, xs_cap, fps, nsm, "dvmark", name, [=](ConvGemmOp& op, int b0) {
+      op.p.epi = EPI_AFFINE; op.p.act = ACT_RELU; op.p.bias = bias; op.p.out16 = out + b0 * hw * N; op.p.ld_out16 = N;
+    });
   }
 
   // the detect plan of B frames at S x S in groups of G -> pl.logits [B][1 + nbits].  Taps: dvm.l1, dvm.l2 (NHWC fp16 at S), dvm.l3
@@ -243,8 +261,7 @@ struct DVMark {
     __half* l3 = pl.pool.alloc_n<__half>((size_t)B * hw2 * kDvC3);
     // frames per conv launch: as many as the budget holds (at least one); the scratch fits the larger of the two layers' slices
     const size_t frame2 = (size_t)hw * temporal_stack_width(kDvC1), frame3 = (size_t)hw2 * temporal_stack_width(kDvC1);
-    const int fps2 = (int)std::max<size_t>(1, std::min<size_t>(B, kDvStackBudget / (frame2 * sizeof(__half))));
-    const int fps3 = (int)std::max<size_t>(1, std::min<size_t>(B, kDvStackBudget / (frame3 * sizeof(__half))));
+    const int fps2 = dv_slice_frames(frame2, B), fps3 = dv_slice_frames(frame3, B);
     const size_t xs_cap = std::max((size_t)fps2 * frame2, (size_t)fps3 * frame3);
     __half* xs = pl.pool.alloc_n<__half>(xs_cap);
     const std::string at = "@" + std::to_string(S);

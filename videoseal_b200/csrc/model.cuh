@@ -8,6 +8,7 @@
 #include "convnext.cuh"
 #include "decoder.cuh"
 #include "dvmark.cuh"
+#include "dvmark_enc.cuh"
 #include "hidden.cuh"
 #include "resize_blend_host.cuh"
 #include "unet.cuh"
@@ -29,6 +30,7 @@ class Model {
   Decoder dec;
   Hidden henc, hdec;   // HiDDeN embedder / extractor, in place of the U-Net / the trunk and decoder (vsb_model_set_hidden_*)
   DVMark dvdec;        // DVMark extractor, in place of the trunk and decoder (vsb_model_set_dvmark_extractor)
+  DVMarkEnc dvenc;     // DVMark embedder, in place of the U-Net (vsb_model_set_dvmark_embedder)
 
   // grow-only device staging for the host-buffer entry points (no cudaMalloc on the steady-state path)
   struct Staging { void* p = nullptr; size_t cap = 0; };
@@ -57,13 +59,14 @@ class Model {
   //   resize: MT, GST, vec, toy, OW       blend: 3 (jnd_blend3_kernel) or 2 (jnd_blend2_kernel), VEC, FASTUP, CD, JIN
   int32_t last_resize[5] = {-1, -1, -1, -1, -1};
   int32_t last_blend[5] = {-1, -1, -1, -1, -1};
-  // test seam (vsb_debug_keep_inputs): detect plans (and HiDDeN embed plans) copy buffers that later steps overwrite aside
+  // test seam (vsb_debug_keep_inputs): detect plans (and HiDDeN embed plans) copy buffers that later steps overwrite aside; DVMark
+  // embed plans give every map a buffer of its own
   bool keep_inputs = false;
   void set_keep_inputs(bool on) {
     keep_inputs = on;
     for (auto& kv : detect_plans) if (kv.second.get() == last_plan) last_plan = nullptr;
     detect_plans.clear();
-    if (henc.on) {   // HiDDeN embed plans have the seam too (Hidden::build)
+    if (henc.on || dvenc.on) {   // HiDDeN and DVMark embed plans have the seam too (Hidden::build, DVMarkEnc::build)
       for (auto& kv : embed_plans) if (kv.second.get() == last_plan) last_plan = nullptr;
       embed_plans.clear();
     }
@@ -79,13 +82,17 @@ class Model {
     ConvNeXt::check(d);
     if (!other_embedder()) unet.choose_kernels();
   }
-  // no U-Net levels but the embedder's RGB in / out channels: the embedder is set by vsb_model_set_hidden_embedder
+  // no U-Net levels but the embedder's RGB in / out channels: the embedder is set by vsb_model_set_hidden_embedder or
+  // vsb_model_set_dvmark_embedder
   bool other_embedder() const { return d.unet_levels == 0 && d.unet_in_ch == 3 && d.unet_out_ch == 3; }
   void check_unfinalized() const { if (finalized) throw Error("model already finalized", kErrState); }
   // channels of the embedder's output delta
-  int delta_ch() const { return henc.on ? 3 : d.unet_out_ch; }
+  int delta_ch() const { return (henc.on || dvenc.on) ? 3 : d.unet_out_ch; }
+  // the embedder's 3x3x3 convs mix the key frames of one embedder call (a temporal U-Net or a DVMark embedder)
+  bool frame_mixing_embedder() const { return unet.temporal || dvenc.on; }
   void set_hidden_embedder(const vsb_hidden_desc& h) {
     check_unfinalized();
+    if (dvenc.on) throw Error("vsb_model_set_hidden_embedder: the model already has a DVMark embedder", kErrState);
     if (!other_embedder())
       throw Error("vsb_model_set_hidden_embedder: the descriptor describes a U-Net (a HiDDeN embedder needs unet_levels 0 and unet_in_ch / "
                   "unet_out_ch 3)", kErrInvalid);
@@ -102,6 +109,17 @@ class Model {
     Hidden e;
     e.set(h, false, d);
     hdec = e;
+  }
+  void set_dvmark_embedder(int nbits) {
+    check_unfinalized();
+    if (henc.on || unet.temporal)
+      throw Error("vsb_model_set_dvmark_embedder: the model already has a HiDDeN embedder or a temporal U-Net", kErrState);
+    if (!other_embedder())
+      throw Error("vsb_model_set_dvmark_embedder: the descriptor describes a U-Net (a DVMark embedder needs unet_levels 0 and "
+                  "unet_in_ch / unet_out_ch 3)", kErrInvalid);
+    DVMarkEnc e;
+    e.set(nbits, d);
+    dvenc = e;
   }
   void set_dvmark_extractor(int nbits) {
     check_unfinalized();
@@ -172,8 +190,9 @@ class Model {
     device = dev;
     num_sms = prop.multiProcessorCount;
     if (henc.on) henc.pack(ws, num_sms);
+    else if (dvenc.on) dvenc.pack(ws, num_sms);
     else {
-      if (other_embedder()) unet.check(d);   // neither a U-Net nor a HiDDeN embedder: the U-Net's rules fail
+      if (other_embedder()) unet.check(d);   // neither a U-Net nor a HiDDeN / DVMark embedder: the U-Net's rules fail
       unet.pack(ws, num_sms);
     }
     if (hdec.on) hdec.pack(ws, num_sms);
@@ -191,7 +210,8 @@ class Model {
   // many different clip / tail lengths would otherwise accumulate up to 64 arenas of up to 2.3 GB each (a temporal U-Net's embed plan
   // holds one more buffer, its time-stacked operand: B * S^2 * temporal_stack_width(z0) fp16 values, 512 MiB at 64 x 256^2 and
   // 4.5 GiB at 64 x 768^2; and its plans are also keyed by the group length; a DVMark detect plan holds three maps, 40 KiB * S^2 in all at
-  // 64 frames, and at most 512 MiB of time-stacked operand: 3 GiB at 64 x 256^2, 23 GiB at 64 x 768^2).  The least recently used plan
+  // 64 frames, and at most 512 MiB of time-stacked operand: 3 GiB at 64 x 256^2, 23 GiB at 64 x 768^2; a DVMark embed plan about 1.9 KiB per
+  // processing pixel with the same stack budget: 8.6 GB at 64 x 256^2, 33 GB at 64 x 512^2, DVMarkEnc::build).  The least recently used plan
   // is dropped (its cudaFree calls synchronise the device, so work still in flight on it completes first).
   uint64_t plan_clock = 0;
   int max_plans = [] { const char* e = getenv("VSB_MAX_PLANS"); const int v = e ? atoi(e) : 8; return v < 2 ? 2 : v; }();
@@ -213,14 +233,16 @@ class Model {
     }
     return ret;
   }
-  // embed plans are keyed by B + kPlanGroup * G: a temporal U-Net's plan also depends on its group length G (0 for a 2-D U-Net)
+  // embed plans are keyed by B + kPlanGroup * G: the plan of a temporal U-Net or a DVMark embedder also depends on its group length
+  // G (0 for the others)
   static constexpr int kPlanGroup = 128;
   void build_embed_plan(Plan& pl, int key) {
-    if (!henc.on) { unet.build(pl, key % kPlanGroup, key / kPlanGroup); return; }
-    const int S = d.img_size;
-    pl.x_res = pl.pool.alloc_n<float>((size_t)key * 3 * S * S);
-    pl.tap("x_res", pl.x_res, 0, key, 3, S, S, S);
-    henc.build(pl, key, S, keep_inputs);
+    if (!henc.on && !dvenc.on) { unet.build(pl, key % kPlanGroup, key / kPlanGroup); return; }
+    const int S = d.img_size, B = key % kPlanGroup;
+    pl.x_res = pl.pool.alloc_n<float>((size_t)B * 3 * S * S);
+    pl.tap("x_res", pl.x_res, 0, B, 3, S, S, S);
+    if (dvenc.on) dvenc.build(pl, B, key / kPlanGroup, S, keep_inputs);
+    else henc.build(pl, B, S, keep_inputs);
   }
   // detect plans are keyed by B + kPlanGroup * G: a DVMark extractor's plan also depends on its group length G (0 for the others)
   void build_detect_plan(Plan& pl, int key) {
@@ -235,12 +257,14 @@ class Model {
     dec.build(pl, B, m, vit.on ? "vit." : "cnx.", d.nbits, num_sms);
   }
   Plan* get_embed_plan(int B, int G) { return get_plan(embed_plans, B + kPlanGroup * G, &Model::build_embed_plan); }
-  // a temporal U-Net convolves across a group of chunk_keys key frames (one reference embedder call), which must fit one sub-batch
+  // a temporal U-Net or a DVMark embedder convolves across a group of chunk_keys key frames (one reference embedder call), which
+  // must fit one sub-batch
   int temporal_group(int chunk_keys) const {
-    if (!unet.temporal) return 0;
-    VSB_CHECK(chunk_keys >= 1, "a temporal U-Net needs chunk_keys >= 1 (key frames per embedder call)");
+    if (!frame_mixing_embedder()) return 0;
+    const std::string what = dvenc.on ? "DVMark embedder" : "temporal U-Net";
+    VSB_CHECK(chunk_keys >= 1, "a " + what + " needs chunk_keys >= 1 (key frames per embedder call)");
     if (chunk_keys > kMaxBatch)
-      throw Error("temporal U-Net: a group of " + std::to_string(chunk_keys) + " frames convolved together (one video chunk, or the "
+      throw Error(what + ": a group of " + std::to_string(chunk_keys) + " frames convolved together (one video chunk, or the "
                   "whole batch in image mode) does not fit one " + std::to_string(kMaxBatch) + "-frame sub-batch; at most " +
                   std::to_string(kMaxBatch) + " are implemented", kErrUnsupported);
     return chunk_keys;
@@ -325,9 +349,9 @@ class Model {
     }
   }
   // frames that must stay in one batch: a key frame and its step - 1 followers, or in 'interpolate' mode, where neighbouring keys
-  // of one reference chunk are mixed, and for a temporal U-Net, which convolves across them, whole chunks
+  // of one reference chunk are mixed, and for a temporal U-Net or a DVMark embedder, which convolve across them, whole chunks
   int key_unit(int step, int video_mode, int chunk_keys) const {
-    if (unet.temporal) return step * temporal_group(chunk_keys);
+    if (frame_mixing_embedder()) return step * temporal_group(chunk_keys);
     return (video_mode == VSB_VIDEO_INTERPOLATE && step > 1) ? step * std::max(1, chunk_keys) : step;
   }
   void embed_detect_host(const float* imgs_h, const uint8_t* msgs_h, int n_msgs, float* imgs_w_h, float* logits_h, int F, int H, int W,

@@ -110,6 +110,15 @@ int vsb_model_set_hidden_extractor(vsb_model* m, const vsb_hidden_desc* h) {
   VSB_API_END
 }
 
+int vsb_model_set_dvmark_embedder(vsb_model* m, int32_t nbits) {
+  VSB_API_BEGIN
+  VSB_CHECK(m != nullptr, "null argument");
+  std::lock_guard<std::recursive_mutex> lk(m->impl.mu);
+  m->impl.set_dvmark_embedder(nbits);
+  return VSB_OK;
+  VSB_API_END
+}
+
 int vsb_model_set_dvmark_extractor(vsb_model* m, int32_t nbits) {
   VSB_API_BEGIN
   VSB_CHECK(m != nullptr, "null argument");

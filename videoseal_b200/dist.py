@@ -33,7 +33,7 @@ def shard_bounds(num_frames: int, world_size: int, step_size: int = 1) -> List[T
 
 def shard_unit(model) -> int:
     """The `step_size` to shard a clip for `model` with: frames that one embed call must see together.  That is a key frame and
-    its step_size - 1 followers, or, for a temporal U-Net, whose 3x3x3 convs mix the key frames of one reference chunk
+    its step_size - 1 followers, or, for a temporal U-Net or a DVMark embedder, whose 3x3x3 convs mix the key frames of one reference chunk
     (models/videoseal.py:292-320), whole chunks of chunk_size * step_size frames.  A DVMark extractor mixes the frames of one
     detect chunk (videoseal.py:373-379), so its shards also hold whole chunks of chunk_size frames."""
     step = int(model.step_size)

@@ -56,7 +56,7 @@ def native_desc(spec: dict) -> _lib.ModelDesc:
     """vsb_model_desc of `spec` (cfg.spec_from_card)"""
     d = _lib.ModelDesc()
     d.nbits, d.hidden, d.img_size, d.yuv = spec["nbits"], spec["hidden"], spec["img_size"], int(spec["yuv"])
-    u = spec.get("unet")          # a HiDDeN embedder spec leaves the U-Net fields zero but its RGB channels
+    u = spec.get("unet")          # a HiDDeN or DVMark embedder spec leaves the U-Net fields zero but its RGB channels
     if u is None:
         d.unet_in_ch, d.unet_out_ch = 3, 3
     else:
@@ -102,7 +102,7 @@ def native_hidden_desc(h: dict, embedder: bool) -> _lib.HiddenDesc:
 
 
 def delta_channels(spec: dict) -> int:
-    """channels of the embedder's output (the U-Net's out_channels; 3 for a HiDDeN encoder)"""
+    """channels of the embedder's output (the U-Net's out_channels; 3 for a HiDDeN or DVMark encoder)"""
     return spec["unet"]["out_channels"] if "unet" in spec else 3
 
 
@@ -117,10 +117,10 @@ def trunk_map(spec: dict) -> int:
 
 def _create(spec: dict):
     """Native handle of `spec` without weights or a device.  vsb_model_create, vsb_model_set_unet_temporal,
-    vsb_model_set_hidden_embedder / _extractor, vsb_model_set_dvmark_extractor, vsb_model_set_vit_extractor and vsb_model_set_pixel_decoder check every rule the kernels place on the model's geometry; a
+    vsb_model_set_hidden_embedder / _extractor, vsb_model_set_dvmark_embedder / _extractor, vsb_model_set_vit_extractor and vsb_model_set_pixel_decoder check every rule the kernels place on the model's geometry; a
     model they do not implement raises NotImplementedError."""
     L = _lib.lib()
-    if "hidden_encoder" not in spec and not spec["unet"]["z"]:
+    if "hidden_encoder" not in spec and "dvmark_encoder" not in spec and not spec["unet"]["z"]:
         # the descriptor of a U-Net without levels looks like one a HiDDeN embedder completes: reject it here, at load
         raise RuntimeError("libvsb200 error -1: unet levels: a U-Net needs 2 to 6 levels (z_channels_mults is empty)")
     h = C.c_void_p()
@@ -130,6 +130,8 @@ def _create(spec: dict):
     rc = L.vsb_model_set_unet_temporal(h, 1) if spec.get("unet", {}).get("temporal", False) else 0
     if rc == 0 and "hidden_encoder" in spec:
         rc = L.vsb_model_set_hidden_embedder(h, C.byref(native_hidden_desc(spec["hidden_encoder"], True)))
+    if rc == 0 and "dvmark_encoder" in spec:
+        rc = L.vsb_model_set_dvmark_embedder(h, int(spec["dvmark_encoder"]["nbits"]))
     if rc == 0 and "hidden_decoder" in spec:
         rc = L.vsb_model_set_hidden_extractor(h, C.byref(native_hidden_desc(spec["hidden_decoder"], False)))
     if rc == 0 and "dvmark_decoder" in spec:
@@ -334,7 +336,7 @@ class Videoseal(nn.Module):
         try:
             temporal, dvmark = self.temporal, self.dvmark
             for k, v in self._sd.items():
-                # 5-D tensors: only the Conv3d weights of a temporal U-Net and of a DVMark extractor are read
+                # 5-D tensors: only the Conv3d weights of a temporal U-Net or a DVMark embedder and of a DVMark extractor are read
                 if k.startswith(("attenuation.", "rgb2yuv.")) or (v.dim() > 4 and not (temporal and k.startswith("embedder.unet."))
                                                                    and not (dvmark and k.startswith("detector.layers."))):
                     continue
@@ -410,17 +412,19 @@ class Videoseal(nn.Module):
 
     @property
     def temporal(self) -> bool:
-        """True for a temporal U-Net (unet.conv_layer 'conv3d'): its 3x3x3 convs mix the key frames of one embedder call"""
-        return bool(self.spec.get("unet", {}).get("temporal", False))
+        """True when the embedder's 3x3x3 convs mix the key frames of one embedder call: a temporal U-Net (unet.conv_layer
+        'conv3d') or a DVMark embedder"""
+        return bool(self.spec.get("unet", {}).get("temporal", False)) or "dvmark_encoder" in self.spec
 
     def _chunk_keys(self, is_video: bool, num_frames: int) -> int:
         """vsb_embed's chunk_keys: key frames per reference embedder call.  A video call is one chunk of chunk_size key frames
         (videoseal.py:292-320); in image mode the whole batch is one call (wam.py:134-204), which matters only to a temporal
-        U-Net.  A temporal group must fit one 64-frame sub-batch."""
+        U-Net or a DVMark embedder.  A temporal group must fit one 64-frame sub-batch."""
         keys = int(self.chunk_size) if is_video or not self.temporal else int(num_frames)
         if self.temporal and keys > 64:
             what = f"chunk_size={keys}" if is_video else f"image mode with {keys} images"
-            raise NotImplementedError(f"temporal U-Net: {what} puts more than 64 frames in one 3x3x3 conv group; at most 64 are "
+            net = "DVMark embedder" if "dvmark_encoder" in self.spec else "temporal U-Net"
+            raise NotImplementedError(f"{net}: {what} puts more than 64 frames in one 3x3x3 conv group; at most 64 are "
                                       "implemented")
         return keys
 
