@@ -166,6 +166,32 @@ int vsb_model_set_dvmark_extractor(vsb_model* m, int32_t nbits);
  * the descriptor's (any nbits >= 1 is implemented); VSB_ERR_UNSUPPORTED for an img_size that is not a positive multiple of 128 or
  * is above 512.  vsb_embed groups its key frames as for a temporal U-Net: at most 64 per group (chunk_keys). */
 int vsb_model_set_dvmark_embedder(vsb_model* m, int32_t nbits);
+/* VAE embedder (modules/vae.py VAEEncoder / VAEDecoder, modules/msg_processor.py 'binary+concat'; models/embedder.py VAEEmbedder,
+ * build_embedder 'vae*'): decoder(msg_processor(encoder(2 imgs - 1), msgs)), 'yuv' cards on x = 2 Y - 1.  Levels of widths
+ * ch * ch_mult[l] at S / 2^l; ResnetBlocks out = shortcut(x) + conv2(silu(GN2(conv1(silu(GN1(x)))))), GN = GroupNorm(16, C, eps 1e-6),
+ * shortcut the identity or the 1x1 nin_shortcut; Downsample pad (0,1,0,1) + 3x3 stride 2; Upsample nearest x2 + 3x3; mid ResnetBlock,
+ * single-head AttnBlock over the whole deepest grid (head dim = last width), ResnetBlock; encoder conv_out -> z_channels; the message
+ * as hidden = nbits * hidden_size_multiplier constant planes sum_k E[2k + m_k] after the latent; decoder conv_out -> out_ch, tanh
+ * when tanh_out: the delta (out_ch channels).  Checkpoint keys embedder.encoder.*, embedder.decoder.*,
+ * embedder.msg_processor.msg_embeddings.weight.  It replaces the U-Net like the HiDDeN embedder: unet_levels 0, unet_in_ch =
+ * unet_out_ch = 3 (else VSB_ERR_INVALID); its own channels travel in the descriptor. */
+typedef struct vsb_vae_desc {
+  int32_t in_ch;             /* encoder in_channels: 3, or 1 for the 'yuv' cards (then the descriptor's yuv is 1) */
+  int32_t out_ch;            /* decoder out_ch: channels of the delta */
+  int32_t ch;                /* base width */
+  int32_t levels;            /* len(ch_mult), 1..6 */
+  int32_t ch_mult[6];
+  int32_t num_res_blocks;    /* encoder blocks per level (the decoder has num_res_blocks + 1) */
+  int32_t z_channels;        /* encoder latent channels (double_z false) */
+  int32_t tanh_out;          /* decoder tanh */
+} vsb_vae_desc;
+/* Called after vsb_model_create and before finalize; no CUDA call.  VSB_ERR_STATE after finalize or when the model already has a
+ * HiDDeN, DVMark or temporal U-Net embedder.  VSB_ERR_INVALID for a descriptor that describes a U-Net, yuv != (in_ch == 1), in_ch
+ * other than 1 / 3, levels outside 1..6, num_res_blocks outside 1..8, tanh_out other than 0 / 1 or non-positive widths.
+ * VSB_ERR_UNSUPPORTED unless: every level width (and ch) is 16, 32, 64 or 128; the last-level width (the attention head dim) is 64
+ * or 128; z_channels <= 16; out_ch 1 or 3; img_size a multiple of 128, at most 768, whose deepest map img_size / 2^(levels - 1)
+ * is a whole multiple of 16 pixels and at most 96 (the attention's 9 216 tokens). */
+int vsb_model_set_vae_embedder(vsb_model* m, const vsb_vae_desc* vae);
 /* fold BN, pack to fp16 KRSC, upload to `device`, build nothing else (plans are built lazily per batch shape) */
 int vsb_model_finalize(vsb_model* m, int32_t device);
 void vsb_model_destroy(vsb_model* m);

@@ -17,7 +17,7 @@ EXPORTS = [
     "vsb_debug_resample_table", "vsb_debug_resample_table2", "vsb_debug_last_dispatch", "vsb_quality_workspace_bytes", "vsb_ssim", "vsb_model_set_vit_extractor",
     "vsb_augment_workspace_bytes", "vsb_augment", "vsb_model_set_unet_temporal", "vsb_model_set_hidden_embedder",
     "vsb_model_set_hidden_extractor", "vsb_model_set_dvmark_extractor", "vsb_detect_grouped",
-    "vsb_model_set_dvmark_embedder",
+    "vsb_model_set_dvmark_embedder", "vsb_model_set_vae_embedder",
 ]
 
 FLAG_CLAMP, FLAG_LOWRES_ATTN, FLAG_NO_ATTENUATION, FLAG_RESIZE_NO_AA = 1, 2, 4, 8
@@ -47,6 +47,11 @@ class VitDesc(C.Structure):
 
 class HiddenDesc(C.Structure):
     _fields_ = [("z_channels", C.c_int32), ("num_layers", C.c_int32), ("norm", C.c_int32), ("act", C.c_int32), ("last_tanh", C.c_int32)]
+
+
+class VaeDesc(C.Structure):
+    _fields_ = [("in_ch", C.c_int32), ("out_ch", C.c_int32), ("ch", C.c_int32), ("levels", C.c_int32), ("ch_mult", C.c_int32 * 6),
+                ("num_res_blocks", C.c_int32), ("z_channels", C.c_int32), ("tanh_out", C.c_int32)]
 
 
 class ConvTest(C.Structure):
@@ -89,6 +94,7 @@ def lib():
     L.vsb_model_set_hidden_extractor.argtypes = [C.c_void_p, C.POINTER(HiddenDesc)]
     L.vsb_model_set_dvmark_extractor.argtypes = [C.c_void_p, C.c_int32]
     L.vsb_model_set_dvmark_embedder.argtypes = [C.c_void_p, C.c_int32]
+    L.vsb_model_set_vae_embedder.argtypes = [C.c_void_p, C.POINTER(VaeDesc)]
     L.vsb_model_finalize.argtypes = [C.c_void_p, C.c_int32]
     L.vsb_model_destroy.argtypes = [C.c_void_p]
     L.vsb_model_destroy.restype = None

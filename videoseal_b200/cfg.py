@@ -70,8 +70,8 @@ def spec_from_card(card: dict) -> dict:
     img_size = a["img_size_proc"] if "img_size_proc" in a else a["img_size_extractor"]
     emb_name = str(card["embedder"]["model"])
     ext_name = str(card["extractor"]["model"])
-    if not emb_name.startswith(("unet", "hidden", "dvmark")):
-        raise NotImplementedError(f"embedder '{emb_name}': only the unet*, hidden* and dvmark* families are on the CUDA hot path")
+    if not emb_name.startswith(("unet", "hidden", "dvmark", "vae")):
+        raise NotImplementedError(f"embedder '{emb_name}': only the unet*, hidden*, dvmark* and vae* families are on the CUDA hot path")
     is_vit = ext_name.startswith("sam")
     if not (ext_name.startswith(("convnext", "hidden", "dvmark")) or is_vit):
         raise NotImplementedError(f"extractor '{ext_name}': only the convnext*, sam*, hidden* and dvmark* families are on the CUDA hot "
@@ -83,6 +83,8 @@ def spec_from_card(card: dict) -> dict:
     elif emb_name.startswith("dvmark"):
         # build_embedder: DVMarkEmbedder(DVMarkEncoder(nbits)); the preset has no parameters (params: [])
         embedder = {"dvmark_encoder": {"nbits": nbits}}
+    elif emb_name.startswith("vae"):
+        embedder = {"vae_encoder": _vae(card["embedder"]["params"], emb_name)}
     else:
         embedder = _unet(card["embedder"]["params"])
     if ext_name.startswith("hidden"):
@@ -135,6 +137,37 @@ def _hidden(p: dict, embedder: bool) -> dict:
     if embedder:
         h["last_tanh"] = bool(p.get("last_tanh", True))
     return h
+
+
+def _vae(p: dict, name: str) -> dict:
+    """spec['vae_encoder'] of a vae* embedder (embedder.py:245-254, modules/vae.py VAEEncoder / VAEDecoder).  The decoder's
+    z_channels is set by build_embedder (z + hidden); the encoder's out_ch, resolution and dropout do nothing in eval."""
+    enc, dec, mp = p["encoder"], p["decoder"], p.get("msg_processor", {})
+    if mp.get("msg_processor_type", "binary+concat") != "binary+concat":
+        raise NotImplementedError("VAE embedder: only the 'binary+concat' message processor is implemented")
+    if float(mp.get("msg_mult", 1.0)) != 1.0:
+        raise NotImplementedError("VAE embedder: msg_mult other than 1 is not implemented")
+    for part, c in (("encoder", enc), ("decoder", dec)):
+        if list(c.get("attn_resolutions", [])):
+            raise NotImplementedError(f"VAE {part}: attention blocks inside levels (attn_resolutions) are not implemented")
+        if c.get("use_linear_attn", False) or str(c.get("attn_type", "vanilla")) != "vanilla":
+            raise NotImplementedError(f"VAE {part}: only the vanilla AttnBlock is implemented (no linear attention)")
+        if not c.get("resamp_with_conv", True):
+            raise NotImplementedError(f"VAE {part}: resamp_with_conv=False (conv-less resampling) is not implemented")
+    if enc.get("double_z", True):
+        # the VAEEncoder default; build_embedder sizes the decoder for z_channels latent channels, so 2 z cannot be built
+        raise NotImplementedError("VAE encoder: double_z=True is not implemented (build_embedder's channel arithmetic needs False)")
+    if dec.get("give_pre_end", False):
+        raise NotImplementedError("VAE decoder: give_pre_end=True is not implemented")
+    if dec.get("bw", False):
+        raise NotImplementedError("VAE decoder: bw=True is not implemented")
+    mult = [int(m) for m in enc["ch_mult"]]
+    if [int(m) for m in dec["ch_mult"]] != mult or int(dec["ch"]) != int(enc["ch"]) or \
+            int(dec["num_res_blocks"]) != int(enc["num_res_blocks"]):
+        raise NotImplementedError("VAE embedder: an encoder and decoder of different ch / ch_mult / num_res_blocks are not implemented")
+    return {"in_channels": int(enc["in_channels"]), "out_ch": int(dec["out_ch"]), "ch": int(enc["ch"]), "ch_mult": mult,
+            "num_res_blocks": int(enc["num_res_blocks"]), "z_channels": int(enc["z_channels"]),
+            "tanh_out": bool(dec.get("tanh_out", False))}
 
 
 def _unet(ep: dict) -> dict:

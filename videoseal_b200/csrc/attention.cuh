@@ -11,7 +11,7 @@
 namespace vsb {
 
 constexpr int kVitPatch = 16;
-constexpr int kAttnHd = 64;      // head dim (the only one implemented)
+constexpr int kAttnHd = 64;      // head dim of the SAM-ViT heads (the VAE's single head also runs at 128)
 constexpr int kAttnTile = 64;    // queries per CTA and keys per online-softmax tile
 constexpr int kAttnLds = 72;     // shared row pitch in halves: 36 words, so the 32-bit fragment loads of a warp hit 32 banks
 constexpr int kAttnTp = 65;      // row pitch (floats) of the per-warp relative-position products
@@ -72,8 +72,10 @@ __device__ __forceinline__ uint32_t attn_pack(float lo, float hi) {
 }
 __device__ __forceinline__ uint32_t ld32(const __half* p) { return *reinterpret_cast<const uint32_t*>(p); }
 
-inline size_t attn_smem_bytes(bool rel) {
-  return (size_t)(rel ? 5 : 3) * kAttnTile * kAttnLds * sizeof(__half) + (rel ? (size_t)4 * 2 * 16 * kAttnTp * sizeof(float) : 0);
+// the q and k tiles have a row pitch of HD + 8 halves at head dim HD, so that the 32-bit fragment loads of a warp hit 32 banks
+inline size_t attn_smem_bytes(bool rel, int hd = kAttnHd) {
+  return (size_t)2 * kAttnTile * (hd + 8) * sizeof(__half) + (size_t)hd * kAttnLds * sizeof(__half) +
+         (rel ? (size_t)2 * kAttnTile * kAttnLds * sizeof(__half) + (size_t)4 * 2 * 16 * kAttnTp * sizeof(float) : 0);
 }
 
 // K7c (vit.py:302-353 Attention.forward, :431-470 add_decomposed_rel_pos).  Grid (B * regions * heads, n*n / 64), 4 warps; warp w
@@ -81,14 +83,17 @@ inline size_t attn_smem_bytes(bool rel) {
 // Tensor cores (mma.m16n8k16, fp16 operands, fp32 accumulators) compute q k^T, and with REL q Rh^T / q Rw^T over the 2n-1 table
 // rows with the UNSCALED q as in the reference; each score then gathers Th[q, qh-kh+n-1] + Tw[q, qw-kw+n-1].  Softmax in fp32,
 // online over 64-key tiles; P is rounded to fp16 for P v and the rows are normalised at the end.  No atomics: a token's output
-// depends only on its own region's rows.
-template <bool REL>
+// depends only on its own region's rows.  HD: head dim, 64 (SAM-ViT; with or without REL) or 128 (the VAE's AttnBlock, no REL); the
+// key loop does not bound the token count.
+template <bool REL, int HD = kAttnHd>
 __global__ void __launch_bounds__(128) vit_attention_kernel(const AttnParams p) {
+  static_assert(HD == 64 || (HD == 128 && !REL), "attention: head dim 64, or 128 without relative positions");
+  constexpr int LDQ = HD + 8, KS = HD / 16, ND = HD / 8, NDS = HD == 64 ? 3 : 4;   // q / k pitch, k-steps, 8-wide dim tiles (2^NDS)
   extern __shared__ __align__(16) unsigned char attn_smem[];
-  __half* sQ = reinterpret_cast<__half*>(attn_smem);   // [64 queries][72]
-  __half* sK = sQ + kAttnTile * kAttnLds;                // [64 keys][72]
-  __half* sVt = sK + kAttnTile * kAttnLds;               // [64 dims][72 keys]: v transposed, the B operand of P v
-  __half* sRh = sVt + kAttnTile * kAttnLds;              // [64 table rows][72] (REL)
+  __half* sQ = reinterpret_cast<__half*>(attn_smem);   // [64 queries][LDQ]
+  __half* sK = sQ + kAttnTile * LDQ;                     // [64 keys][LDQ]
+  __half* sVt = sK + kAttnTile * LDQ;                    // [HD dims][72 keys]: v transposed, the B operand of P v
+  __half* sRh = sVt + HD * kAttnLds;                     // [64 table rows][72] (REL)
   __half* sRw = sRh + kAttnTile * kAttnLds;
   float* sT = reinterpret_cast<float*>(sRw + kAttnTile * kAttnLds);   // [warp][h/w][16][kAttnTp] (REL)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
@@ -103,26 +108,26 @@ __global__ void __launch_bounds__(128) vit_attention_kernel(const AttnParams p) 
   const int q0 = blockIdx.y * kAttnTile;
   const int ld = 3 * p.E;
   auto row_of = [&](int tok) -> long { return (frame * p.G + ry0 + tok / n) * p.G + rx0 + tok % n; };
-  const int qcol = head * kAttnHd, kcol = p.E + head * kAttnHd, vcol = 2 * p.E + head * kAttnHd;
+  const int qcol = head * HD, kcol = p.E + head * HD, vcol = 2 * p.E + head * HD;
 
-  for (int i = threadIdx.x; i < kAttnTile * 8; i += 128) {
-    const int r = i >> 3, c = (i & 7) * 8;
-    *reinterpret_cast<uint4*>(sQ + r * kAttnLds + c) = *reinterpret_cast<const uint4*>(p.qkv + row_of(q0 + r) * ld + qcol + c);
+  for (int i = threadIdx.x; i < kAttnTile * ND; i += 128) {
+    const int r = i >> NDS, c = (i & (ND - 1)) * 8;
+    *reinterpret_cast<uint4*>(sQ + r * LDQ + c) = *reinterpret_cast<const uint4*>(p.qkv + row_of(q0 + r) * ld + qcol + c);
     if (REL) {
       *reinterpret_cast<uint4*>(sRh + r * kAttnLds + c) = *reinterpret_cast<const uint4*>(p.rel_h + r * kAttnHd + c);
       *reinterpret_cast<uint4*>(sRw + r * kAttnLds + c) = *reinterpret_cast<const uint4*>(p.rel_w + r * kAttnHd + c);
     }
   }
   __syncthreads();
-  uint32_t qa[4][4];   // A fragments of the warp's 16 query rows over the 4 k-steps of the head dim
+  uint32_t qa[KS][4];   // A fragments of the warp's 16 query rows over the KS k-steps of the head dim
   {
-    const __half* qb = sQ + warp * 16 * kAttnLds;
+    const __half* qb = sQ + warp * 16 * LDQ;
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      qa[kk][0] = ld32(qb + g * kAttnLds + kk * 16 + 2 * t);
-      qa[kk][1] = ld32(qb + (g + 8) * kAttnLds + kk * 16 + 2 * t);
-      qa[kk][2] = ld32(qb + g * kAttnLds + kk * 16 + 8 + 2 * t);
-      qa[kk][3] = ld32(qb + (g + 8) * kAttnLds + kk * 16 + 8 + 2 * t);
+    for (int kk = 0; kk < KS; ++kk) {
+      qa[kk][0] = ld32(qb + g * LDQ + kk * 16 + 2 * t);
+      qa[kk][1] = ld32(qb + (g + 8) * LDQ + kk * 16 + 2 * t);
+      qa[kk][2] = ld32(qb + g * LDQ + kk * 16 + 8 + 2 * t);
+      qa[kk][3] = ld32(qb + (g + 8) * LDQ + kk * 16 + 8 + 2 * t);
     }
   }
   const int qi0 = q0 + warp * 16 + g, qi1 = qi0 + 8;
@@ -134,7 +139,7 @@ __global__ void __launch_bounds__(128) vit_attention_kernel(const AttnParams p) 
     for (int j = 0; j < nt; ++j) {
       float ch[4] = {0.f, 0.f, 0.f, 0.f}, cw[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
+      for (int kk = 0; kk < KS; ++kk) {
         const __half* rh = sRh + (j * 8 + g) * kAttnLds + kk * 16 + 2 * t;
         const __half* rw = sRw + (j * 8 + g) * kAttnLds + kk * 16 + 2 * t;
         attn_mma(ch, qa[kk], ld32(rh), ld32(rh + 8));
@@ -150,15 +155,15 @@ __global__ void __launch_bounds__(128) vit_attention_kernel(const AttnParams p) 
   }
 
   float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
-  float o[8][4];
+  float o[ND][4];
 #pragma unroll
-  for (int j = 0; j < 8; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
+  for (int j = 0; j < ND; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
   for (int k0 = 0; k0 < T; k0 += kAttnTile) {
     __syncthreads();   // every warp is done with the previous key tile
-    for (int i = threadIdx.x; i < kAttnTile * 8; i += 128) {
-      const int r = i >> 3, c = (i & 7) * 8;
+    for (int i = threadIdx.x; i < kAttnTile * ND; i += 128) {
+      const int r = i >> NDS, c = (i & (ND - 1)) * 8;
       const __half* src = p.qkv + row_of(k0 + r) * ld;
-      *reinterpret_cast<uint4*>(sK + r * kAttnLds + c) = *reinterpret_cast<const uint4*>(src + kcol + c);
+      *reinterpret_cast<uint4*>(sK + r * LDQ + c) = *reinterpret_cast<const uint4*>(src + kcol + c);
       __align__(16) __half v[8];
       *reinterpret_cast<uint4*>(v) = *reinterpret_cast<const uint4*>(src + vcol + c);
 #pragma unroll
@@ -169,16 +174,17 @@ __global__ void __launch_bounds__(128) vit_attention_kernel(const AttnParams p) 
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
-      const __half* kb = sK + (j * 8 + g) * kAttnLds + 2 * t;
+      const __half* kb = sK + (j * 8 + g) * LDQ + 2 * t;
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) attn_mma(s[j], qa[kk], ld32(kb + kk * 16), ld32(kb + kk * 16 + 8));
+      for (int kk = 0; kk < KS; ++kk) attn_mma(s[j], qa[kk], ld32(kb + kk * 16), ld32(kb + kk * 16 + 8));
     }
     float mx0 = m0, mx1 = m1;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        float v = s[j][e] * p.scale;   // == (q * scale) k^T exactly: scale is a power of two at head dim 64
+        // == (q * scale) k^T exactly when scale is a power of two (head dim 64); the VAE scales the product (vae.py AttnBlock)
+        float v = s[j][e] * p.scale;
         if (REL) {
           const int key = k0 + j * 8 + 2 * t + (e & 1), kh = key / n, kw = key % n;
           const int r = e < 2 ? g : g + 8, qh = e < 2 ? qh0 : qh1, qw = e < 2 ? qw0 : qw1;
@@ -197,7 +203,7 @@ __global__ void __launch_bounds__(128) vit_attention_kernel(const AttnParams p) 
     m0 = mx0; m1 = mx1;
     l0 *= a0; l1 *= a1;
 #pragma unroll
-    for (int j = 0; j < 8; ++j) { o[j][0] *= a0; o[j][1] *= a0; o[j][2] *= a1; o[j][3] *= a1; }
+    for (int j = 0; j < ND; ++j) { o[j][0] *= a0; o[j][1] *= a0; o[j][2] *= a1; o[j][3] *= a1; }
     uint32_t pa[4][4];   // P as the A operand of P v: the accumulator layout of two key n-tiles is one k-step's A fragment
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -207,7 +213,7 @@ __global__ void __launch_bounds__(128) vit_attention_kernel(const AttnParams p) 
       pa[j >> 1][(j & 1) * 2 + 1] = attn_pack(p2, p3);
     }
 #pragma unroll
-    for (int jd = 0; jd < 8; ++jd) {
+    for (int jd = 0; jd < ND; ++jd) {
       const __half* vb = sVt + (jd * 8 + g) * kAttnLds + 2 * t;
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) attn_mma(o[jd], pa[kk], ld32(vb + kk * 16), ld32(vb + kk * 16 + 8));
@@ -218,10 +224,10 @@ __global__ void __launch_bounds__(128) vit_attention_kernel(const AttnParams p) 
   l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
   l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
   const float i0 = 1.0f / l0, i1 = 1.0f / l1;
-  __half* out0 = p.out + row_of(qi0) * p.E + head * kAttnHd + 2 * t;
-  __half* out1 = p.out + row_of(qi1) * p.E + head * kAttnHd + 2 * t;
+  __half* out0 = p.out + row_of(qi0) * p.E + head * HD + 2 * t;
+  __half* out1 = p.out + row_of(qi1) * p.E + head * HD + 2 * t;
 #pragma unroll
-  for (int jd = 0; jd < 8; ++jd) {
+  for (int jd = 0; jd < ND; ++jd) {
     *reinterpret_cast<__half2*>(out0 + jd * 8) = __floats2half2_rn(o[jd][0] * i0, o[jd][1] * i0);
     *reinterpret_cast<__half2*>(out1 + jd * 8) = __floats2half2_rn(o[jd][2] * i1, o[jd][3] * i1);
   }

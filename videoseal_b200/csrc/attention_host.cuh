@@ -21,13 +21,18 @@ inline void launch_vit_pos_add(float* x, long M, int P, int E, const float* tabl
   VSB_CUDA(cudaGetLastError());
 }
 
-// B frames of a G x G token grid, attention over n x n regions (n = G: global)
+// B frames of a G x G token grid, attention over n x n regions (n = G: global); head dim HD (128: no relative positions)
+template <int HD = kAttnHd>
 inline void launch_vit_attention(AttnParams p, int B, cudaStream_t st) {
   const dim3 grid((unsigned)(B * p.regions * p.heads), (unsigned)(p.n * p.n / kAttnTile));
   const bool rel = p.rel_h != nullptr;
   VSB_CHECK(!rel || p.n <= kAttnMaxRelSide, "attention: relative positions over regions wider than 32 tokens");
-  const size_t smem = attn_smem_bytes(rel);
-  if (rel) {
+  const size_t smem = attn_smem_bytes(rel, HD);
+  if constexpr (HD != kAttnHd) {
+    VSB_CHECK(!rel, "attention: relative positions need head dim 64");
+    smem_optin<vit_attention_kernel<false, HD>>(smem);
+    vit_attention_kernel<false, HD><<<grid, 128, smem, st>>>(p);
+  } else if (rel) {
     smem_optin<vit_attention_kernel<true>>(smem);
     vit_attention_kernel<true><<<grid, 128, smem, st>>>(p);
   } else {

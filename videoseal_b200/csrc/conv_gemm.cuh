@@ -9,7 +9,7 @@
 //                       chunk (zero fill = conv padding) and the tap tiles are copied smem->smem into the 128-byte-swizzled
 //                       wgmma operand layout (input pixels cross L2->SM once instead of nine times)
 //       LD_GATHER_CONV: generic strided / reflect-padded conv gathered from global memory (stride-2 3x3, k2s2 patchify,
-//                       reflect-padded head conv)
+//                       reflect-padded head conv, the 3x3 conv of a nearest x2 up-sample read from the low-resolution map)
 //
 //   next 8 warps  : two MMA warpgroups; warpgroup h issues the wgmma of rows [64h, 64h + 64) of the tile
 //   last warp     : TMA producer (weights unless resident; activations for LD_TMA; input halo tiles for LD_HALO_CONV3)
@@ -89,7 +89,7 @@ struct ConvGemmParams {
   // ---- gather loaders (NHWC fp16 sources; K order = (r, s, c) with c over the virtual concat [src0 | src1])
   const __half* src0;
   const __half* src1;
-  int C0, C1, ld0, ld1, IH, IW, OH, OW, stride, pad_mode /*0 zero, 1 reflect*/, Ktot;
+  int C0, C1, ld0, ld1, IH, IW, OH, OW, stride, pad_mode /*0 zero, 1 reflect, 2 zero on the nearest x2 up-sample*/, Ktot;
   int rows_per_sample;            // GEMM rows per sample (GRN statistics, per-sample weights)
   int b_sample_rows;              // > 0: per-sample weights [samples][N][K] (GRN folded into pwconv2); = N
   FastDiv fd_tps;                 // M tiles per sample
@@ -1047,6 +1047,9 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               if (p.pad_mode == 1) {
                 iy = reflect_idx(iy, p.IH);
                 ix = reflect_idx(ix, p.IW);
+              } else if (p.pad_mode == 2) {   // zero padding around the nearest x2 up-sample of the 2x smaller source
+                ok = (iy >= 0) && (iy < 2 * p.IH) && (ix >= 0) && (ix < 2 * p.IW);
+                iy >>= 1; ix >>= 1;
               } else {
                 ok = (iy >= 0) && (iy < p.IH) && (ix >= 0) && (ix < p.IW);
               }

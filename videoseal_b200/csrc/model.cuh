@@ -12,6 +12,7 @@
 #include "hidden.cuh"
 #include "resize_blend_host.cuh"
 #include "unet.cuh"
+#include "vae.cuh"
 #include "vit_trunk.cuh"
 
 namespace vsb {
@@ -31,6 +32,7 @@ class Model {
   Hidden henc, hdec;   // HiDDeN embedder / extractor, in place of the U-Net / the trunk and decoder (vsb_model_set_hidden_*)
   DVMark dvdec;        // DVMark extractor, in place of the trunk and decoder (vsb_model_set_dvmark_extractor)
   DVMarkEnc dvenc;     // DVMark embedder, in place of the U-Net (vsb_model_set_dvmark_embedder)
+  VaeEnc vae;          // VAE embedder, in place of the U-Net (vsb_model_set_vae_embedder)
 
   // grow-only device staging for the host-buffer entry points (no cudaMalloc on the steady-state path)
   struct Staging { void* p = nullptr; size_t cap = 0; };
@@ -60,13 +62,13 @@ class Model {
   int32_t last_resize[5] = {-1, -1, -1, -1, -1};
   int32_t last_blend[5] = {-1, -1, -1, -1, -1};
   // test seam (vsb_debug_keep_inputs): detect plans (and HiDDeN embed plans) copy buffers that later steps overwrite aside; DVMark
-  // embed plans give every map a buffer of its own
+  // and VAE embed plans give every map a buffer of its own
   bool keep_inputs = false;
   void set_keep_inputs(bool on) {
     keep_inputs = on;
     for (auto& kv : detect_plans) if (kv.second.get() == last_plan) last_plan = nullptr;
     detect_plans.clear();
-    if (henc.on || dvenc.on) {   // HiDDeN and DVMark embed plans have the seam too (Hidden::build, DVMarkEnc::build)
+    if (henc.on || dvenc.on || vae.on) {   // HiDDeN, DVMark and VAE embed plans have the seam too (their build)
       for (auto& kv : embed_plans) if (kv.second.get() == last_plan) last_plan = nullptr;
       embed_plans.clear();
     }
@@ -82,17 +84,17 @@ class Model {
     ConvNeXt::check(d);
     if (!other_embedder()) unet.choose_kernels();
   }
-  // no U-Net levels but the embedder's RGB in / out channels: the embedder is set by vsb_model_set_hidden_embedder or
-  // vsb_model_set_dvmark_embedder
+  // no U-Net levels but the embedder's RGB in / out channels: the embedder is set by vsb_model_set_hidden_embedder,
+  // vsb_model_set_dvmark_embedder or vsb_model_set_vae_embedder
   bool other_embedder() const { return d.unet_levels == 0 && d.unet_in_ch == 3 && d.unet_out_ch == 3; }
   void check_unfinalized() const { if (finalized) throw Error("model already finalized", kErrState); }
   // channels of the embedder's output delta
-  int delta_ch() const { return (henc.on || dvenc.on) ? 3 : d.unet_out_ch; }
+  int delta_ch() const { return vae.on ? vae.v.out_ch : ((henc.on || dvenc.on) ? 3 : d.unet_out_ch); }
   // the embedder's 3x3x3 convs mix the key frames of one embedder call (a temporal U-Net or a DVMark embedder)
   bool frame_mixing_embedder() const { return unet.temporal || dvenc.on; }
   void set_hidden_embedder(const vsb_hidden_desc& h) {
     check_unfinalized();
-    if (dvenc.on) throw Error("vsb_model_set_hidden_embedder: the model already has a DVMark embedder", kErrState);
+    if (dvenc.on || vae.on) throw Error("vsb_model_set_hidden_embedder: the model already has a DVMark or VAE embedder", kErrState);
     if (!other_embedder())
       throw Error("vsb_model_set_hidden_embedder: the descriptor describes a U-Net (a HiDDeN embedder needs unet_levels 0 and unet_in_ch / "
                   "unet_out_ch 3)", kErrInvalid);
@@ -112,14 +114,25 @@ class Model {
   }
   void set_dvmark_embedder(int nbits) {
     check_unfinalized();
-    if (henc.on || unet.temporal)
-      throw Error("vsb_model_set_dvmark_embedder: the model already has a HiDDeN embedder or a temporal U-Net", kErrState);
+    if (henc.on || unet.temporal || vae.on)
+      throw Error("vsb_model_set_dvmark_embedder: the model already has a HiDDeN or VAE embedder or a temporal U-Net", kErrState);
     if (!other_embedder())
       throw Error("vsb_model_set_dvmark_embedder: the descriptor describes a U-Net (a DVMark embedder needs unet_levels 0 and "
                   "unet_in_ch / unet_out_ch 3)", kErrInvalid);
     DVMarkEnc e;
     e.set(nbits, d);
     dvenc = e;
+  }
+  void set_vae_embedder(const vsb_vae_desc& v) {
+    check_unfinalized();
+    if (henc.on || dvenc.on || unet.temporal)
+      throw Error("vsb_model_set_vae_embedder: the model already has a HiDDeN or DVMark embedder or a temporal U-Net", kErrState);
+    if (!other_embedder())
+      throw Error("vsb_model_set_vae_embedder: the descriptor describes a U-Net (a VAE embedder needs unet_levels 0 and "
+                  "unet_in_ch / unet_out_ch 3)", kErrInvalid);
+    VaeEnc e;
+    e.set(v, d);
+    vae = e;
   }
   void set_dvmark_extractor(int nbits) {
     check_unfinalized();
@@ -191,8 +204,9 @@ class Model {
     num_sms = prop.multiProcessorCount;
     if (henc.on) henc.pack(ws, num_sms);
     else if (dvenc.on) dvenc.pack(ws, num_sms);
+    else if (vae.on) vae.pack(ws, num_sms);
     else {
-      if (other_embedder()) unet.check(d);   // neither a U-Net nor a HiDDeN / DVMark embedder: the U-Net's rules fail
+      if (other_embedder()) unet.check(d);   // neither a U-Net nor a HiDDeN / DVMark / VAE embedder: the U-Net's rules fail
       unet.pack(ws, num_sms);
     }
     if (hdec.on) hdec.pack(ws, num_sms);
@@ -237,11 +251,12 @@ class Model {
   // G (0 for the others)
   static constexpr int kPlanGroup = 128;
   void build_embed_plan(Plan& pl, int key) {
-    if (!henc.on && !dvenc.on) { unet.build(pl, key % kPlanGroup, key / kPlanGroup); return; }
+    if (!henc.on && !dvenc.on && !vae.on) { unet.build(pl, key % kPlanGroup, key / kPlanGroup); return; }
     const int S = d.img_size, B = key % kPlanGroup;
     pl.x_res = pl.pool.alloc_n<float>((size_t)B * 3 * S * S);
     pl.tap("x_res", pl.x_res, 0, B, 3, S, S, S);
     if (dvenc.on) dvenc.build(pl, B, key / kPlanGroup, S, keep_inputs);
+    else if (vae.on) vae.build(pl, B, S, keep_inputs);
     else henc.build(pl, B, S, keep_inputs);
   }
   // detect plans are keyed by B + kPlanGroup * G: a DVMark extractor's plan also depends on its group length G (0 for the others)

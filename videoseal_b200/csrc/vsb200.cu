@@ -119,6 +119,15 @@ int vsb_model_set_dvmark_embedder(vsb_model* m, int32_t nbits) {
   VSB_API_END
 }
 
+int vsb_model_set_vae_embedder(vsb_model* m, const vsb_vae_desc* vae) {
+  VSB_API_BEGIN
+  VSB_CHECK(m != nullptr && vae != nullptr, "null argument");
+  std::lock_guard<std::recursive_mutex> lk(m->impl.mu);
+  m->impl.set_vae_embedder(*vae);
+  return VSB_OK;
+  VSB_API_END
+}
+
 int vsb_model_set_dvmark_extractor(vsb_model* m, int32_t nbits) {
   VSB_API_BEGIN
   VSB_CHECK(m != nullptr, "null argument");

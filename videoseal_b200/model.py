@@ -56,7 +56,7 @@ def native_desc(spec: dict) -> _lib.ModelDesc:
     """vsb_model_desc of `spec` (cfg.spec_from_card)"""
     d = _lib.ModelDesc()
     d.nbits, d.hidden, d.img_size, d.yuv = spec["nbits"], spec["hidden"], spec["img_size"], int(spec["yuv"])
-    u = spec.get("unet")          # a HiDDeN or DVMark embedder spec leaves the U-Net fields zero but its RGB channels
+    u = spec.get("unet")          # a HiDDeN, DVMark or VAE embedder spec leaves the U-Net fields zero but its RGB channels
     if u is None:
         d.unet_in_ch, d.unet_out_ch = 3, 3
     else:
@@ -101,12 +101,26 @@ def native_hidden_desc(h: dict, embedder: bool) -> _lib.HiddenDesc:
     return v
 
 
+def native_vae_desc(v: dict) -> _lib.VaeDesc:
+    """vsb_vae_desc of spec['vae_encoder'] (cfg.spec_from_card)"""
+    d = _lib.VaeDesc()
+    d.in_ch, d.out_ch, d.ch, d.levels = v["in_channels"], v["out_ch"], v["ch"], len(v["ch_mult"])
+    for i, m in enumerate(v["ch_mult"][:6]):
+        d.ch_mult[i] = m
+    d.num_res_blocks, d.z_channels, d.tanh_out = v["num_res_blocks"], v["z_channels"], int(v["tanh_out"])
+    return d
+
+
 def delta_channels(spec: dict) -> int:
-    """channels of the embedder's output (the U-Net's out_channels; 3 for a HiDDeN or DVMark encoder)"""
+    """channels of the embedder's output (the U-Net's or the VAE decoder's out channels; 3 for a HiDDeN or DVMark encoder)"""
+    if "vae_encoder" in spec:
+        return spec["vae_encoder"]["out_ch"]
     return spec["unet"]["out_channels"] if "unet" in spec else 3
 
 
 def embedder_in_channels(spec: dict) -> int:
+    if "vae_encoder" in spec:
+        return spec["vae_encoder"]["in_channels"]
     return spec["unet"]["in_channels"] if "unet" in spec else 3
 
 
@@ -117,10 +131,10 @@ def trunk_map(spec: dict) -> int:
 
 def _create(spec: dict):
     """Native handle of `spec` without weights or a device.  vsb_model_create, vsb_model_set_unet_temporal,
-    vsb_model_set_hidden_embedder / _extractor, vsb_model_set_dvmark_embedder / _extractor, vsb_model_set_vit_extractor and vsb_model_set_pixel_decoder check every rule the kernels place on the model's geometry; a
+    vsb_model_set_hidden_embedder / _extractor, vsb_model_set_dvmark_embedder / _extractor, vsb_model_set_vae_embedder, vsb_model_set_vit_extractor and vsb_model_set_pixel_decoder check every rule the kernels place on the model's geometry; a
     model they do not implement raises NotImplementedError."""
     L = _lib.lib()
-    if "hidden_encoder" not in spec and "dvmark_encoder" not in spec and not spec["unet"]["z"]:
+    if "hidden_encoder" not in spec and "dvmark_encoder" not in spec and "vae_encoder" not in spec and not spec["unet"]["z"]:
         # the descriptor of a U-Net without levels looks like one a HiDDeN embedder completes: reject it here, at load
         raise RuntimeError("libvsb200 error -1: unet levels: a U-Net needs 2 to 6 levels (z_channels_mults is empty)")
     h = C.c_void_p()
@@ -132,6 +146,8 @@ def _create(spec: dict):
         rc = L.vsb_model_set_hidden_embedder(h, C.byref(native_hidden_desc(spec["hidden_encoder"], True)))
     if rc == 0 and "dvmark_encoder" in spec:
         rc = L.vsb_model_set_dvmark_embedder(h, int(spec["dvmark_encoder"]["nbits"]))
+    if rc == 0 and "vae_encoder" in spec:
+        rc = L.vsb_model_set_vae_embedder(h, C.byref(native_vae_desc(spec["vae_encoder"])))
     if rc == 0 and "hidden_decoder" in spec:
         rc = L.vsb_model_set_hidden_extractor(h, C.byref(native_hidden_desc(spec["hidden_decoder"], False)))
     if rc == 0 and "dvmark_decoder" in spec:
