@@ -92,6 +92,45 @@ def grouped(sd, imgs: Tensor, group: int, taps: Optional[dict] = None) -> Tensor
     return torch.cat(outs)
 
 
+# ---------------------------------------------------------------------------------------------------------------------------------
+# the plans' frame slices (csrc/dvmark.cuh add_conv3d_sliced), restated: a 3x3x3 conv over C channels at h x h runs in launches of
+# slice_frames(h * h * stack_width(C), B) frames, each stacking its frames' time taps into a [frames][h * h][stack_width(C)] operand
+
+STACK_BUDGET = 512 << 20   # bytes of stacked operand per launch (kDvStackBudget)
+
+
+def stack_width(C: int) -> int:
+    return (3 * C + 63) // 64 * 64
+
+
+def slice_frames(frame_elems: int, B: int) -> int:
+    """dv_slice_frames: frames per launch whose fp16 stacked operand stays within the budget, at least one"""
+    return max(1, min(B, STACK_BUDGET // (frame_elems * 2)))
+
+
+def conv_slices(C: int, h: int, B: int):
+    """(start, end) of each launch of the 3x3x3 conv over C channels at h x h on B frames"""
+    fps = slice_frames(h * h * stack_width(C), B)
+    return [(b0, min(b0 + fps, B)) for b0 in range(0, B, fps)]
+
+
+def crossing_groups(slices, B: int, G: int):
+    """the groups of G frames that some slice boundary cuts (the frames on either side are time neighbours)"""
+    return [g for g in range(0, B, G) if any(g < b0 < min(g + G, B) for b0, _ in slices)]
+
+
+def segments(B: int, G: int, slices=()):
+    """(start, end) of the runs of frames that share a group and, given slices, a slice: the runs a 3x3x3 conv would see if its
+    time neighbours were cut at slice boundaries too"""
+    cuts = sorted({0, B} | set(range(0, B, G)) | {b0 for b0, _ in slices})
+    return list(zip(cuts, cuts[1:]))
+
+
+def slice_offset_ignored(ref: Tensor, slices) -> Tensor:
+    """a conv output whose every slice was stacked from the first slice's frames: slice (b0, e) holds ref[0 : e - b0]"""
+    return torch.cat([ref[:e - b0] for b0, e in slices])
+
+
 class DVMarkOracle(ho.HiddenOracle):
     """HiddenOracle (and so restate.OracleModel) with the DVMark detector: one detector call is one clip"""
 

@@ -1,9 +1,9 @@
 """The DVMark embedder on the GPU against the float64 oracle (tests/dvmark_enc_oracle.py; the embedder runs in float64 on the same
-device, the resize / JND / blend of oracle/restate.OracleModel on the CPU): imgs_w within the 1e-3 contract in image mode at 256 x 256
-with 96 bits across stacked-operand frame slices, in video mode with unequal chunks in every video_mode, on resized non-square input,
+device, the resize / JND / blend of oracle/restate.OracleModel on the CPU): imgs_w within the 1e-3 contract in image mode at 256 and
+384 with 96 bits across stacked-operand frame slices, in video mode with unequal chunks in every video_mode, on resized non-square input,
 on 64 frames in two chunks and at K = 1 and 30; the DVMark extractor's bits on its output; the group rules; group isolation;
-determinism; the streaming entry point; and every step of the plan on the exact fp16 inputs it read, with a bound derived from the
-step's roundings and a mutated reference per step that must leave it."""
+determinism; the streaming entry point; and every step of the plan on the exact fp16 inputs it read at 128, 256, 384 and 512
+(STEP_CONFIGS), with a bound derived from the step's roundings and a mutated reference per step that must leave it."""
 import ctypes as C
 
 import pytest
@@ -52,11 +52,20 @@ def _embed_both(model, orc, x, m, is_video):
 
 def test_image_mode_256_k96_12_frames():
     """12 frames in one call: every 3x3x3 conv at 256 x 256 runs in several frame slices"""
-    model, orc = _model(256, 96)
-    x, m = _frames(12, 256, 1), _msgs(12, 96, 2)
+    _image_mode_k96_12_frames(256)
+
+
+def test_image_mode_384_k96_12_frames():
+    """the half-resolution convs (192 wide) run on the gather loader"""
+    _image_mode_k96_12_frames(384)
+
+
+def _image_mode_k96_12_frames(S):
+    model, orc = _model(S, 96)
+    x, m = _frames(12, S, 1), _msgs(12, 96, 2)
     out, ref, err = _embed_both(model, orc, x, m, False)
     assert (out["preds_w"].cpu() - ref["preds_w"]).abs().max().item() <= TOL
-    print("image 256 K=96 x12: max |imgs_w - oracle|", f"{err:.2e}")
+    print("image", S, "K=96 x12: max |imgs_w - oracle|", f"{err:.2e}")
     # the DVMark extractor reads the same bits from the GPU's imgs_w as from the oracle's wherever the oracle's logit clears the margin
     got = model.detect(out["imgs_w"], is_video=False)["preds"].double()
     sd = {k: v.to(DEV, torch.float64) for k, v in orc.sd.items() if k.startswith("detector.")}
@@ -157,47 +166,93 @@ def _judge(name, got, ref, bound, mutants):
     return r
 
 
+# (S, B, G): 5 frames at 128 and 256 (K = 30; emb_layer3.0's 1152-wide operand in slices of 3 at 256), 3 at 384 (one-frame slices,
+# the half-resolution convs on the gather loader) and at 512 (one-frame and two-frame slices, a short last slice)
+STEP_CONFIGS = [(128, 5, 2), (256, 5, 2), (384, 3, 3), (512, 3, 3)]
+
+
 def test_each_step_against_float64_on_its_inputs():
-    """5 frames in chunks of 2 key frames (groups 2 | 2 | 1) at 128 x 128, K = 30, one message per frame.  Conv bound: fp16 weights
-    (2^-11 each) and fp32 sums (K 2^-24) times sum |x| |w|, plus the fp16 output rounding (2^-11 |y|, and 2^-25 near zero).  Mutations: messages of the
-    neighbouring frame, align_corners=False, the skip concat order swapped, the time taps reversed."""
-    S, K, G, B = 128, 30, 2, 5
+    """the STEP_CONFIGS row 128 x 5 G2: every conv in one launch"""
+    _each_step(*STEP_CONFIGS[0])
+
+
+@pytest.mark.parametrize("S,B,G", STEP_CONFIGS[1:], ids=[f"{s}x{b}-G{g}" for s, b, g in STEP_CONFIGS[1:]])
+def test_each_step_across_frame_slices(S, B, G):
+    """the STEP_CONFIGS rows in which some 3x3x3 conv runs in several frame slices"""
+    _each_step(S, B, G)
+
+
+def _each_step(S, B, G):
+    """B frames in chunks of G key frames, K = 30, one message per frame.  Conv bound: fp16 weights (2^-11 each) and fp32 sums
+    (K 2^-24) times sum |x| |w|, plus the fp16 output rounding (2^-11 |y|, and 2^-25 near zero).  Each 3x3x3 conv runs in the frame
+    slices dv_slice_frames gives (pinned by the tstack launch counts).  Mutations: messages of the neighbouring frame,
+    align_corners=False, the skip concat order swapped, the time taps reversed, and in every conv cut into slices, time neighbours
+    zeroed at slice boundaries (slice_is_group) and every slice stacked from the first slice's frames (slice_offset_ignored)."""
+    K = 30
     model, orc = _model(S, K)
     sd = orc.emb_sd
     x, m = _frames(B, S, 17).to(DEV), _msgs(B, K, 18).to(torch.uint8).to(DEV)
     out = torch.empty_like(x)
     L = _lib.lib()
     h = model._handle()
+    P1, P2 = (64 + K + 7) // 8 * 8, (128 + K + 7) // 8 * 8
+    # every 3x3x3 conv of the plan as (stacked channels, map side): its launches are the slices of conv_slices
+    c3 = [(64, S), (P1, S), (256, S), (128, S), (P2, S // 2), (512, S // 2), (256, S // 2), (384, S), (256, S), (128, S)]
+    want = {}
+    for c, hh in c3:
+        k = f"dvmark_enc.tstack.{c}-{dv.stack_width(c)}@{hh}"
+        want[k] = want.get(k, 0) + len(dv.conv_slices(c, hh, B))
     _lib.check(L.vsb_debug_keep_inputs(h, 1))
     try:
-        _lib.check(L.vsb_embed(h, x.data_ptr(), m.data_ptr(), B, out.data_ptr(), None, B, S, S, 1, 0, G,
-                               C.c_float(1.0), C.c_float(0.2), _lib.FLAG_NO_ATTENUATION, model._stream()))
         torch.cuda.synchronize()
+        L.vsb_profile_enable(1)
+        try:
+            _lib.check(L.vsb_embed(h, x.data_ptr(), m.data_ptr(), B, out.data_ptr(), None, B, S, S, 1, 0, G,
+                                   C.c_float(1.0), C.c_float(0.2), _lib.FLAG_NO_ATTENUATION, model._stream()))
+            torch.cuda.synchronize()
+            buf = C.create_string_buffer(1 << 16)
+            L.vsb_profile_read(buf, len(buf))
+        finally:
+            L.vsb_profile_enable(0)
+        launches = {ln.split("\t")[0]: int(ln.split("\t")[2]) for ln in buf.value.decode().splitlines()}
+        assert {k: launches.get(k) for k in want} == want, launches
         t = {n: _nchw(model.debug_tensor(n)) for n in ("dve.t0", "dve.t2", "dve.t4", "dve.cat1", "dve.e1_0", "dve.e1_2", "dve.cat2",
                                                         "dve.e2_0", "dve.e2_2", "dve.e2_4", "dve.cat3", "dve.e3_0", "dve.e3_2")}
         delta = model.debug_tensor("delta").to(DEV, torch.float64)
     finally:
         _lib.check(L.vsb_debug_keep_inputs(h, 0))
-    P1, P2 = (64 + K + 7) // 8 * 8, (128 + K + 7) // 8 * 8
     md = m.double()
+    groups = dv.segments(B, G)
 
-    def conv(key, inp, w=None, group=G):
+    def conv(key, inp, w=None, segs=groups):
         ww = sd[de.P + key + ".weight"] if w is None else w
         bb = sd[de.P + key + ".bias"] if w is None else torch.zeros_like(sd[de.P + key + ".bias"])
         pad = (ww.shape[2] // 2, 1, 1)
-        return torch.cat([F.conv3d(inp[g:g + group].permute(1, 0, 2, 3).unsqueeze(0), ww, bb, padding=pad).squeeze(0).permute(1, 0, 2, 3)
-                          for g in range(0, inp.shape[0], group)])
+        return torch.cat([F.conv3d(inp[a:e].permute(1, 0, 2, 3).unsqueeze(0), ww, bb, padding=pad).squeeze(0).permute(1, 0, 2, 3)
+                          for a, e in segs])
 
-    def conv_step(name, key, inp, got, relu=True, fp16_w=True, mutants=None):
+    def slice_mutants(key, inp, ref, C):
+        """the two slicing mutations of a 3x3x3 conv over C stacked channels (none when it runs in one launch)"""
+        slices = dv.conv_slices(C, inp.shape[-1], B)
+        if len(slices) == 1:
+            return {}
+        assert dv.crossing_groups(slices, B, G), (key, "no group crosses a slice boundary", slices)
+        return {"slice_is_group": conv(key, inp, segs=dv.segments(B, G, slices)),
+                "slice_offset_ignored": dv.slice_offset_ignored(ref, slices)}
+
+    def conv_step(name, key, inp, got, relu=True, fp16_w=True, mutants=None, C=None):
         w = sd[de.P + key + ".weight"]
         ref = conv(key, inp)
         kk = w[0].numel()
         mag = conv(key, inp.abs(), w.abs())
         bound = ((U16 if fp16_w else 0.0) + kk * U32) * mag
+        mutants = dict(mutants or {})
+        if w.shape[2] == 3:
+            mutants.update(slice_mutants(key, inp, ref, C or inp.shape[1]))
         if relu:
             ref = torch.relu(ref)
             bound = bound + U16 * ref + SUB
-        return _judge(name, got, ref, bound, {k: (torch.relu(v) if relu else v) for k, v in (mutants or {}).items()})
+        return _judge(name, got, ref, bound, {k: (torch.relu(v) if relu else v) for k, v in mutants.items()})
 
     xin = 2 * x.double() - 1
     conv_step("t0", "transform_layer.0", xin, t["dve.t0"], fp16_w=False)
@@ -213,7 +268,7 @@ def test_each_step_against_float64_on_its_inputs():
            {"neighbour_msgs": torch.roll(planes, 1, 0)})
     w10 = sd[de.P + "emb_layer1.0.weight"]
     cat1 = t["dve.cat1"][:, :64 + K]
-    conv_step("e1_0", "emb_layer1.0", cat1, t["dve.e1_0"],
+    conv_step("e1_0", "emb_layer1.0", cat1, t["dve.e1_0"], C=P1,
               mutants={"taps_reversed": conv("emb_layer1.0", cat1, w10.flip(2)) + sd[de.P + "emb_layer1.0.bias"].view(1, -1, 1, 1)})
     conv_step("e1_2", "emb_layer1.2", t["dve.e1_0"], t["dve.e1_2"])
     skip = t["dve.cat3"][:, :128]
@@ -224,7 +279,7 @@ def test_each_step_against_float64_on_its_inputs():
     planes2 = torch.zeros(B, P2 - 128, S // 2, S // 2, dtype=torch.float64, device=DEV)
     planes2[:, :K] = md[:, :, None, None]
     _judge("planes/2", t["dve.cat2"][:, 128:], planes2, torch.full_like(planes2, 1e-30), {"neighbour_msgs": torch.roll(planes2, 1, 0)})
-    conv_step("e2_0", "emb_layer2.0", t["dve.cat2"][:, :128 + K], t["dve.e2_0"])
+    conv_step("e2_0", "emb_layer2.0", t["dve.cat2"][:, :128 + K], t["dve.e2_0"], C=P2)
     conv_step("e2_2", "emb_layer2.2", t["dve.e2_0"], t["dve.e2_2"])
     conv_step("e2_4", "emb_layer2.4", t["dve.e2_2"], t["dve.e2_4"])
     # up-sample: one fp16 rounding of an fp32 blend, plus the fp32 source coordinate (|error| <= 2^-24 * index in lambda)
@@ -242,7 +297,10 @@ def test_each_step_against_float64_on_its_inputs():
     pre = conv("emb_layer3.4", t["dve.e3_2"])
     dbound = (U16 + w34[0].numel() * U32) * conv("emb_layer3.4", t["dve.e3_2"], w34.abs()) + 4 * U32
     _judge("out+tanh", delta, torch.tanh(pre), dbound,
-           {"taps_reversed": torch.tanh(conv("emb_layer3.4", t["dve.e3_2"], w34.flip(2)) + sd[de.P + "emb_layer3.4.bias"].view(1, -1, 1, 1))})
-    # the groups: frame 4 is a group of its own, so its output does not depend on frames 0-3
-    iso = conv("emb_layer3.4", t["dve.e3_2"][4:5], group=1)
-    assert (torch.tanh(iso) - delta[4:5]).abs().max().item() <= dbound[4:5].max().item()
+           {"taps_reversed": torch.tanh(conv("emb_layer3.4", t["dve.e3_2"], w34.flip(2)) + sd[de.P + "emb_layer3.4.bias"].view(1, -1, 1, 1)),
+            **{k: torch.tanh(v) for k, v in slice_mutants("emb_layer3.4", t["dve.e3_2"], pre, 128).items()}})
+    # the groups: the last group's output does not depend on the frames before it
+    g0 = (B - 1) // G * G
+    iso = conv("emb_layer3.4", t["dve.e3_2"][g0:], segs=[(0, B - g0)])
+    assert (torch.tanh(iso) - delta[g0:]).abs().max().item() <= dbound[g0:].max().item()
+    print(f"{S}x{B} G{G}: launches per stacked conv {want}")

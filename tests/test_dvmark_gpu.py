@@ -1,7 +1,8 @@
 """The DVMark extractor on the GPU against the float64 oracle (tests/dvmark_oracle.py, run in float64 on the same device): end to end
-in image and video mode, at 256 x 256 with 96 bits and across the stacked-operand frame slices, extract_message, the group rules
-through the C ABI, determinism, and every step of the plan on the exact fp16 inputs it read, with a mutated reference per step
-that must leave the step's bound."""
+in image and video mode, at 256, 384 and 640 with 96 bits and across the stacked-operand frame slices, extract_message, the group
+rules through the C ABI, determinism, and every step of the plan on the exact fp16 inputs it read at every processing size from 128
+to 768 (STEP_CONFIGS: one-frame, short and group-crossing slices), with a mutated reference per step that must leave the step's
+bound."""
 import ctypes as C
 
 import pytest
@@ -39,13 +40,24 @@ def _check_logits(got, ref, what):
     return err
 
 
+def _image_mode_k96(S, B):
+    model, sd = _model(S, 96)
+    x = _frames(B, S, 1)
+    got = model.detect(x, is_video=False)["preds"]
+    ref = dv.grouped(sd, x.double(), B)
+    print("image", S, "K=96 rel err", _check_logits(got, ref, "image"))
+
+
 def test_image_mode_256_k96_across_frame_slices():
     """12 frames in one call: layer2's stacked operand is cut into slices of 10 frames at 256 x 256"""
-    model, sd = _model(256, 96)
-    x = _frames(12, 256, 1)
-    got = model.detect(x, is_video=False)["preds"]
-    ref = dv.grouped(sd, x.double(), 12)
-    print("image 256 K=96 rel err", _check_logits(got, ref, "image"))
+    _image_mode_k96(256, 12)
+
+
+@pytest.mark.parametrize("S,B", [(384, 6), (640, 3)])
+def test_image_mode_k96_unaligned_half_size(S, B):
+    """layer3's map (192, 320) does not tile by 128 pixels and runs on the gather loader; layer2 in slices of 4 (384) and 1 frame
+    (640)"""
+    _image_mode_k96(S, B)
 
 
 def test_video_mode_two_unequal_chunks_and_extract_message():
@@ -116,6 +128,7 @@ def _step(name, got, ref, mutants, bound_rel):
     for mname, m in mutants.items():
         merr = (got - m).abs().max().item() / scale
         assert merr > bound_rel, (name, mname, merr)
+    print(f"  {name:12s} err {err:.2e} / {bound_rel:.0e}", {k: "rejected" for k in mutants})
     return err
 
 
@@ -133,41 +146,92 @@ def _head_mutant_no_borders(sd, l3, G):
     return torch.cat(outs)
 
 
-def test_each_step_against_float64_on_its_inputs():
-    """each kernel against float64 on the fp16 taps it read: layer1 (CUDA cores) from the frames, layer2 from layer1, layer3 from
-    layer2 (the pool fused into the stack), the head (rows, window sums, layer4 + mean) from layer3.  Mutations: the time padding
-    leaking across groups (one clip over the whole batch), the pool left out, the border windows ignored."""
-    model, sd = _model(128, 32)
-    x = _frames(5, 128, 5)
-    G = 2
-    out = torch.empty(5, 33, device=DEV)
-    L = _lib.lib()
-    _lib.check(L.vsb_detect_grouped(model._handle(), x.data_ptr(), out.data_ptr(), 5, 128, 128, G, 0, model._stream()))
+# (S, B, G): 5 frames at 128 fit one launch per conv; above, layer2's stacked operand is cut into slices of 10 (256), 4 (384), 2 (512)
+# and 1 frame (640, 768), with a group across a slice boundary, a short last slice at 256, 384 and 512, and layer3 (on the gather
+# loader at 384 and 640) in one launch
+STEP_CONFIGS = [(128, 5, 2), (256, 12, 4), (384, 6, 3), (512, 5, 5), (640, 3, 3), (768, 3, 3)]
+
+
+def _profiled(L, fn):
+    """run fn with the per-launch profiler on: {step name: launches}"""
     torch.cuda.synchronize()
+    L.vsb_profile_enable(1)
+    try:
+        fn()
+        torch.cuda.synchronize()
+        buf = C.create_string_buffer(1 << 16)
+        L.vsb_profile_read(buf, len(buf))
+    finally:
+        L.vsb_profile_enable(0)
+    return {ln.split("\t")[0]: int(ln.split("\t")[2]) for ln in buf.value.decode().splitlines()}
+
+
+def _each_step(S, B, G):
+    """each kernel against float64 on the fp16 taps it read: layer1 (CUDA cores) from the frames, layer2 from layer1, layer3 from
+    layer2 (the pool fused into the stack), the head (rows, window sums, layer4 + mean) from layer3.  Each stacked conv runs in the
+    frame slices dv_slice_frames gives (pinned by its tstack launch count).  Mutations: the time padding leaking across groups (one
+    clip over the whole batch), the pool left out, the border windows ignored, and in a conv cut into slices, time neighbours zeroed
+    at slice boundaries (slice_is_group) and every slice stacked from the first slice's frames (slice_offset_ignored)."""
+    model, sd = _model(S, 32)
+    x = _frames(B, S, 5)
+    out = torch.empty(B, 33, device=DEV)
+    L = _lib.lib()
+    h2 = S // 2
+    sl2, sl3 = dv.conv_slices(128, S, B), dv.conv_slices(128, h2, B)
+    launches = _profiled(L, lambda: _lib.check(L.vsb_detect_grouped(model._handle(), x.data_ptr(), out.data_ptr(), B, S, S, G, 0,
+                                                                     model._stream())))
+    assert launches.get(f"dvmark.tstack.128-384@{S}") == len(sl2), launches
+    assert launches.get(f"dvmark.tstack+pool.128-384@{h2}") == len(sl3), launches
     P = "detector.layers.layer"
     l1, l2, l3 = (_nchw(model.debug_tensor(f"dvm.l{i}")) for i in (1, 2, 3))
     xd = x.double()
 
-    def conv(i, inp, group):
-        return torch.cat([torch.relu(dv.conv3d(inp[g:g + group], sd[P + f"{i}.weight"], sd[P + f"{i}.bias"]))
-                          for g in range(0, inp.shape[0], group)])
+    def conv(i, inp, segs):
+        return torch.cat([torch.relu(dv.conv3d(inp[a:e], sd[P + f"{i}.weight"], sd[P + f"{i}.bias"])) for a, e in segs])
+
+    def slice_mutants(i, inp, ref, slices):
+        if len(slices) == 1:
+            return {}
+        assert dv.crossing_groups(slices, B, G), ("no group crosses a slice boundary", slices)
+        return {"slice_is_group": conv(i, inp, dv.segments(B, G, slices)), "slice_offset_ignored": dv.slice_offset_ignored(ref, slices)}
+    groups = dv.segments(B, G)
+
+    def leak(f):   # one clip over the whole batch: a mutation only where the batch holds more than one group
+        return {"leak": f()} if len(groups) > 1 else {}
     errs = {}
     # fp16 outputs (2^-11 relative) of fp32 sums; layers 2-3 also read fp16 weights (2^-12 relative each)
-    errs["l1"] = _step("layer1", l1, conv(1, xd, G), {"leak": conv(1, xd, 5)}, 2e-3)
-    errs["l2"] = _step("layer2", l2, conv(2, l1, G), {"leak": conv(2, l1, 5)}, 8e-3)
+    errs["l1"] = _step("layer1", l1, conv(1, xd, groups), leak(lambda: conv(1, xd, [(0, B)])), 2e-3)
+    ref2 = conv(2, l1, groups)
+    errs["l2"] = _step("layer2", l2, ref2, {**leak(lambda: conv(2, l1, [(0, B)])), **slice_mutants(2, l1, ref2, sl2)}, 8e-3)
+    del ref2, l1
     p2 = F.avg_pool2d(l2, 2).half().double()      # the stack kernel rounds the pooled operand to fp16
-    errs["l3"] = _step("layer3", l3, conv(3, p2, G),
-                       {"leak": conv(3, p2, 5), "no_pool": conv(3, l2[:, :, ::2, ::2], G)}, 8e-3)
-    head = torch.cat([dv.conv3d(F.avg_pool2d(l3[g:g + G], 2), sd[P + "4.weight"], sd[P + "4.bias"]).mean(dim=[2, 3])
-                      for g in range(0, 5, G)])
-    leak = dv.conv3d(F.avg_pool2d(l3, 2), sd[P + "4.weight"], sd[P + "4.bias"]).mean(dim=[2, 3])
-    errs["head"] = _step("head", out.double(), head, {"leak": leak, "borders": _head_mutant_no_borders(sd, l3, G)}, 1e-5)
-    # the window sums the head read: per frame, tap (1, 1, 1) is the whole pooled map's sum
-    win = model.debug_tensor("dvm.win").to(DEV, torch.float64).reshape(5, 27, 256)
+    ref3 = conv(3, p2, groups)
+    errs["l3"] = _step("layer3", l3, ref3, {**leak(lambda: conv(3, p2, [(0, B)])), "no_pool": conv(3, l2[:, :, ::2, ::2], groups),
+                                            **slice_mutants(3, p2, ref3, sl3)}, 8e-3)
+    del ref3, l2, p2
+    head = torch.cat([dv.conv3d(F.avg_pool2d(l3[a:e], 2), sd[P + "4.weight"], sd[P + "4.bias"]).mean(dim=[2, 3]) for a, e in groups])
+    errs["head"] = _step("head", out.double(), head,
+                         {**leak(lambda: dv.conv3d(F.avg_pool2d(l3, 2), sd[P + "4.weight"], sd[P + "4.bias"]).mean(dim=[2, 3])),
+                          "borders": _head_mutant_no_borders(sd, l3, G)}, 1e-5)
+    # the window sums the head read: per frame, tap (1, 1, 1) is the whole pooled map's sum; taps dt = 0 / 2 are zero exactly at the
+    # first / last frame of each group
+    win = model.debug_tensor("dvm.win").to(DEV, torch.float64).reshape(B, 27, 256)
     tot = F.avg_pool2d(l3, 2).sum(dim=[2, 3])
     _step("window sums", win[:, 13], tot, {}, 1e-5)
     zero = lambda t: torch.equal(t, torch.zeros_like(t))   # noqa: E731
-    assert zero(win[1, 18:]) and zero(win[2, :9]), "frames 1 and 2 lie in different groups"
-    assert zero(win[4, :9]) and zero(win[4, 18:]), "frame 4 is a group of its own"
-    assert not zero(win[3, :9]) and not zero(win[1, :9]), "frames 2-3 and 0-1 share a group"
-    print("step errors (relative to max|ref|):", {k: f"{v:.2e}" for k, v in errs.items()})
+    for b in range(B):
+        assert zero(win[b, :9]) == (b % G == 0), ("previous-frame taps", b)
+        assert zero(win[b, 18:]) == (b % G == G - 1 or b == B - 1), ("next-frame taps", b)
+    print(f"{S}x{B} G{G}: layer2 slices {sl2}, layer3 slices {sl3}; step errors (relative to max|ref|):",
+          {k: f"{v:.2e}" for k, v in errs.items()})
+
+
+def test_each_step_against_float64_on_its_inputs():
+    """the STEP_CONFIGS row 128 x 5 G2: every conv in one launch"""
+    _each_step(*STEP_CONFIGS[0])
+
+
+@pytest.mark.parametrize("S,B,G", STEP_CONFIGS[1:], ids=[f"{s}x{b}-G{g}" for s, b, g in STEP_CONFIGS[1:]])
+def test_each_step_across_frame_slices(S, B, G):
+    """the STEP_CONFIGS rows whose layer2 runs in several frame slices"""
+    _each_step(S, B, G)

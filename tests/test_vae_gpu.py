@@ -3,8 +3,8 @@ resize / JND / blend of oracle/restate.OracleModel on the CPU): imgs_w within th
 for vae_small at 512 and 768, on 64 and 70 frames, in video mode in every video_mode and on resized 1080p input; the paired
 extractor's bits; determinism and independence from the sub-batch split; the streaming entry point; the step names; vae_tiny on 64
 frames against the error of the fp16 emulation of its plan; and every step of the plan on the exact fp16 inputs it read, with a bound
-from the step's roundings and mutated references that must leave it (tests/vae_kernels.py), for head dims 64 and 128 and every
-GroupNorm group width."""
+from the step's roundings and mutated references that must leave it (tests/vae_kernels.py), at every processing size from 128 to 768
+(CONFIGS), for head dims 64 and 128, every GroupNorm group width and both loaders of the 3x3 convs, with the steps' names pinned."""
 import ctypes as C
 
 import pytest
@@ -144,8 +144,24 @@ def _nchw(t):
     return t.to(DEV, torch.float64).permute(0, 3, 1, 2)
 
 
-def _run_steps(model, orc, x, m, eps_steps=()):
-    """one vsb_embed of the frames x (at processing size) with every map kept, then every step judged on the taps it read"""
+def _profiled_names(fn):
+    """the vae.* step names of the launches fn makes"""
+    L = _lib.lib()
+    torch.cuda.synchronize()
+    L.vsb_profile_enable(1)
+    try:
+        fn()
+        torch.cuda.synchronize()
+        buf = C.create_string_buffer(1 << 16)
+        L.vsb_profile_read(buf, len(buf))
+    finally:
+        L.vsb_profile_enable(0)
+    return {line.split("\t")[0] for line in buf.value.decode().splitlines() if line.startswith("vae.")}
+
+
+def _run_steps(model, orc, x, m, eps_steps=(), names=None):
+    """one vsb_embed of the frames x (at processing size) with every map kept, then every step judged on the taps it read; the
+    plan's step names are added to `names`"""
     B, S = x.shape[0], x.shape[-1]
     K = m.shape[1]
     x, m8 = x.to(DEV).contiguous(), m.to(torch.uint8).to(DEV).contiguous()
@@ -154,9 +170,11 @@ def _run_steps(model, orc, x, m, eps_steps=()):
     h = model._handle()
     _lib.check(L.vsb_debug_keep_inputs(h, 1))
     try:
-        _lib.check(L.vsb_embed(h, x.data_ptr(), m8.data_ptr(), B, out.data_ptr(), None, B, S, S, 1, 0, B,
-                               C.c_float(1.0), C.c_float(0.2), _lib.FLAG_NO_ATTENUATION, model._stream()))
-        torch.cuda.synchronize()
+        got = _profiled_names(lambda: _lib.check(L.vsb_embed(h, x.data_ptr(), m8.data_ptr(), B, out.data_ptr(), None, B, S, S, 1, 0, B,
+                                                             C.c_float(1.0), C.c_float(0.2), _lib.FLAG_NO_ATTENUATION,
+                                                             model._stream())))
+        if names is not None:
+            names |= got
         cache = {}
 
         class Taps:   # read lazily, a few at a time: all taps of a plan in float64 would not fit
@@ -167,30 +185,122 @@ def _run_steps(model, orc, x, m, eps_steps=()):
                     cache[name] = _nchw(model.debug_tensor(name))
                 return cache[name]
         delta = model.debug_tensor("delta").to(DEV, torch.float64)
-        res = vk.run_steps(orc.emb_sd, orc.spec["vae_encoder"], x.double(), m.to(DEV), Taps(), delta, print, eps_steps)
+        xe = vo.restate.rgb_to_y(x.float().cpu()).to(DEV, torch.float64) if orc.spec["yuv"] else x.double()   # the embedder's input
+        res = vk.run_steps(orc.emb_sd, orc.spec["vae_encoder"], xe, m.to(DEV), Taps(), delta, print, eps_steps)
     finally:
         _lib.check(L.vsb_debug_keep_inputs(h, 0))
     assert K == m.shape[1]
     return res
 
 
-def test_vae_tiny_steps_on_the_64_frame_input():
-    """vae_tiny (head dim 64; one, two and four channels per GroupNorm group) on the 64 frames of the 64-frame parity test, in
-    slices of 8 frames: every step within its fp16 bound"""
-    model, orc = _model("vae_tiny", 256)
-    x, m = _frames(64, 256, 5), _msgs(64, 32, 6)
-    worst = {}
-    for b in range(0, 64, 8):
-        for k, r in _run_steps(model, orc, x[b:b + 8], m[b:b + 8]).items():
+# (preset, S, frames) -> the steps the plan must name (prefix "vae."): every processing size the four-level presets accept, both
+# head dims (64: vae_tiny, 128: the others), token counts 256 to 9 216, and both loaders of the stride-1 3x3 convs: the TMA conv where
+# a map tiles by 128 pixels, the gather loader (conv3x3g, conv_outg) at the 48 to 320 wide maps of 384, 640 and 768.  vae_tiny at
+# 256 runs the 64 frames of the 64-frame parity test in slices of 8; at 640 and 768 B stays small (every map has its own buffer).
+CONFIGS = {
+    ("vae_tiny", 256, 64): """enc.conv_in.3-16@256 enc.conv3x3.16-16@256 enc.conv3x3+res.16-16@256 enc.conv3x3.16-32@128
+        enc.conv3x3+res.32-32@128 enc.conv3x3.32-32@64 enc.conv3x3+res.32-32@64 enc.conv3x3.32-64@32 enc.conv3x3+res.64-64@32
+        enc.conv_out.64-4@32 attn.64@32 dec.conv3x3+res.16-16@256 dec.conv3x3+res.32-32@128 dec.conv3x3+res.32-32@64
+        dec.conv3x3+res.64-64@32 dec.conv_out+tanh.16-3@256""",
+    ("vae_small", 256, 3): """enc.conv_in.3-32@256 enc.conv3x3.32-32@256 enc.conv3x3+res.32-32@256 enc.conv3x3.32-64@128
+        enc.conv3x3+res.64-64@128 enc.conv3x3.64-64@64 enc.conv3x3+res.64-64@64 enc.conv3x3.64-128@32 enc.conv3x3+res.128-128@32
+        enc.conv_out.128-4@32 attn.128@32 dec.conv3x3+res.32-32@256 dec.conv3x3+res.64-64@128 dec.conv3x3+res.64-64@64
+        dec.conv3x3+res.128-128@32 dec.conv_out+tanh.32-3@256""",
+    ("vae_big", 256, 3): """enc.conv_in.3-64@256 enc.conv3x3.64-64@256 enc.conv3x3+res.64-64@256 enc.conv3x3.64-64@128
+        enc.conv3x3+res.64-64@128 enc.conv3x3.64-128@64 enc.conv3x3+res.128-128@64 enc.conv3x3.128-128@32 enc.conv3x3+res.128-128@32
+        enc.conv_out.128-4@32 attn.128@32 dec.conv3x3+res.64-64@256 dec.conv3x3+res.64-64@128 dec.conv3x3+res.128-128@64
+        dec.conv3x3+res.128-128@32 dec.conv_out+tanh.64-3@256""",
+    ("vae_tiny", 384, 3): """enc.conv_in.3-16@384 enc.conv3x3.16-16@384 enc.conv3x3+res.16-16@384 enc.conv3x3g.16-32@192
+        enc.conv3x3g+res.32-32@192 enc.conv3x3g.32-32@96 enc.conv3x3g+res.32-32@96 enc.conv3x3g.32-64@48 enc.conv3x3g+res.64-64@48
+        enc.conv_outg.64-4@48 attn.64@48 dec.conv3x3+res.16-16@384 dec.conv3x3g+res.32-32@192 dec.conv3x3g+res.32-32@96
+        dec.conv3x3g+res.64-64@48 dec.conv_out+tanh.16-3@384""",
+    ("vae_tiny", 640, 2): """enc.conv_in.3-16@640 enc.conv3x3.16-16@640 enc.conv3x3+res.16-16@640 enc.conv3x3g.16-32@320
+        enc.conv3x3g+res.32-32@320 enc.conv3x3g.32-32@160 enc.conv3x3g+res.32-32@160 enc.conv3x3g.32-64@80 enc.conv3x3g+res.64-64@80
+        enc.conv_outg.64-4@80 attn.64@80 dec.conv3x3+res.16-16@640 dec.conv3x3g+res.32-32@320 dec.conv3x3g+res.32-32@160
+        dec.conv3x3g+res.64-64@80 dec.conv_out+tanh.16-3@640""",
+    ("vae_small", 128, 4): """enc.conv_in.3-32@128 enc.conv3x3.32-32@128 enc.conv3x3+res.32-32@128 enc.conv3x3.32-64@64
+        enc.conv3x3+res.64-64@64 enc.conv3x3.64-64@32 enc.conv3x3+res.64-64@32 enc.conv3x3.64-128@16 enc.conv3x3+res.128-128@16
+        enc.conv_out.128-4@16 attn.128@16 dec.conv3x3+res.32-32@128 dec.conv3x3+res.64-64@64 dec.conv3x3+res.64-64@32
+        dec.conv3x3+res.128-128@16 dec.conv_out+tanh.32-3@128""",
+    ("vae_small", 768, 2): """enc.conv_in.3-32@768 enc.conv3x3.32-32@768 enc.conv3x3+res.32-32@768 enc.conv3x3.32-64@384
+        enc.conv3x3+res.64-64@384 enc.conv3x3g.64-64@192 enc.conv3x3g+res.64-64@192 enc.conv3x3g.64-128@96
+        enc.conv3x3g+res.128-128@96 enc.conv_outg.128-4@96 attn.128@96 dec.conv3x3+res.32-32@768 dec.conv3x3+res.64-64@384
+        dec.conv3x3g+res.64-64@192 dec.conv3x3g+res.128-128@96 dec.conv_out+tanh.32-3@768""",
+    ("vae_big", 512, 2): """enc.conv_in.3-64@512 enc.conv3x3.64-64@512 enc.conv3x3+res.64-64@512 enc.conv3x3.64-64@256
+        enc.conv3x3+res.64-64@256 enc.conv3x3.64-128@128 enc.conv3x3+res.128-128@128 enc.conv3x3.128-128@64 enc.conv3x3+res.128-128@64
+        enc.conv_out.128-4@64 attn.128@64 dec.conv3x3+res.64-64@512 dec.conv3x3+res.64-64@256 dec.conv3x3+res.128-128@128
+        dec.conv3x3+res.128-128@64 dec.conv_out+tanh.64-3@512""",
+    ("vae_big", 640, 2): """enc.conv_in.3-64@640 enc.conv3x3.64-64@640 enc.conv3x3+res.64-64@640 enc.conv3x3g.64-64@320
+        enc.conv3x3g+res.64-64@320 enc.conv3x3g.64-128@160 enc.conv3x3g+res.128-128@160 enc.conv3x3g.128-128@80
+        enc.conv3x3g+res.128-128@80 enc.conv_outg.128-4@80 attn.128@80 dec.conv3x3+res.64-64@640 dec.conv3x3g+res.64-64@320
+        dec.conv3x3g+res.128-128@160 dec.conv3x3g+res.128-128@80 dec.conv_out+tanh.64-3@640""",
+    ("vae_small_yuv", 384, 2): """enc.conv_in.1-32@384 enc.conv3x3.32-32@384 enc.conv3x3+res.32-32@384 enc.conv3x3g.32-64@192
+        enc.conv3x3g+res.64-64@192 enc.conv3x3g.64-64@96 enc.conv3x3g+res.64-64@96 enc.conv3x3g.64-128@48 enc.conv3x3g+res.128-128@48
+        enc.conv_outg.128-4@48 attn.128@48 dec.conv3x3+res.32-32@384 dec.conv3x3g+res.64-64@192 dec.conv3x3g+res.64-64@96
+        dec.conv3x3g+res.128-128@48 dec.conv_out+tanh.32-1@384""",
+}
+
+
+def _expect(cfg_):
+    return {"vae." + n for n in CONFIGS[cfg_].split()}
+
+
+def _tiles_128(h):
+    """the h x h map tiles the TMA conv by 128 pixels"""
+    return h % 128 == 0 if h >= 128 else 128 % h == 0 and h % (128 // h) == 0
+
+
+def _check_steps(cfg_):
+    """every step of the plan within its fp16 bound on the taps it read, every mutation outside it (tests/vae_kernels.py); the
+    plan names the expected steps, and every stride-1 3x3 conv runs on the loader its map's side selects"""
+    preset, S, B = cfg_
+    model, orc = _model(preset, S)
+    x, m = _frames(B, S, 5 if B == 64 else 17), _msgs(B, 32, 6 if B == 64 else 18)
+    worst, names = {}, set()
+    for b in range(0, B, 8):
+        for k, r in _run_steps(model, orc, x[b:b + 8], m[b:b + 8], names=names).items():
             worst[k] = max(worst.get(k, 0.0), r)
-    print("vae_tiny 64 frames: worst err/bound", max(worst.values()))
+    assert _expect(cfg_) <= names, sorted(_expect(cfg_) - names)
+    for n in names:
+        for conv in ("conv3x3", "conv_out"):
+            if f".{conv}" in n and not n.startswith("vae.dec.conv_out"):
+                assert (f".{conv}g" in n) != _tiles_128(int(n.rsplit("@", 1)[1])), n
+    print(f"{preset} {S}x{B}: worst err/bound {max(worst.values()):.3f}; gather-loader steps",
+          sorted(n for n in names if "3x3g" in n or "conv_outg" in n))
+
+
+def test_vae_tiny_steps_on_the_64_frame_input():
+    """the CONFIGS row vae_tiny 256 x 64: head dim 64; one, two and four channels per GroupNorm group; in slices of 8 frames"""
+    _check_steps(("vae_tiny", 256, 64))
 
 
 @pytest.mark.parametrize("preset", ["vae_small", "vae_big"])
 def test_steps_head_dim_128(preset):
-    """head dim 128; two, four and eight channels per group"""
-    model, orc = _model(preset, 256)
-    _run_steps(model, orc, _frames(3, 256, 17), _msgs(3, 32, 18))
+    """the CONFIGS rows at 256 x 256 with head dim 128; two, four and eight channels per group"""
+    _check_steps((preset, 256, 3))
+
+
+SIZED = [c for c in CONFIGS if c[1] != 256]
+
+
+@pytest.mark.parametrize("cfg_", SIZED, ids=[f"{p}-{s}x{b}" for p, s, b in SIZED])
+def test_steps(cfg_):
+    """the CONFIGS rows at the other processing sizes (128, 384, 512, 640, 768)"""
+    _check_steps(cfg_)
+
+
+def test_configs_reach_every_size_head_dim_and_loader():
+    """the CONFIGS rows together: every processing size from 128 to 768, attention at head dims 64 and 128, and conv3x3,
+    conv3x3+res and the latent conv_out on both the TMA conv and the gather loader"""
+    assert {S for _, S, _ in CONFIGS} == set(range(128, 769, 128))
+    names = set().union(*(_expect(c) for c in CONFIGS))
+    assert {n.split("@")[0] for n in names if n.startswith("vae.attn.")} == {"vae.attn.64", "vae.attn.128"}
+    for tma, gather in ((".conv3x3.", ".conv3x3g."), (".conv3x3+res.", ".conv3x3g+res."), ("enc.conv_out.", "enc.conv_outg.")):
+        assert any(tma in n for n in names) and any(gather in n for n in names), (tma, gather)
+    for n in names:
+        h = int(n.rsplit("@", 1)[1])
+        if "conv3x3" in n or "enc.conv_out" in n:
+            assert ("3x3g" in n or "conv_outg" in n) != _tiles_128(h), n
 
 
 def test_groupnorm_eps_on_a_flat_frame():
@@ -251,6 +361,7 @@ def test_step_names():
     L.vsb_profile_read(buf, len(buf))
     L.vsb_profile_enable(0)
     names = {line.split("\t")[0] for line in buf.value.decode().splitlines() if line.startswith("vae.")}
+    assert not [n for n in names if "3x3g" in n or "conv_outg" in n], "256 x 256 runs every 3x3 conv on the TMA conv"
     want = {"vae.enc.conv_in.3-32@256", "vae.gn16.silu.32@256", "vae.gn16.silu.64@128", "vae.gn16.silu.128@32", "vae.gn16.128@32",
             "vae.enc.conv3x3.32-32@256", "vae.enc.conv3x3+res.32-32@256", "vae.enc.nin.32-64@128", "vae.enc.down.32@256",
             "vae.enc.qkv.128@32", "vae.attn.128@32", "vae.enc.proj+res.128@32", "vae.enc.conv_out.128-4@32", "vae.msg_table",

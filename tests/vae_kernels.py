@@ -111,8 +111,11 @@ def vae_forward_emulated(sd, v: dict, x: Tensor, msgs: Tensor, plan: Plan16, tap
 # per-step references, bounds and mutations
 
 
+BORDER_ONLY = ("replicate_border",)   # mutations that differ from the reference on the one-pixel border of the map only
+
+
 def judge(name: str, got: Tensor, ref: Tensor, bound: Tensor, mutants: Dict[str, Tensor]) -> float:
-    """|got - ref| <= bound everywhere; every mutant leaves the bound somewhere"""
+    """|got - ref| <= bound everywhere; every mutant leaves the bound somewhere, and a BORDER_ONLY mutant nowhere but on the border"""
     q = (got - ref).abs() / bound
     r = q.max().item()
     if r > 1.0:
@@ -120,14 +123,34 @@ def judge(name: str, got: Tensor, ref: Tensor, bound: Tensor, mutants: Dict[str,
         raise AssertionError((name, r, "got", got.reshape(-1)[i].item(), "ref", ref.reshape(-1)[i].item(), "bound",
                               bound.reshape(-1)[i].item(), "index", i, "shape", tuple(got.shape)))
     for mname, mut in mutants.items():
-        mr = ((got - mut).abs() / bound).max().item()
-        assert mr > 1.0, (name, mname, mr)
+        out = (got - mut).abs() > bound
+        assert bool(out.any()), (name, mname, ((got - mut).abs() / bound).max().item())
+        if mname in BORDER_ONLY:
+            inside = int(out[..., 1:-1, 1:-1].sum())
+            assert inside == 0, (name, mname, inside, "violations off the one-pixel border")
     return r
 
 
 def conv_ref(sd, key, inp, stride=1, pad=1, w=None, bias=True):
     ww = sd[key + ".weight"] if w is None else w
     return F.conv2d(inp, ww, sd[key + ".bias"] if bias else None, stride=stride, padding=pad if ww.shape[-1] == 3 else 0)
+
+
+def conv3_mutants(sd, key, inp, add=0.0, post=None, w=None):
+    """mutations of a stride-1 zero-padded 3x3 conv of inp (+ add, then post): the (r, s) taps transposed, and replicate instead of
+    zero padding (which moves the one-pixel border only)"""
+    ww = sd[key + ".weight"] if w is None else w
+    post = post or (lambda u: u)
+    return {"taps_transposed": post(add + F.conv2d(inp, ww.transpose(-1, -2), sd[key + ".bias"], padding=1)),
+            "replicate_border": post(add + F.conv2d(F.pad(inp, (1, 1, 1, 1), mode="replicate"), ww, sd[key + ".bias"]))}
+
+
+def nearest_shifted(x: Tensor) -> Tensor:
+    """a wrong nearest x2 up-sample: output row / column i reads source (i + 1) // 2, clamped to the map"""
+    h, w = x.shape[-2:]
+    ri = ((torch.arange(2 * h, device=x.device) + 1) // 2).clamp(max=h - 1)
+    ci = ((torch.arange(2 * w, device=x.device) + 1) // 2).clamp(max=w - 1)
+    return x[..., ri, :][..., ci]
 
 
 def conv_bound(sd, key, inp, ref, fp16_w=True, stride=1, pad=1, out16=True):
@@ -188,7 +211,8 @@ def small_variance_map(B: int, C: int, h: int, seed: int, device=None) -> Tensor
 
 def attn_step(qkv: Tensor, got: Tensor):
     """softmax(q k^T / sqrt(C)) v from the fp16 qkv rows: fp32 scores and exponentials, P rounded to fp16 (2^-11 relative), fp32
-    accumulation, one fp16 rounding of the output.  Mutations: no 1/sqrt(C), softmax over queries, k and v swapped."""
+    accumulation, one fp16 rounding of the output.  Mutations: no 1/sqrt(C), softmax over queries, k and v swapped, and the last
+    tile of 64 keys left out of the softmax and the sum."""
     B, C3, hh, ww = qkv.shape
     C = C3 // 3
     q, k, v = (qkv[:, i * C:(i + 1) * C].reshape(B, C, hh * ww) for i in range(3))
@@ -201,7 +225,8 @@ def attn_step(qkv: Tensor, got: Tensor):
     # P's fp16 rounding and the exp / score error (|s| 2^-22 relative, scores up to |q||k|): 3 x 2^-11 of sum p |v|
     bound = 3 * U16 * of(p, v.abs()) + U16 * o.abs() + SUB
     return got, o, bound, {"no_scale": of(torch.softmax(sc, 2), v), "softmax_over_queries": of(torch.softmax(sc * C ** -0.5, 1), v),
-                           "k_v_swapped": of(torch.softmax(torch.bmm(q.permute(0, 2, 1), v) * C ** -0.5, 2), k)}
+                           "k_v_swapped": of(torch.softmax(torch.bmm(q.permute(0, 2, 1), v) * C ** -0.5, 2), k),
+                           "last_key_tile_dropped": of(torch.softmax(sc[:, :, :-64] * C ** -0.5, 2), v[:, :, :-64])}
 
 
 def steps(sd, v: dict, x: Tensor, msgs: Tensor, t, delta: Tensor, eps_steps=()):
@@ -211,7 +236,8 @@ def steps(sd, v: dict, x: Tensor, msgs: Tensor, t, delta: Tensor, eps_steps=()):
     L, nr = len(v["ch_mult"]), v["num_res_blocks"]
     xin = 2 * x - 1
     ref = conv_ref(sd, E + "conv_in", xin)
-    yield ("conv_in",) + (t["vae.enc.conv_in"], ref, conv_bound(sd, E + "conv_in", xin, ref, fp16_w=False), {})
+    yield ("conv_in",) + (t["vae.enc.conv_in"], ref, conv_bound(sd, E + "conv_in", xin, ref, fp16_w=False),
+                          conv3_mutants(sd, E + "conv_in", xin))
     # every ResnetBlock: both norms, conv1, the shortcut, conv2 + residual
     blocks = [(E + f"down.{l}.block.{i}", f"vae.enc.d{l}.{i}") for l in range(L) for i in range(nr)]
     blocks += [(E + "mid.block_1", "vae.enc.mid1"), (E + "mid.block_2", "vae.enc.mid2"), (D + "mid.block_1", "vae.dec.mid1"),
@@ -234,7 +260,7 @@ def steps(sd, v: dict, x: Tensor, msgs: Tensor, t, delta: Tensor, eps_steps=()):
                                             tp + ".gn1" in eps_steps)
         a1 = t[tp + ".gn1"]
         ref = conv_ref(sd, key + ".conv1", a1)
-        yield (tp + ".conv1",) + (t[tp + ".conv1"], ref, conv_bound(sd, key + ".conv1", a1, ref), {})
+        yield (tp + ".conv1",) + (t[tp + ".conv1"], ref, conv_bound(sd, key + ".conv1", a1, ref), conv3_mutants(sd, key + ".conv1", a1))
         yield (tp + ".gn2",) + gn_step(t[tp + ".conv1"], sd[key + ".norm2.weight"], sd[key + ".norm2.bias"], True, t[tp + ".gn2"])
         sc = xb
         if key + ".nin_shortcut.weight" in sd:
@@ -244,21 +270,26 @@ def steps(sd, v: dict, x: Tensor, msgs: Tensor, t, delta: Tensor, eps_steps=()):
         a2 = t[tp + ".gn2"]
         body = conv_ref(sd, key + ".conv2", a2)
         ref = sc + body
-        yield (tp + ".out",) + (t[tp + ".out"], ref, conv_bound(sd, key + ".conv2", a2, ref), {"missing_shortcut": body})
+        yield (tp + ".out",) + (t[tp + ".out"], ref, conv_bound(sd, key + ".conv2", a2, ref),
+                                {"missing_shortcut": body, **conv3_mutants(sd, key + ".conv2", a2, add=sc)})
     # resampling
     for l in range(L - 1):
         xd = t[f"vae.enc.d{l}.{nr - 1}.out"]
         xp = F.pad(xd, (0, 1, 0, 1))
         ref = conv_ref(sd, E + f"down.{l}.downsample.conv", xp, 2, 0)
+        wd = sd[E + f"down.{l}.downsample.conv.weight"]
         yield (f"down{l}",) + (t[f"vae.enc.down{l}"], ref, conv_bound(sd, E + f"down.{l}.downsample.conv", xp, ref, stride=2, pad=0),
-                           {"symmetric_pad": conv_ref(sd, E + f"down.{l}.downsample.conv", xd, 2, 1)})
+                           {"symmetric_pad": conv_ref(sd, E + f"down.{l}.downsample.conv", xd, 2, 1),
+                            "taps_transposed": conv_ref(sd, E + f"down.{l}.downsample.conv", xp, 2, 0, w=wd.transpose(-1, -2))})
     for l in range(1, L):
         xu = t[f"vae.dec.u{l}.{nr}.out"]
         up = F.interpolate(xu, scale_factor=2.0, mode="nearest")
         ref = conv_ref(sd, D + f"up.{l}.upsample.conv", up)
         yield (f"up{l}",) + (t[f"vae.dec.up{l}"], ref, conv_bound(sd, D + f"up.{l}.upsample.conv", up, ref),
                          {"bilinear": conv_ref(sd, D + f"up.{l}.upsample.conv",
-                                               F.interpolate(xu, scale_factor=2.0, mode="bilinear", align_corners=False))})
+                                               F.interpolate(xu, scale_factor=2.0, mode="bilinear", align_corners=False)),
+                          "nearest_shifted": conv_ref(sd, D + f"up.{l}.upsample.conv", nearest_shifted(xu)),
+                          **conv3_mutants(sd, D + f"up.{l}.upsample.conv", up)})
     # the AttnBlocks: norm (no activation), qkv, attention, proj_out + residual
     for P, tp, xin_name in ((E, "vae.enc.attn", "vae.enc.mid1.out"), (D, "vae.dec.attn", "vae.dec.mid1.out")):
         key = P + "mid.attn_1"
@@ -282,7 +313,7 @@ def steps(sd, v: dict, x: Tensor, msgs: Tensor, t, delta: Tensor, eps_steps=()):
         yield (tp + ".gn_out",) + gn_step(src, sd[key + ".weight"], sd[key + ".bias"], True, t[tp + ".gn_out"])
     ga = t["vae.enc.gn_out"]
     ref = conv_ref(sd, E + "conv_out", ga)
-    yield ("latent",) + (t["vae.latent"], ref, conv_bound(sd, E + "conv_out", ga, ref, out16=False), {})
+    yield ("latent",) + (t["vae.latent"], ref, conv_bound(sd, E + "conv_out", ga, ref, out16=False), conv3_mutants(sd, E + "conv_out", ga))
     lat = t["vae.latent"]
     K = msgs.shape[1]
     ax = vo.aux(sd, msgs.long(), torch.float64)
@@ -301,7 +332,8 @@ def steps(sd, v: dict, x: Tensor, msgs: Tensor, t, delta: Tensor, eps_steps=()):
     pre = conv_ref(sd, D + "conv_out", go)
     ob = conv_bound(sd, D + "conv_out", go, pre, out16=False) + 4 * U32
     fin = torch.tanh(pre) if v["tanh_out"] else pre
-    yield ("out",) + (delta, fin, ob, {"tanh_ignored": pre} if v["tanh_out"] else {})
+    yield ("out",) + (delta, fin, ob, {**({"tanh_ignored": pre} if v["tanh_out"] else {}),
+                                       **conv3_mutants(sd, D + "conv_out", go, post=torch.tanh if v["tanh_out"] else None)})
 
 
 def run_steps(sd, v, x, msgs, t, delta, log: Optional[Callable[[str], None]] = None, eps_steps=()) -> Dict[str, float]:
@@ -310,5 +342,6 @@ def run_steps(sd, v, x, msgs, t, delta, log: Optional[Callable[[str], None]] = N
     for name, got, ref, bound, mut in steps(sd, v, x, msgs, t, delta, eps_steps):
         res[name] = judge(name, got, ref, bound, mut)
         if log:
-            log(f"  {name:22s} err/bound {res[name]:.3f} " + " ".join(f"{k}:rejected" for k in mut))
+            log(f"  {name:22s} err/bound {res[name]:.3f} " +
+                " ".join(f"{k}:rejected" + (" (border only)" if k in BORDER_ONLY else "") for k in mut))
     return res

@@ -517,6 +517,14 @@ inline void setup_gather_conv(ConvGemmOp& op, int loader, const __half* src0, in
   p.num_kb = (p.Ktot + 63) / 64;
 }
 
+// stride-1 3x3 zero-padded conv of x [B][h*h][C] (pixel pitch ld), weights [N][9*C] with K order (r, s, c): the TMA conv where the
+// h x h map tiles by 128 pixels (sides 16, 32, 64 or a multiple of 128), else the gather loader, which reads the same weights (sides
+// such as 48, 80, 96, 160, 192 and 320, the maps at and below processing sizes that are odd multiples of 128).  op.loader tells which.
+inline void setup_conv3x3(ConvGemmOp& op, const __half* x, int B, int h, int C, int ld) {
+  if (h >= kBlockM ? h % kBlockM == 0 : kBlockM % h == 0 && h % (kBlockM / h) == 0) setup_tma_conv(op, x, B, h, h, C, ld, 3, 3, 1);
+  else setup_gather_conv(op, LD_GATHER_CONV, x, C, ld, nullptr, 0, 0, B, h, h, h, h, 3, 3, 1, 1, 0);
+}
+
 // launch with programmatic stream serialization: the kernel may begin while its predecessor drains and synchronises
 // itself with pdl_wait() (ptx.cuh).
 template <class... KArgs, class... Args>

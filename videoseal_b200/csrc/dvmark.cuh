@@ -173,7 +173,7 @@ void add_conv3d_sliced(Plan& pl, const ConvW& w, const __half* x, int C, int h, 
     pl.add(unit + ".tstack" + std::string(POOL ? "+pool." : ".") + std::to_string(C) + "-" + std::to_string(Cs) + "@" + std::to_string(h),
            [=](cudaStream_t st) { launch_temporal_stack(x, C, C, hw, b0, n, B, G, xs, Cs, nsm, st, POOL, h); });
     ConvGemmOp op;
-    setup_tma_conv(op, xs, n, h, h, Cs, Cs, 3, 3, 1);
+    setup_conv3x3(op, xs, n, h, Cs, Cs);
     epi(op, b0);
     vsb::add_conv(pl, op, w, name, nsm);
   }
@@ -190,7 +190,8 @@ struct DVMark {
   void set(int nb, const vsb_model_desc& d) {
     VSB_CHECK(nb >= 1, "DVMark extractor: nbits must be at least 1");
     VSB_CHECK(nb == d.nbits, "DVMark extractor: nbits must equal the descriptor's nbits");
-    // layer3's map (S / 2) tiles the tensor-core conv by 128 pixels, and layer4's (S / 4) has a row of its own per block
+    // layer2's map (S) tiles the TMA conv by 128 pixels; layer3's (S / 2) does only when S is a multiple of 256, else it runs on the
+    // gather loader (setup_conv3x3); layer4's (S / 4) has a row of its own per block
     if (d.img_size < 128 || d.img_size % 128 != 0)
       throw Error("DVMark extractor: processing size " + std::to_string(d.img_size) + " is not implemented (a positive multiple of 128)",
                   kErrUnsupported);

@@ -119,7 +119,8 @@ struct DVMarkEnc {
   void set(int nb, const vsb_model_desc& d) {
     VSB_CHECK(nb >= 1, "DVMark embedder: nbits must be at least 1");
     VSB_CHECK(nb == d.nbits, "DVMark embedder: nbits must equal the descriptor's nbits");
-    // the half-resolution maps tile the tensor-core conv by 128 pixels; above 512 a 64-frame plan outgrows the card (row a13f)
+    // the half-resolution maps tile the TMA conv by 128 pixels when S is a multiple of 256, else their convs run on the gather loader
+    // (setup_conv3x3); above 512 a 64-frame plan outgrows the card (row a13f)
     if (d.img_size < 128 || d.img_size % 128 != 0 || d.img_size > kDvEncMaxSize)
       throw Error("DVMark embedder: processing size " + std::to_string(d.img_size) + " is not implemented (a positive multiple of 128, "
                   "at most " + std::to_string(kDvEncMaxSize) + ")", kErrUnsupported);

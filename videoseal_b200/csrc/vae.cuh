@@ -447,20 +447,15 @@ struct VaeEnc {
         VSB_CUDA(cudaGetLastError());
       }, 3);
     };
-    // stride-1 3x3 conv of x [B][h*h][C]: the TMA conv where the map tiles by 128 pixels (sides 16, 32, 64 or a multiple of 128),
-    // else the gather loader, which reads the same weights: the 192 and 96 wide maps at 768, 320 / 160 / 80 at 640, 192 / 96 / 48
-    // at 384 (not measured; 256 and 512 run only the TMA conv)
-    auto setup_c3 = [&](ConvGemmOp& op, const __half* x, int h, int C) {
-      if (h >= kBlockM ? h % kBlockM == 0 : kBlockM % h == 0 && h % (kBlockM / h) == 0) setup_tma_conv(op, x, B, h, h, C, C, 3, 3, 1);
-      else setup_gather_conv(op, LD_GATHER_CONV, x, C, C, nullptr, 0, 0, B, h, h, h, h, 3, 3, 1, 1, 0);
-    };
-    // stride-1 3x3 conv x (cin) -> out (cout) + bias (+ fp16 residual)
+    // stride-1 3x3 conv (setup_conv3x3: the 192 and 96 wide maps at 768, 320 / 160 / 80 at 640 and 192 / 96 / 48 at 384 run on
+    // the gather loader; not measured) x (cin) -> out (cout) + bias (+ fp16 residual).  Gather-loader steps are named conv3x3g.
     auto add_c3 = [&](const std::string& net, const ConvW& w, const __half* x, int h, int cin, __half* out, const __half* resid) {
       ConvGemmOp op;
-      setup_c3(op, x, h, cin);
+      setup_conv3x3(op, x, B, h, cin, cin);
       op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.bias = w.bias; op.p.out16 = out; op.p.ld_out16 = w.N;
       if (resid) { op.p.resid16 = resid; op.p.ld_res16 = w.N; }
-      vsb::add_conv(pl, op, w, net + ".conv3x3" + (resid ? "+res." : ".") + std::to_string(cin) + "-" + std::to_string(w.N) + at(h), sms);
+      vsb::add_conv(pl, op, w, net + ".conv3x3" + (op.loader == LD_GATHER_CONV ? "g" : "") + (resid ? "+res." : ".") +
+                                   std::to_string(cin) + "-" + std::to_string(w.N) + at(h), sms);
     };
     // 1x1 GEMM over M rows of x (K columns) -> out (pitch N) + bias (+ fp16 residual)
     auto add_gemm = [&](const std::string& name, const ConvW& w, const __half* x, long M, __half* out, const __half* resid) {
@@ -555,9 +550,10 @@ struct VaeEnc {
       add_gn(cur, hL, CL, enc.nout, true, a);
       tap16("vae.enc.gn_out", a, hL, CL);
       ConvGemmOp op;
-      setup_c3(op, a, hL, CL);
+      setup_conv3x3(op, a, B, hL, CL, CL);
       op.p.epi = EPI_AFFINE; op.p.act = ACT_NONE; op.p.bias = e_out.bias; op.p.out32 = lat; op.p.ld_out32 = kVaeMaxZ;
-      vsb::add_conv(pl, op, e_out, "vae.enc.conv_out." + std::to_string(CL) + "-" + std::to_string(v.z_channels) + at(hL), sms);
+      vsb::add_conv(pl, op, e_out, "vae.enc.conv_out" + std::string(op.loader == LD_GATHER_CONV ? "g." : ".") + std::to_string(CL) + "-" +
+                                       std::to_string(v.z_channels) + at(hL), sms);
       pl.tap("vae.latent", lat, 0, B, hL, hL, v.z_channels, kVaeMaxZ);
     }
     // ---- message and decoder conv_in
