@@ -280,7 +280,7 @@ int vsb_ssim(const float* x_dev, const float* y_dev, int32_t B, int32_t C, int32
              float* ssim_out_dev, float* msssim_out_dev, void* workspace_dev, int64_t workspace_bytes, void* stream);
 
 /* ---- validation augmentations (handle-less)  <-  augmentation/geometric.py, valuemetric.py as get_validation_augs lists them
- * (evals/full.py:188-239).  x_dev [B,3,H,W] fp32 contiguous, y_dev [B,3,OH,OW] (OH, OW = H, W for every op but crop, resize
+ * (evals/full.py:188-239), and video.py's WindowAveraging.  x_dev [B,3,H,W] fp32 contiguous, y_dev [B,3,OH,OW] (OH, OW = H, W for every op but crop, resize
  * and the grid ops); y_dev must not overlap x_dev.  params are host floats, n_params of them:
  *   VSB_AUG_CROP_FLIP      {i, j, flip}: y = x[..., i:i+OH, j:j+OW], mirrored along W when flip != 0      (F.crop, F.hflip)
  *   VSB_AUG_GRID_*         {t00, t01, t10, t11, t20, t21, c6, c7, perspective}: torchvision's rescaled theta [3][2] (and the
@@ -294,12 +294,21 @@ int vsb_ssim(const float* x_dev, const float* y_dev, int32_t B, int32_t C, int32
  *   VSB_AUG_JPEG           {quality}: PIL's JPEG save and load (4:2:0, islow DCT, fancy upsampling), bit-exact, then the
  *                          reference's pass-through (jpeg - x) + x on the clamped input                    (utils/image.py:13-34)
  *   VSB_AUG_RESIZE         {}: bilinear, antialias=True, align_corners=False, H x W -> OH x OW           (F.resize)
+ *   VSB_AUG_WINDOW_AVG     {window, alpha, 1 - alpha}, the two blend factors rounded to fp32 from the caller's doubles: x is a
+ *                          clip of B = T frames; with w = min(window, T) and h = w / 2, frame i becomes
+ *                          (1 - alpha) x[i] + alpha mean(x[max(0, i - h) : min(T, i + h + 1)]), the mean a fresh fp32 sum in
+ *                          frame order over the count (video.py:455-485; an even window spans w + 1 frames inside the clip).
+ *                          window is an integer >= 1 and alpha finite (VSB_ERR_INVALID); w > 17 is VSB_ERR_UNSUPPORTED.
+ *                          The caller returns a clip of T <= min_window_size unchanged, as the reference's class does.
+ *                          x_dev and y_dev need only fp32 (4-byte) alignment: the 16-byte vector path is taken when both are
+ *                          16-byte aligned and 3 H W is a multiple of 4, the one-float path otherwise.
  * The caller supplies vsb_augment_workspace_bytes(op, B, H, W) bytes of device workspace (16-byte aligned; 0 = none needed).
  * Deterministic: the contrast mean is a fixed-order fp64 sum.  Runs on x_dev's device; VSB_ERR_UNSUPPORTED on anything but
  * compute capability 9.0; arguments are checked before any CUDA call. */
 enum vsb_aug_op {
   VSB_AUG_CROP_FLIP = 0, VSB_AUG_GRID_NEAREST = 1, VSB_AUG_GRID_BILINEAR = 2, VSB_AUG_BRIGHTNESS = 3, VSB_AUG_CONTRAST = 4,
-  VSB_AUG_SATURATION = 5, VSB_AUG_HUE = 6, VSB_AUG_GRAYSCALE = 7, VSB_AUG_BLUR = 8, VSB_AUG_JPEG = 9, VSB_AUG_RESIZE = 10
+  VSB_AUG_SATURATION = 5, VSB_AUG_HUE = 6, VSB_AUG_GRAYSCALE = 7, VSB_AUG_BLUR = 8, VSB_AUG_JPEG = 9, VSB_AUG_RESIZE = 10,
+  VSB_AUG_WINDOW_AVG = 11
 };
 int64_t vsb_augment_workspace_bytes(int32_t op, int32_t B, int32_t H, int32_t W);   /* host-only; < 0 on error */
 int vsb_augment(int32_t op, const float* x_dev, float* y_dev, int32_t B, int32_t C, int32_t H, int32_t W, int32_t OH, int32_t OW,

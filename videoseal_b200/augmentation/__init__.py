@@ -1,27 +1,40 @@
-"""The reference's validation augmentations (videoseal/augmentation/__init__.py, geometric.py, valuemetric.py, sequential.py) on
-the GPU.  Each class has the reference's `forward(image, mask, strength) -> (image, mask)` and `__repr__`, so that the evaluation's
-column names match; random draws (crop offsets, sizes, angles, perspective endpoints, factors) make the reference's torch.randint /
-torch.rand calls on the global CPU generator in the same order, so a seed gives the same parameters.  The pixels are computed by
-libvsb200's vsb_augment kernels (csrc/augment.cuh) on CUDA tensors; CPU tensors raise, as everywhere in this package.  Masks
-([B, 1, H, W]) go through the geometric ops.  The video codecs (H264, H264rgb, H265, VP9, AV1) need ffmpeg and raise
-NotImplementedError."""
+"""The reference's validation augmentations (videoseal/augmentation/__init__.py, geometric.py, valuemetric.py, sequential.py, and
+the temporal attacks of video.py) on the GPU.  Each class has the reference's `forward(image, mask, strength) -> (image, mask)`
+and `__repr__`, so that the evaluation's column names match; random draws (crop offsets, sizes, angles, perspective endpoints,
+factors) make the reference's torch.randint / torch.rand calls on the global CPU generator in the same order, so a seed gives the
+same parameters.  The pixels are computed by libvsb200's vsb_augment kernels (csrc/augment.cuh) on CUDA tensors; CPU tensors
+raise, as everywhere in this package.  Masks ([B, 1, H, W]) go through the geometric ops.  The video codecs (H264, H264rgb, H265,
+VP9, AV1) need ffmpeg and raise NotImplementedError.
+
+The temporal attacks take a clip [T, 3, H, W] and draw from Python's `random` module in the reference's order, so that
+random.seed(s) gives the reference's parameters.  SpeedChange, TemporalReorder and DropFrame re-index frames: the index table is
+built on the host with the reference's arithmetic and applied on the device with index_select, so the frame count may change
+(speed 0.5 doubles it).  WindowAveraging blends each frame with the mean of its temporal window in vsb_augment's window kernel.
+Masks move with the frames of SpeedChange and TemporalReorder; DropFrame and WindowAveraging return the mask unchanged, as the
+reference does.  A tuple strength is unpacked into the forward's parameters in order: (window_size, alpha) and (chunk_size, swap_probability), as
+the reference's commented-out video rows mean them."""
 from __future__ import annotations
 
 import ctypes as C
 import math
+import random
 
 import torch
 
 from .. import _lib
 
 OPS = {"crop_flip": 0, "grid_nearest": 1, "grid_bilinear": 2, "brightness": 3, "contrast": 4, "saturation": 5, "hue": 6,
-       "grayscale": 7, "blur": 8, "jpeg": 9, "resize": 10}
+       "grayscale": 7, "blur": 8, "jpeg": 9, "resize": 10, "window_avg": 11}
+
+
+def _require_cuda(x: torch.Tensor):
+    if not x.is_cuda:
+        raise RuntimeError("videoseal_b200.augmentation runs on CUDA tensors only (no CPU fallback)")
 
 
 def apply(op: str, x: torch.Tensor, out_hw=None, params=(), aux: torch.Tensor | None = None) -> torch.Tensor:
     """One vsb_augment call on a CUDA fp32 [B, 3, H, W] tensor; returns [B, 3, OH, OW]."""
-    if not x.is_cuda:
-        raise RuntimeError("videoseal_b200.augmentation runs on CUDA tensors only (no CPU fallback)")
+    _require_cuda(x)
     if x.dim() != 4 or x.shape[1] != 3:
         raise ValueError(f"expected a [B, 3, H, W] tensor, got {tuple(x.shape)}")
     x = x.float().contiguous()
@@ -382,8 +395,161 @@ class AV1(_Codec):
     name = "AV1"
 
 
+class _Temporal(_Aug):
+    """A clip [T, 3, H, W] in, a clip out; a tuple strength fills the forward's parameters in order."""
+
+    def __call__(self, frames, mask=None, *args):
+        if len(args) == 1 and isinstance(args[0], tuple):
+            args = args[0]
+        return self.forward(frames, mask, *args)
+
+
+def _reindex(frames, mask, idx):
+    """frames[idx] and mask[idx] on the device; idx None returns both unchanged"""
+    if idx is None:
+        return frames, mask
+    idx = idx.to(frames.device)
+    return frames.index_select(0, idx), (mask.index_select(0, idx) if mask is not None else None)
+
+
+class SpeedChange(_Temporal):
+    def __init__(self, min_speed=0.5, max_speed=1.5):
+        self.min_speed, self.max_speed = min_speed, max_speed
+
+    def get_random_speed(self):
+        if self.min_speed is None or self.max_speed is None:
+            raise ValueError("min_speed and max_speed must be provided")
+        return random.uniform(self.min_speed, self.max_speed)
+
+    def get_indices(self, num_frames: int, speed_factor=None):
+        """The frame table of forward (video.py:292-307), or None where the reference returns its input: an fp32 linspace,
+        rounded and clamped; a speed-up keeps its first num_frames entries."""
+        speed_factor = speed_factor if speed_factor is not None else self.get_random_speed()
+        if speed_factor == 1.0:
+            return None
+        if speed_factor < 1.0:
+            return torch.linspace(0, num_frames - 1, int(num_frames / speed_factor)).round().long().clamp(0, num_frames - 1)
+        idx = torch.linspace(0, num_frames - 1, int(num_frames * speed_factor))
+        return idx[:num_frames].round().long().clamp(0, num_frames - 1)
+
+    def forward(self, frames, mask=None, speed_factor=None, *args, **kwargs):
+        _require_cuda(frames)
+        return _reindex(frames, mask, self.get_indices(frames.shape[0], speed_factor))
+
+    def __repr__(self):
+        return f"SpeedChange(min_speed={self.min_speed}, max_speed={self.max_speed})"
+
+
+class TemporalReorder(_Temporal):
+    def __init__(self, min_chunk_size=2, max_chunk_size=5, reorder_prob=0.5):
+        self.min_chunk_size, self.max_chunk_size, self.reorder_prob = min_chunk_size, max_chunk_size, reorder_prob
+
+    def get_random_chunk_size(self):
+        if self.min_chunk_size is None or self.max_chunk_size is None:
+            raise ValueError("min_chunk_size and max_chunk_size must be provided")
+        return random.randint(self.min_chunk_size, self.max_chunk_size)
+
+    def get_indices(self, num_frames: int, chunk_size=None, swap_probability=None):
+        """The frame table of forward (video.py:352-405), or None where the reference returns its input: one random.random() per
+        chunk pair swaps the pair; the frames after the last whole chunk stay."""
+        chunk_size = chunk_size if chunk_size is not None else self.get_random_chunk_size()
+        swap_probability = swap_probability if swap_probability is not None else self.reorder_prob
+        if num_frames < chunk_size * 2:
+            return None
+        num_chunks = num_frames // chunk_size
+        order = list(range(num_chunks))
+        for i in range(0, num_chunks - 1, 2):
+            if random.random() < swap_probability and i + 1 < num_chunks:
+                order[i], order[i + 1] = order[i + 1], order[i]
+        usable = num_chunks * chunk_size
+        return torch.tensor([c * chunk_size + k for c in order for k in range(chunk_size)] + list(range(usable, num_frames)))
+
+    def forward(self, frames, mask=None, chunk_size=None, swap_probability=None, *args, **kwargs):
+        _require_cuda(frames)
+        return _reindex(frames, mask, self.get_indices(frames.shape[0], chunk_size, swap_probability))
+
+    def __repr__(self):
+        return (f"TemporalReorder(min_chunk_size={self.min_chunk_size}, max_chunk_size={self.max_chunk_size}, "
+                f"reorder_prob={self.reorder_prob})")
+
+
+class WindowAveraging(_Temporal):
+    def __init__(self, min_window_size=2, max_window_size=5, min_alpha=0.3, max_alpha=0.7):
+        self.min_window_size, self.max_window_size = min_window_size, max_window_size
+        self.min_alpha, self.max_alpha = min_alpha, max_alpha
+
+    def get_random_window_size(self):
+        if self.min_window_size is None or self.max_window_size is None:
+            raise ValueError("min_window_size and max_window_size must be provided")
+        return random.randint(self.min_window_size, self.max_window_size)
+
+    def get_random_alpha(self):
+        if self.min_alpha is None or self.max_alpha is None:
+            raise ValueError("min_alpha and max_alpha must be provided")
+        return random.uniform(self.min_alpha, self.max_alpha)
+
+    def get_params(self, num_frames: int, window_size=None, alpha=None):
+        """(min(window_size, num_frames), alpha) as forward draws them (video.py:455-464), or None where the reference returns its
+        input: a clip of at most min_window_size frames, the class's minimum and not the given window."""
+        if num_frames <= self.min_window_size:
+            return None
+        window_size = window_size if window_size is not None else self.get_random_window_size()
+        alpha = alpha if alpha is not None else self.get_random_alpha()
+        if window_size != int(window_size):
+            raise ValueError(f"window_size ({window_size}) must be an integer")
+        return min(int(window_size), num_frames), alpha      # video.py:463
+
+    def forward(self, frames, mask=None, window_size=None, alpha=None, *args, **kwargs):
+        _require_cuda(frames)
+        p = self.get_params(frames.shape[0], window_size, alpha)
+        if p is None:
+            return frames, mask
+        # the blend factors round as torch rounds the Python scalars
+        return apply("window_avg", frames, None, (p[0], _f32(p[1]), _f32(1 - p[1]))), mask
+
+    def __repr__(self):
+        return f"WindowAveraging(min_window={self.min_window_size}, max_window={self.max_window_size})"
+
+
+class DropFrame(_Temporal):
+    def __init__(self, drop_frame_prob=0.125):
+        self.drop_frame_prob = drop_frame_prob
+
+    def get_random_drop_prob(self):
+        return self.drop_frame_prob
+
+    def get_indices(self, num_frames: int, drop_prob=None):
+        """The frame table of forward (video.py:516-525): one random.random() per frame, and one more for the direction of each
+        dropped frame's neighbour, which wraps."""
+        drop_prob = drop_prob if drop_prob is not None else self.drop_frame_prob
+        idx = list(range(num_frames))
+        for i in range(num_frames):
+            if random.random() >= drop_prob:
+                continue
+            idx[i] = (i + (-1 if random.random() < 0.5 else 1)) % num_frames
+        return torch.tensor(idx)
+
+    def forward(self, frames, mask=None, drop_prob=None, *args, **kwargs):
+        """The mask comes back unchanged, as in the reference."""
+        _require_cuda(frames)
+        return _reindex(frames, None, self.get_indices(frames.shape[0], drop_prob))[0], mask
+
+    def __repr__(self):
+        return f"DropFrame(prob={self.drop_frame_prob})"
+
+
 def _has_codec(augs) -> bool:
     return any(isinstance(a, _Codec) or (isinstance(a, Sequential) and _has_codec([(t, None) for t in a.transforms])) for a, _ in augs)
+
+
+def _video_augs() -> list:
+    """The reference's full video validation list (augmentation/__init__.py:76-105)."""
+    return [
+        (Identity(), [0]), (HorizontalFlip(), [0]), (Rotate(), [10, 90]), (Resize(), [0.55, 0.71]), (Crop(), [0.55, 0.71]),
+        (Perspective(), [0.5]), (Brightness(), [0.5, 1.5]), (Contrast(), [0.5, 1.5]), (Saturation(), [0.5, 1.5]), (Hue(), [0.25]),
+        (Grayscale(), [-1]), (JPEG(), [40]), (GaussianBlur(), [9]), (H264(), [23, 30, 40, 50]), (H264rgb(), [23, 30, 40, 50]),
+        (H265(), [23, 30, 40, 50]), (VP9(), [-1]),
+    ] + [(Sequential(H264(), Crop(), Brightness()), [(crf, 0.71, 0.5)]) for crf in (23, 30, 40, 50)]
 
 
 def get_validation_augs(is_video: bool = False, only_identity: bool = False, only_combined: bool = False) -> list:
@@ -398,12 +564,7 @@ def get_validation_augs(is_video: bool = False, only_identity: bool = False, onl
         else:
             augs = [(Identity(), [0]), (Sequential(JPEG(), Crop(), Brightness()), [(40, 0.71, 0.5)])]
     elif is_video:
-        augs = [
-            (Identity(), [0]), (HorizontalFlip(), [0]), (Rotate(), [10, 90]), (Resize(), [0.55, 0.71]), (Crop(), [0.55, 0.71]),
-            (Perspective(), [0.5]), (Brightness(), [0.5, 1.5]), (Contrast(), [0.5, 1.5]), (Saturation(), [0.5, 1.5]), (Hue(), [0.25]),
-            (Grayscale(), [-1]), (JPEG(), [40]), (GaussianBlur(), [9]), (H264(), [23, 30, 40, 50]), (H264rgb(), [23, 30, 40, 50]),
-            (H265(), [23, 30, 40, 50]), (VP9(), [-1]),
-        ] + [(Sequential(H264(), Crop(), Brightness()), [(crf, 0.71, 0.5)]) for crf in (23, 30, 40, 50)]
+        augs = _video_augs()
     else:
         augs = [
             (Identity(), [0]), (HorizontalFlip(), [0]), (Rotate(), [5, 10, 30, 45, 90]),
@@ -419,6 +580,13 @@ def get_validation_augs(is_video: bool = False, only_identity: bool = False, onl
         raise NotImplementedError("this validation list holds video codecs (H264 / H265 / VP9), which need ffmpeg; "
                                   "pass an explicit list of augmentations instead")
     return augs
+
+
+def get_codec_free_video_augs() -> list:
+    """The reference's video validation list without its codec rows and codec Sequentials, followed by the four temporal attacks
+    with the strengths of the list's commented-out block (augmentation/__init__.py:100-104)."""
+    return [(a, s) for a, s in _video_augs() if not _has_codec([(a, s)])] + [
+        (SpeedChange(), [0.5, 2.0]), (WindowAveraging(), [(3, 1.0)]), (DropFrame(), [0.2, 0.5]), (TemporalReorder(), [(4, 0.7)])]
 
 
 def column_key(aug, strength) -> str:

@@ -11,6 +11,7 @@
 //   aug_blur_h/v_kernel   F.gaussian_blur: the separable form of the 2-D kernel torchvision builds, reflect padding
 //   jpeg_mcu_kernel       PIL's JPEG save at quality q (libjpeg-turbo: 4:2:0, islow DCT) and its decode, up to the chroma
 //   jpeg_rgb_kernel       upsampling: integer arithmetic throughout, so the round trip is bit-exact (tests/jpeg_oracle.py)
+//   aug_window_avg_kernel video.py's WindowAveraging: each frame blended with the mean of its temporal window, one pass over the clip
 // Every fp32 expression that has to match torchvision's rounding is written with __f*_rn intrinsics so that nvcc cannot contract it.
 #pragma once
 #include <cuda_runtime.h>
@@ -217,6 +218,67 @@ __global__ void __launch_bounds__(256) aug_blur_v_kernel(const float* __restrict
     float acc = 0.f;
     for (int j = 0; j < t.k; ++j) acc = __fmaf_rn(t.w[j], __ldg(x + plane + (int64_t)aug_reflect(r + j - pad, H) * W + c), acc);
     y[plane + k] = acc;
+  }
+}
+
+// ---------------------------------------------------------------- temporal window averaging
+// The reference's WindowAveraging (augmentation/video.py:455-485) on a clip x [T, n] (n = 3 H W floats per frame), with
+// HH = window // 2 after window = min(window, T):
+//   y[i] = (1 - alpha) x[i] + alpha mean(x[max(0, i - HH) : min(T, i + HH + 1)])
+// The mean is what torch.mean computes there: a fresh fp32 sum of the window's frames in frame order, divided by their count; the
+// blend is the three rounded operations of the Python expression, with a_keep = fp32(1 - alpha) and a_avg = fp32(alpha).
+// Each thread owns one VEC-float vector of a frame position and walks the T frames, keeping the 2 HH + 1 newest frame vectors in a
+// register ring (frame j in slot j % K), so every input byte is read once and every output byte written once.  The time loop is
+// unrolled by K so that every slot index is a compile-time constant.
+template <int VEC> struct AugVec;
+template <> struct AugVec<4> { using T = float4; };
+template <> struct AugVec<1> { using T = float; };
+
+template <int VEC>
+__device__ __forceinline__ void aug_vadd(float* s, const typename AugVec<VEC>::T& v) {
+  const float* f = reinterpret_cast<const float*>(&v);
+#pragma unroll
+  for (int e = 0; e < VEC; ++e) s[e] = __fadd_rn(s[e], f[e]);
+}
+
+constexpr int kAugMaxHalfWindow = 8;   // windows of up to 17 frames
+
+template <int HH, int VEC>
+__global__ void __launch_bounds__(256) aug_window_avg_kernel(const float* __restrict__ x, float* __restrict__ y, int T, int64_t nvec,
+                                                             float a_keep, float a_avg) {
+  using V = typename AugVec<VEC>::T;
+  constexpr int K = 2 * HH + 1;
+  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= nvec) return;
+  const V* src = reinterpret_cast<const V*>(x) + p;
+  V* dst = reinterpret_cast<V*>(y) + p;
+  V ring[K];
+#pragma unroll
+  for (int j = 0; j < HH; ++j)
+    if (j < T) ring[j] = __ldg(src + (int64_t)j * nvec);
+  for (int i0 = 0; i0 < T; i0 += K) {
+#pragma unroll
+    for (int s = 0; s < K; ++s) {
+      const int i = i0 + s;
+      if (i < T) {
+        if (i + HH < T) ring[(s + HH) % K] = __ldg(src + (int64_t)(i + HH) * nvec);
+        float sum[VEC];
+#pragma unroll
+        for (int e = 0; e < VEC; ++e) sum[e] = 0.f;
+#pragma unroll
+        for (int k = 0; k < K; ++k) {          // frames i - HH .. i + HH, in order
+          const int j = i - HH + k;
+          if (j >= 0 && j < T) aug_vadd<VEC>(sum, ring[(s + k + K - HH % K) % K]);
+        }
+        const float cnt = (float)(min(T, i + HH + 1) - max(0, i - HH));
+        const float* xi = reinterpret_cast<const float*>(&ring[s % K]);
+        V o;
+        float* of = reinterpret_cast<float*>(&o);
+#pragma unroll
+        for (int e = 0; e < VEC; ++e) of[e] = __fadd_rn(__fmul_rn(a_keep, xi[e]), __fmul_rn(a_avg, __fdiv_rn(sum[e], cnt)));
+        dst[(int64_t)i * nvec] = o;
+      }
+    }
   }
 }
 

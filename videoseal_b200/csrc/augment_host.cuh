@@ -2,7 +2,9 @@
 // launches of one call.
 #pragma once
 #include <algorithm>
+#include <cmath>
 #include <string>
+#include <type_traits>
 #include "augment.cuh"
 #include "plan.cuh"
 #include "resize_blend_host.cuh"
@@ -20,7 +22,7 @@ inline size_t aug_align(size_t n) { return (n + 255) & ~(size_t)255; }
 // Workspace bytes of one call (0 when the op needs none); throws Error(kErrInvalid) on a bad op or shape.
 inline size_t aug_workspace_bytes(int op, int B, int H, int W) {
   VSB_CHECK(B >= 1 && H >= 1 && W >= 1, "augment: B, H and W must be positive");
-  VSB_CHECK(op >= VSB_AUG_CROP_FLIP && op <= VSB_AUG_RESIZE, "augment: unknown op");
+  VSB_CHECK(op >= VSB_AUG_CROP_FLIP && op <= VSB_AUG_WINDOW_AVG, "augment: unknown op");
   const int64_t HW = (int64_t)H * W;
   if (op == VSB_AUG_CONTRAST) return aug_align((size_t)B * aug_sum_blocks(HW) * sizeof(double));
   if (op == VSB_AUG_BLUR) return aug_align((size_t)B * 3 * HW * sizeof(float));
@@ -57,6 +59,16 @@ inline void aug_check(int op, int B, int C, int H, int W, int OH, int OW, const 
       need(1);
       VSB_CHECK(params[0] >= 1.f && params[0] <= 100.f && params[0] == (float)(int)params[0], "augment: JPEG quality must be an integer in 1..100");
       break;
+    case VSB_AUG_WINDOW_AVG: {
+      need(3);
+      VSB_CHECK(params[0] >= 1.f && params[0] <= 16777216.f && params[0] == std::floor(params[0]), "augment: the averaging window must be an integer >= 1");
+      VSB_CHECK(std::isfinite(params[1]) && std::isfinite(params[2]), "augment: the window-averaging alpha must be finite");
+      const int64_t window = std::min<int64_t>((int64_t)params[0], B);
+      if (window / 2 > kAugMaxHalfWindow)
+        throw Error("augment: window averaging implements windows of at most " + std::to_string(2 * kAugMaxHalfWindow + 1) +
+                        " frames (after window = min(window, T)); got " + std::to_string(window), kErrUnsupported);
+      break;
+    }
     default: break;
   }
   if (op != VSB_AUG_CROP_FLIP && op != VSB_AUG_GRID_NEAREST && op != VSB_AUG_GRID_BILINEAR && op != VSB_AUG_RESIZE)
@@ -141,6 +153,35 @@ inline void aug_run(int op, const float* x, float* y, int B, int H, int W, int O
       const std::string variant = ".mt" + std::to_string(resize_mt(r)) + "g" + std::to_string(r.gstage);
       prof_scope("aug.resize" + variant + tag, st, 1, [&] { launch_resize(r, x, 3 * HW, B, H, W, OH, OW, y, rec, st); });
       VSB_CUDA(cudaStreamSynchronize(st));   // the tables are freed with r
+      break;
+    }
+    case VSB_AUG_WINDOW_AVG: {
+      // x is a clip of B = T frames; a thread per VEC-float vector of a frame: float4 when a frame is a whole number of them and x
+      // and y are 16-byte aligned (a contiguous fp32 view may start at any 4-byte offset), one float otherwise
+      const int T = B, hh = (int)(std::min<int64_t>((int64_t)params[0], T) / 2);
+      const int64_t n = 3 * HW;
+      const bool v4 = n % 4 == 0 && (reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) % 16 == 0;
+      const int64_t nvec = v4 ? n / 4 : n;
+      const unsigned blocks = (unsigned)((nvec + 255) / 256);
+      const float a_avg = params[1], a_keep = params[2];
+      auto go = [&](auto hc) {
+        constexpr int HH = decltype(hc)::value;
+        prof_scope("aug.window_avg.h" + std::to_string(HH) + (v4 ? ".v4" : ".v1") + tag, st, 1, [&] {
+          if (v4) aug_window_avg_kernel<HH, 4><<<blocks, 256, 0, st>>>(x, y, T, nvec, a_keep, a_avg);
+          else aug_window_avg_kernel<HH, 1><<<blocks, 256, 0, st>>>(x, y, T, nvec, a_keep, a_avg);
+        });
+      };
+      switch (hh) {
+        case 0: go(std::integral_constant<int, 0>{}); break;
+        case 1: go(std::integral_constant<int, 1>{}); break;
+        case 2: go(std::integral_constant<int, 2>{}); break;
+        case 3: go(std::integral_constant<int, 3>{}); break;
+        case 4: go(std::integral_constant<int, 4>{}); break;
+        case 5: go(std::integral_constant<int, 5>{}); break;
+        case 6: go(std::integral_constant<int, 6>{}); break;
+        case 7: go(std::integral_constant<int, 7>{}); break;
+        default: go(std::integral_constant<int, kAugMaxHalfWindow>{}); break;
+      }
       break;
     }
     default: break;

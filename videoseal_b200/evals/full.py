@@ -7,7 +7,10 @@ image_metrics=("psnr", "ssim", "msssim") gives the reference's columns (full.py:
 With only_identity=False each item's imgs_w also goes through the reference's validation bank (augmentation.get_validation_augs,
 run by the GPU kernels of videoseal_b200.augmentation) at frame resolution before detection, and every (augmentation, strength)
 adds its `bit_acc_<key>` / `pvalue_<key>` / `log_pvalue_<key>` / `capacity_<key>` group in the reference's order and key rule
-(full.py:188-239).  Deviation: only_identity defaults to True here (the reference's default is False), so that a default run keeps
+(full.py:188-239).  Every non-identity video list of the reference holds a codec, so a video run takes an explicit list; the CLI's
+--codec_free_video True passes augmentation.get_codec_free_video_augs(): the reference's video list without its codecs, plus the
+temporal attacks (SpeedChange, WindowAveraging, DropFrame, TemporalReorder) that may change the clip's frame count before
+extract_message.  Deviation: only_identity defaults to True here (the reference's default is False), so that a default run keeps
 its Identity-only columns; `extract_time` times the Identity detection.  The video codecs (H264 / H265 / VP9), LPIPS / VMAF, the
 detection (mask IoU) columns and the image dumps need packages outside this path."""
 from __future__ import annotations
@@ -141,14 +144,22 @@ def main(argv=None):
     ap.add_argument("--only_identity", type=_bool, default=True,
                     help="only the Identity rows (the reference defaults to False: the whole validation bank)")
     ap.add_argument("--only_combined", type=_bool, default=False, help="with --only_identity False: only the combined augmentations")
+    ap.add_argument("--codec_free_video", type=_bool, default=False,
+                    help="with --is_video True --only_identity False: the video bank without its codecs, plus the temporal attacks")
     add_interpolation_args(ap)
     a = ap.parse_args(argv)
+    augs = None
+    if a.codec_free_video:
+        if not a.is_video or a.only_identity or a.only_combined:
+            ap.error("--codec_free_video True needs --is_video True --only_identity False (and not --only_combined)")
+        from ..augmentation import get_codec_free_video_augs
+        augs = get_codec_free_video_augs()
     model = setup_model_from_checkpoint(a.checkpoint).eval().to(a.device)
     if a.scaling_w is not None:
         model.blender.scaling_w = float(a.scaling_w)
     rows = evaluate(model, synthetic_items(a.num_samples, a.is_video, a.num_frames, a.size[0], a.size[-1], a.device), a.is_video,
                     a.output_dir, a.num_frames, a.video_aggregation, interpolation=interpolation_of(a), lowres_attenuation=a.lowres_attenuation,
-                    image_metrics=a.image_metrics, only_identity=a.only_identity, only_combined=a.only_combined)
+                    image_metrics=a.image_metrics, only_identity=a.only_identity, only_combined=a.only_combined, validation_augs=augs)
     keys = [k for k in rows[0] if k not in ("iteration", "t", "h", "w")]
     print({k: sum(r[k] for r in rows) / len(rows) for k in keys})
 
