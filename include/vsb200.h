@@ -379,6 +379,8 @@ typedef struct vsb_conv_test {
   int32_t* kernel_ran;       /* if not null (host memory): receives 1 or 2, the kernel this call launched */
   int32_t grn_part;          /* with grn_stats: 1 = per-32-row partial rows [M / 32][N] (stored, no atomics), 0 = [samples][N] (atomics) */
   int32_t w_samples;         /* > 1: weights are [w_samples][N][K], sample = GEMM row / rows_per_sample (0 or 1: one weight matrix) */
+  int32_t longk_block_n;     /* the 256-row long-K kernel's tile width: 0 = the one the library selects, 128 or 192 = that one (an
+                              * error with kernel = 2 unless the op can run at it); block_n sets the 128-row kernel's */
 } vsb_conv_test;
 int vsb_debug_conv(const vsb_conv_test* t, void* stream);
 /* host-only (no GPU needed): the separable table the resize kernels use along one axis of length `in` -> `out`, i.e. the library's

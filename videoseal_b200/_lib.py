@@ -66,7 +66,7 @@ class ConvTest(C.Structure):
         ("out16", C.c_void_p), ("out32", C.c_void_p), ("delta", C.c_void_p), ("grn_stats", C.c_void_p),
         ("ld0", C.c_int32), ("ldw", C.c_int32), ("ld_out", C.c_int32),
         ("kernel", C.c_int32), ("kernel_ran", C.POINTER(C.c_int32)),
-        ("grn_part", C.c_int32), ("w_samples", C.c_int32),
+        ("grn_part", C.c_int32), ("w_samples", C.c_int32), ("longk_block_n", C.c_int32),
     ]
 
 

@@ -1090,10 +1090,16 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 // main loop (the producer keeps filling the ring meanwhile).  The K-block order, the k16 order inside a block, the epilogue
 // arithmetic and the order of the GRN row sums (32 rows paired by row bit 4, 3, 2, 1, 0) are those of conv_gemm_kernel's lean
 // paths: both kernels produce the same bits.
+//
+// BN = 192 (lean affine epilogue only): a K block moves 32 KB of A and 24 KB of B for 6.3 MFLOP, 0.78x the operand bytes per FLOP of
+// BN = 128.  Shared memory: 1 KB barriers + 3 stages x 56 KB + 8 warps x 6 KB staging (one chain's [16 rows][192] fp16) = 217 KB,
+// + 1 KB alignment slack <= 227 KB.  Each consumer thread holds 2 x 96 accumulators in the 232 registers setmaxnreg gives it.
 constexpr int kLongM = 256;
 constexpr int kLongThreads = 384;
 constexpr int kLongHeaderBytes = 1024;                // full / empty barriers
-constexpr uint32_t kLongOstWarpBytes = 16 * kMaxBlockN * 2;   // staging of one consumer warp: one chain's [16 rows][BN] fp16
+constexpr int kLongWideN = 192;                       // the widest block_n (lean affine epilogue only)
+// staging of one consumer warp: one chain's [16 rows][BN] fp16, 4 KB for every block_n up to 128 and 6 KB at kLongWideN
+__host__ __device__ constexpr uint32_t long_ost_warp_bytes(int bn) { return 16u * (uint32_t)(bn > kMaxBlockN ? bn : kMaxBlockN) * 2u; }
 constexpr int kLongConsumerWarps = 8;
 
 // read-only global loads that keep their place among the barrier / wgmma statements
@@ -1179,7 +1185,7 @@ conv_gemm_longk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     constexpr int kBoxCols = BN % 64 == 0 ? 64 : 16;
     constexpr uint32_t kBoxRowB = kBoxCols * 2, kBoxBytes = 8 * kBoxRowB;
     const uint32_t swz_x = kBoxCols == 64 ? (uint32_t)rl : (uint32_t)((rl >> 2) & 1);
-    uint8_t* ost = smem + p.ostage_off + (size_t)(warp - 4) * kLongOstWarpBytes;
+    uint8_t* ost = smem + p.ostage_off + (size_t)(warp - 4) * long_ost_warp_bytes(BN);
     auto box_ptr = [&](int j /*8-column group*/, int hh) -> uint8_t* {
       return ost + (uint32_t)(((8 * j) / kBoxCols) * 2 + hh) * kBoxBytes + (uint32_t)rl * kBoxRowB +
              (((uint32_t)(((8 * j) % kBoxCols) >> 3) ^ swz_x) << 4) + 4u * q;
@@ -1192,7 +1198,7 @@ conv_gemm_longk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     // residual half2 of step t + 1 are loaded while step t is converted.  Only two steps' worth sit in registers beside the
     // 2 x BN / 2 accumulators (the whole tile's would not fit), and the loads are ordered statements so that they stay where they
     // are put.
-    constexpr int kGrp = BN % 32 == 0 ? 4 : 5, kSteps = BN / 8 / kGrp;     // steps per chain
+    constexpr int kGrp = BN > kMaxBlockN ? 2 : (BN % 32 == 0 ? 4 : 5), kSteps = BN / 8 / kGrp;     // steps per chain
     static_assert(kGrp * kSteps * 8 == BN, "block_n must split into whole epilogue steps");
     float2 gb0[kGrp], gb1[kGrp];
     uint32_t gr0[2 * kGrp], gr1[2 * kGrp];
@@ -1203,7 +1209,9 @@ conv_gemm_longk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       const long m_warp = (long)m_tile * kLongM + h * 128 + wq * 32;     // first of this warp's 32 rows
       int prev = -1;
       for (int kb = 0; kb < p.num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
+        // 192 accumulators per thread only stay in registers with the watchdog's trap out of line (mbar_wait_cold_trap)
+        if constexpr (BN > kMaxBlockN) mbar_wait_cold_trap(&full_bar[stage], phase);
+        else mbar_wait(&full_bar[stage], phase);
         const uint32_t sa = smem_u32(tiles + (size_t)stage * p.stage_bytes);
         const uint64_t adesc0 = make_smem_desc(sa + a_off, kRowBytes, 16 * kRowBytes);
         const uint64_t adesc1 = make_smem_desc(sa + a_off + 8u * kRowBytes, kRowBytes, 16 * kRowBytes);

@@ -147,12 +147,15 @@ inline bool longk_conv_tile(int H, int W, int& tile_w, int& tile_h) {
 // The output-tile width the long-K kernel would run this op at, or 0 when it cannot run it.  Everything but the tile count: a
 // TMA-fed op with 64-wide K blocks in whole 256-row tiles, and one of the kernel's epilogues at a width it is instantiated for:
 //   - the lean affine one (bias, ReLU or none, optional fp16 residual, fp16 output) on long main loops, at the 128-row kernel's
-//     block_n (128 or 80);
+//     block_n (128 or 80), or at kLongWideN (192) where that block_n is 128, N splits into 192-wide tiles and those still make
+//     at least two tiles per SM: a 256 x 192 tile moves 56 KB per K block for 3.1 M MACs where 256 x 128 moves 48 KB for 2.1 M;
 //   - ConvNeXt pwconv1: bias + GELU, fp16 output, GRN statistics as per-32-row partial rows, block_n 128 (the float-atomic GRN
 //     mode and GELU GEMMs without GRN, the ViT MLP, stay on the 128-row kernel: not measured on this one);
 //   - ConvNeXt pwconv2: no activation, fp32 residual stream updated in place, optional fp16 copy, per-sample weights whose samples
 //     are whole 256-row tiles, block_n 128 or 96.
-inline int longk_block_n(const ConvGemmOp& op, int N, int block_n_override) {
+// longk_bn (test seam of vsb_debug_conv): 0 = choose as above, else the long-K width to take (0 is returned when the op cannot run
+// at it).  It does not change the 128-row kernel's block_n, which block_n_override sets.
+inline int longk_block_n(const ConvGemmOp& op, int N, int block_n_override, int num_sms, int longk_bn = 0) {
   const ConvGemmParams& p = op.p;
   int tw, th;
   if (!(op.loader == LD_TMA && op.a_rank != 0 && p.kblk == 64 && p.num_kb >= 2 && p.epi == EPI_AFFINE && p.outc_w == nullptr &&
@@ -175,8 +178,11 @@ inline int longk_block_n(const ConvGemmOp& op, int N, int block_n_override) {
              op.w_samples == 1 && (p.resid16 == nullptr || ((reinterpret_cast<uintptr_t>(p.resid16) & 3) == 0 && p.ld_res16 % 8 == 0)) &&
              (p.block_n == 128 || p.block_n == 80)) {
     bn = p.block_n;
+    if (bn == 128 && block_n_override == 0 && N % kLongWideN == 0 &&
+        (longk_bn == kLongWideN || (longk_bn == 0 && (long)(p.M / kLongM) * (N / kLongWideN) >= 2L * num_sms)))
+      bn = kLongWideN;
   }
-  if (bn == 0 || N % bn != 0 || (block_n_override != 0 && block_n_override != bn)) return 0;
+  if (bn == 0 || N % bn != 0 || (block_n_override != 0 && block_n_override != bn) || (longk_bn != 0 && longk_bn != bn)) return 0;
   return bn;
 }
 
@@ -205,10 +211,12 @@ inline void finalize_longk(ConvGemmOp& op, const __half* W, int N, int Kw, int l
   p.a_stage_bytes = (uint32_t)(kLongM * 64 * 2);
   p.b_stage_bytes = (uint32_t)(p.block_n * 64 * 2);
   p.stage_bytes = p.a_stage_bytes + ((p.b_stage_bytes + 1023u) & ~1023u);
-  // shared memory: [barriers | stages x (A|B) | staging boxes of the 8 consumer warps (fp16 outputs)]; 4 stages of 48 KB at
-  // block_n 128.  The fp32 residual-stream epilogue stores from registers and spends the staging bytes on a pipeline stage.
+  // shared memory: [barriers | stages x (A|B) | staging boxes of the 8 consumer warps (fp16 outputs)] within 226 KB:
+  //   block_n 128: 1 KB + 4 x 48 KB + 8 x 4 KB = 225 KB;  block_n 192: 1 KB + 3 x 56 KB + 8 x 6 KB = 217 KB
+  // (+ 1 KB alignment slack, <= 227 KB).  The fp32 residual-stream epilogue stores from registers and spends the staging bytes on
+  // a pipeline stage.
   const bool staged = p.resid32 == nullptr;
-  const size_t ostage_total = staged ? (size_t)kLongConsumerWarps * kLongOstWarpBytes : 0;
+  const size_t ostage_total = staged ? (size_t)kLongConsumerWarps * long_ost_warp_bytes(p.block_n) : 0;
   int stages = (int)((226 * 1024 - kLongHeaderBytes - ostage_total) / p.stage_bytes);
   if (stages > kMaxStages) stages = kMaxStages;
   VSB_CHECK(stages >= 3, "long-K tile does not fit in shared memory");
@@ -234,7 +242,7 @@ inline void finalize_longk(ConvGemmOp& op, const __half* W, int N, int Kw, int l
 // Common finalisation: weights map, tiling, stage count, smem, grid.
 // W: [N, Kw] fp16 row-major (K-major), Kw >= num_kb*kblk need not hold (TMA zero-fills out-of-bounds K).
 inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw, int num_sms, int block_n_override = 0,
-                        int kernel_sel = kKernelAuto) {
+                        int kernel_sel = kKernelAuto, int longk_bn = 0) {
   ConvGemmParams& p = op.p;
   p.N = N;
   // block_n <= 128: the two MMA warpgroups hold a 128 x block_n fp32 accumulator in registers (block_n / 2 per thread); an fp32
@@ -247,7 +255,7 @@ inline void finalize_op(ConvGemmOp& op, const __half* W, int N, int Kw, int ldw,
     // machine better: it has twice the tiles to spread, and the last wave of 256-row tiles would leave SMs idle for a whole
     // 256-row main loop.  (Not measured below the threshold; the bottleneck convs at 64 frames have 5.8 tiles per SM, the
     // ConvNeXt pwconv1s and stage 1's pwconv2 at 64 frames 2.9 or more.)
-    const int lbn = longk_block_n(op, N, block_n_override);
+    const int lbn = longk_block_n(op, N, block_n_override, num_sms, longk_bn);
     VSB_CHECK(kernel_sel != kKernelLongK || lbn != 0, "the long-K kernel cannot run this op");
     // The fp32 residual-stream epilogue also needs 12 K blocks: below that the tile's 8 bytes of stream traffic per output outlast
     // its main loop, and the 128-row kernel, which overlaps the two, is faster (videoseal_1.0 stage 0's pwconv2, K = 384: 188
@@ -576,6 +584,7 @@ inline void launch(const ConvGemmOp& op, cudaStream_t st) {
     const int bn = op.p.block_n;
     if (op.p.resid32 != nullptr) { if (bn == 128) launch_longk<128, ACT_NONE, true>(op, st); else launch_longk<96, ACT_NONE, true>(op, st); }
     else if (a == ACT_GELU) launch_longk<128, ACT_GELU>(op, st);
+    else if (bn == kLongWideN) { if (a == ACT_RELU) launch_longk<kLongWideN, ACT_RELU>(op, st); else launch_longk<kLongWideN, ACT_NONE>(op, st); }
     else if (bn == 128) { if (a == ACT_RELU) launch_longk<128, ACT_RELU>(op, st); else launch_longk<128, ACT_NONE>(op, st); }
     else { if (a == ACT_RELU) launch_longk<80, ACT_RELU>(op, st); else launch_longk<80, ACT_NONE>(op, st); }
     VSB_CUDA(cudaGetLastError());

@@ -375,7 +375,8 @@ int vsb_debug_conv(const vsb_conv_test* t, void* stream) {
   if (t->rows_per_sample) p.rows_per_sample = t->rows_per_sample;
   if (t->w_samples > 1) op.w_samples = t->w_samples;
   VSB_CHECK(t->kernel >= kKernelAuto && t->kernel <= kKernelLongK, "bad kernel selector");
-  finalize_op(op, (const __half*)t->weights, t->N, K, t->ldw ? t->ldw : K, num_sms, t->block_n, t->kernel);
+  VSB_CHECK(t->longk_block_n == 0 || t->longk_block_n == 128 || t->longk_block_n == kLongWideN, "bad long-K block_n");
+  finalize_op(op, (const __half*)t->weights, t->N, K, t->ldw ? t->ldw : K, num_sms, t->block_n, t->kernel, t->longk_block_n);
   if (t->kernel_ran) *t->kernel_ran = op.longk ? kKernelLongK : kKernel128;
   launch(op, (cudaStream_t)stream);
   g_launches += 1;
